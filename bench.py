@@ -41,8 +41,8 @@ def peaks():
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get('hbm_gbs', 6650.0), 'measured'
-    return 6650.0, 'fallback'
+        return d.get('hbm_gbs', 3350.0), 'measured'
+    return 3350.0, 'H100 SXM data sheet'
 
 
 class ClockSampler:
@@ -237,15 +237,8 @@ def run_ours(args):
     import torch.distributed as dist
     from serl_b200 import rollout, _native, engine
     from serl_b200 import refsig
-    if not os.path.exists(_native.LIB_PATH):      # normally prebuilt in-tree; build the CUDA extension if it is not there
-        if int(os.environ.get('LOCAL_RANK', '0')) == 0:
-            from serl_b200 import build as _b
-            _b.build()
-        else:
-            for _ in range(600):
-                if os.path.exists(_native.LIB_PATH):
-                    break
-                time.sleep(0.5)
+    if not os.path.exists(_native.LIB_PATH):      # the benchmark never writes into the tree: build first
+        raise SystemExit('bench.py: %s is missing; run `python -m serl_b200.build` first' % _native.LIB_PATH)
 
     world = int(os.environ.get('WORLD_SIZE', '1'))
     rank = int(os.environ.get('RANK', '0'))
@@ -264,7 +257,7 @@ def run_ours(args):
     st_host = torch.from_numpy(st_np).pin_memory()
     nominal = torch.full((N_ENVS,), rollout.mode_code('nominal'), dtype=torch.int32)
     mixed = torch.tensor([rollout.mode_code(m) for m in mixed_modes(N_ENVS)], dtype=torch.int32)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)      # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)      # > 50 MB L2 of an H100
 
     def sync_all():
         if world > 1:
@@ -314,6 +307,8 @@ def run_ours(args):
     clocks = sampler.stop() if sampler else None
     launches = (_native.lib().serl_launch_count() - launches0) // (args.steps + args.warmup) * args.steps
     res = m['res']
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res)
 
     # ---- end to end through the public API with host buffers (H2D genomes + env params, D2H fitness) every step
     pop_local = wl['w'].shape[0]
@@ -433,12 +428,6 @@ def run_ours(args):
 
     if rank == 0:
         peak, how = peaks()
-        traffic = None
-        for name in ('r02_rollout_traffic.json', 'r01_rollout_traffic.json'):
-            tpath = os.path.join(ROOT, 'profiles', name)
-            if os.path.exists(tpath):
-                traffic = json.load(open(tpath)).get('dram_bytes_per_launch')
-                break
         per_gpu_steps = m['total_steps'] / world
         kern_ms = m['kern_ms']
         achieved = BYTES_PER_STEP * per_gpu_steps / (kern_ms * 1e-3) / 1e9
@@ -460,7 +449,7 @@ def run_ours(args):
             'other_scaling_mode': other,
             'generation_ms': gen_ms, 'epoch_breakdown': (epoch_timing if gen_ms is not None else None), 'agent_train': agent_line,
             'smoothness': smooth_timing, 'other_workloads': extras,
-            'roofline': {'bound': 'hbm', 'achieved': achieved, 'peak': peak, 'unit': 'GB/s', 'frac': achieved / peak, 'traffic': traffic,
+            'roofline': {'bound': 'hbm', 'achieved': achieved, 'peak': peak, 'unit': 'GB/s', 'frac': achieved / peak,
                          'peak_source': how, 'kernel': 'rollout_kernel_persist', 'kernel_ms': kern_ms,
                          'note': 'BASELINE metric denominator (208 B/env-step state round-trip model); the kernel keeps state on chip and is '
                                  'bound by fp64/fp32 issue, see fp_issue',
@@ -486,6 +475,14 @@ def run_ours(args):
         dist.destroy_process_group()
 
 
+def dump_outputs(out_dir, res):
+    """what the timed path returned in its last timed step: per-trajectory returns and executed step counts [pop, envs] and
+    the per-actor fitness [pop], as float64 .npy files (pop=512 x 128 envs: 1 MB in all)"""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in (('returns', res.returns), ('steps', res.steps), ('fitness', res.fitness)):
+        np.save(os.path.join(out_dir, name + '.npy'), t.detach().cpu().numpy().astype(np.float64))
+
+
 def main():
     # exactly ONE line on stdout (the JSON): libraries that print there (NCCL's version banner) are sent to stderr
     real_stdout = os.dup(1)
@@ -499,6 +496,8 @@ def main():
     ap.add_argument('--no-cpu', action='store_true', help='skip the cpu_baseline leg')
     ap.add_argument('--no-generation', action='store_true', help='skip the rollout+epoch generation timing and the other-workload legs')
     ap.add_argument('--no-agent', action='store_true', help='skip the Agent.train() timing')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write the last step\'s outputs (returns, steps, fitness) as DIR/<name>.npy')
     ap.add_argument('--scaling', default='weak', choices=['weak', 'strong'],
                     help='weak: BASELINE config 3 per GPU (pop=512/GPU); strong: BASELINE config 4 (ONE pop=512, mixed faults, sharded)')
     args = ap.parse_args()

@@ -111,7 +111,7 @@ int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shap
  *                by `shape` (K1, warp-GEMV on CUDA cores).  n_widths == 2: the two-hidden-layer generalisation
  *                Linear(7,w1) act Linear(w1,w2) LayerNorm act Linear(w2,3) tanh (BASELINE config 5: [400,300], [128,128]);
  *                genome = parameters() order, serl_actor_num_params_wide floats per actor; only shape.activation is read
- *                from `shape`; layer 2 runs on the tensor cores (tcgen05, 3xTF32) with TMA-streamed weight slabs
+ *                from `shape`; layer 2 runs on the tensor cores (wgmma, 3xTF32) with TMA-streamed weight slabs
  *   d_sensor_noise optional [pop, n_envs, horizon + 1, 7] fp32 standard-normal draws: the sensor-noise shim of
  *                envs/noise/citation.py:72-82 (mode 'noise'; also the outputs of envs/gust) applied to every native step
  *                output — row 0 for reset()'s step, row k + 1 for env step k; order p,q,r, alpha, beta, phi, theta

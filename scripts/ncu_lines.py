@@ -6,7 +6,7 @@ steps = float(sys.argv[3]) if len(sys.argv) > 3 else 7577600.0
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 tmp = tempfile.mkdtemp()
 subprocess.run(['cuobjdump', '-xelf', 'all', os.path.join(ROOT, 'serl_b200', 'libserl_b200.so')], cwd=tmp, capture_output=True)
-sass = subprocess.run(['nvdisasm', '-c', '-g', os.path.join(tmp, 'rollout.sm_100a.cubin')], capture_output=True, text=True).stdout.split('\n')
+sass = subprocess.run(['nvdisasm', '-c', '-g', os.path.join(tmp, 'rollout.sm_90a.cubin')], capture_output=True, text=True).stdout.split('\n')
 start = [i for i, l in enumerate(sass) if l.startswith('.text.') and kern in l][0]
 end = next((i for i in range(start + 1, len(sass)) if sass[i].startswith('//--------------------- .text.')), len(sass))
 cur, ins = None, []

@@ -12,7 +12,7 @@ want = ['Kernel Name', 'gpu__time_duration.sum', 'launch__grid_size', 'launch__b
         'sm__inst_executed_pipe_fp64.avg.pct_of_peak_sustained_active', 'sm__inst_executed_pipe_fma.avg.pct_of_peak_sustained_active',
         'sm__inst_executed_pipe_lsu.avg.pct_of_peak_sustained_active', 'sm__inst_executed_pipe_alu.avg.pct_of_peak_sustained_active',
         'sm__inst_executed_pipe_tc.avg.pct_of_peak_sustained_active', 'sm__pipe_tensor_cycles_active.avg.pct_of_peak_sustained_active',
-        'sm__inst_executed_pipe_tmem.avg.pct_of_peak_sustained_active', 'sm__inst_executed_pipe_tma.avg.pct_of_peak_sustained_active',
+        'sm__inst_executed_pipe_tma.avg.pct_of_peak_sustained_active',
         'l1tex__t_sector_pipe_lsu_mem_local_op_ld_hit_rate.pct', 'l1tex__t_sector_pipe_lsu_mem_local_op_st_hit_rate.pct',
         'l1tex__t_sector_pipe_lsu_mem_global_op_ld_hit_rate.pct', 'lts__t_sector_hit_rate.pct',
         'l1tex__data_pipe_lsu_wavefronts_mem_shared.sum.pct_of_peak_sustained_elapsed']

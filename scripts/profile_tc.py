@@ -4,7 +4,7 @@ from serl_b200 import rollout, refsig
 from oracle import actor as A
 dev = torch.device('cuda:0')
 widths = [int(x) for x in sys.argv[1].split(',')] if len(sys.argv) > 1 else [400, 300]
-pop, n_envs, horizon = 148, 256, int(sys.argv[2]) if len(sys.argv) > 2 else 60
+pop, n_envs, horizon = 132, 256, int(sys.argv[2]) if len(sys.argv) > 2 else 60
 torch.manual_seed(7)
 g = np.stack([A.flatten(A.WideActor(widths)) for _ in range(4)])
 w = torch.from_numpy(np.tile(g, (pop // 4, 1)).astype(np.float32)).to(dev)

@@ -1,7 +1,7 @@
-"""Compile the CUDA extension (C-ABI shared library) for sm_100a, in-tree.
+"""Compile the CUDA extension (C-ABI shared library) for sm_90a (H100), in-tree.
 
     python -m serl_b200.build          -> serl_b200/libserl_b200.so
-nvcc cross-compiles without a GPU; the .so travels to the GPU box with the repo snapshot.
+nvcc cross-compiles without a GPU.
 """
 import os
 import subprocess
@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libserl_b200.so')
 SOURCES = ['common.cu', 'rollout.cu', 'rollout_tc.cu', 'evo.cu', 'evo_plan.cpp']
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '-Xptxas', '-v']
 
 

@@ -1,4 +1,4 @@
-// K2-K5 — neuro-evolution kernels over the flat [pop, P] fp32 genome matrix (sm_100a).
+// K2-K5 — neuro-evolution kernels over the flat [pop, P] fp32 genome matrix (sm_90a).
 //
 //   K2 ssne_select_kernel    rank by fitness + 3-way tournaments        base/core/mod_neuro_evo.py:460-461, :40-47
 //   K3 ssne_clone_kernel     genome row copies (elitism)                 :371-376, :489-493

@@ -1,4 +1,4 @@
-// Device code shared by the rollout kernels (rollout.cu: K1 warp-GEMV actor; rollout_tc.cu: tcgen05 actor for wide
+// Device code shared by the rollout kernels (rollout.cu: K1 warp-GEMV actor; rollout_tc.cu: wgmma actor for wide
 // two-hidden-layer policies): the generated PH-LAB plant, the ode5 step, CitationEnv (reset / step / reward / termination,
 // envs/phlabenv.py:401-482), the launch argument block, and the mbarrier / TMA primitives.  Every translation unit that
 // includes this file gets its own copy of the (static) tables and __noinline__ plant functions.
@@ -278,45 +278,13 @@ static __device__ __noinline__ void plant_step_nav(double* Xnav, const double* X
 }
 
 // Stage loop fully unrolled (h*B folds to constants).  The right-hand side is ONE __noinline__ function (the same code for
-// every plant variant), so the compact state x[14] and the stage derivative it writes are in local memory; the six stage
-// derivatives are kept in tensor memory (TMF, below) or, in traced launches, in local memory.  The integrator state and the
+// every plant variant), so the compact state x[14], the stage derivative it writes and the six stage derivatives are in
+// local memory (672 bytes per thread, cached in L1 / L2).  The integrator state and the
 // stage combinations are double in every build; `real` (the type of the right-hand side) is double unless PLANT_F32.
 // pv_post / call: time-triggered builds (cg_timed): the parameter row switches to pv_post when the model clock
 // call * 0.01 + c_s * 0.01 of a stage reaches 20 s: every stage from call SERL_TRIGGER_CALLS on, and the LAST stage (c = 1) of
 // call SERL_TRIGGER_CALLS - 1, whose time 19.99 + 0.01 already compares >= 20 in the binary.
-// ---- tensor memory as per-thread scratch ---------------------------------------------------------------------
-// K1 has no use for the tensor cores, so the SM's 256 KB of tensor memory would sit idle — while the six ode5 stage
-// derivatives (6 x 14 doubles per thread, 172 KB per CTA) lived in per-thread LOCAL memory, missed L1 (60 KB next to
-// 187 KB of shared memory) and made an L2 round trip at every stage combination (long_scoreboard 15 % of the warp samples,
-// 12 GB of DRAM write-back per launch).  tcgen05.st / tcgen05.ld with the 32x32b shape give every thread of a warp its
-// own TMEM lane and consecutive 32-bit columns: a private, on-chip array with a 12-cycle load.  A warp owns the lanes of
-// its quadrant (warp % 4) and 192 columns (6 stages x 32; warps w and w+4 share a quadrant and take columns 0.. / 192..).
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32])
-{
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-                 "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-                 :: "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-                    "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]),
-                    "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]),
-                    "r"(r[30]), "r"(r[31]) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32])
-{
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-                 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-                   "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-                   "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-                   "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                 : "r"(taddr) : "memory");
-}
-#define PLANT_TMEM_COLS_PER_WARP 192       // 6 stages x 32 columns (28 used: 14 doubles)
-
 // STAB: tables + parameter rows staged at the start of dynamic shared memory (see plant_rhs_common_smem).
-// TMF: stage derivatives in tensor memory at `taddr` (this warp's lanes + column base) instead of local memory.  The
-// tcgen05 transfers are warp-collective: with TMF EVERY lane of the warp must make the call; lanes whose trajectory is
-// over pass active = false and keep their state.  (Builds with a float right-hand side and traced episodes, which hand
-// all six stages to the navigation integrator, use the local-memory form.)
 // GUST instantiation (launches with a `gust` env, SERL_MODE_GUST): bit 30 of `call` marks a gust env, and u[3], the
 // right-hand side's angle-of-attack offset, is atan(w_gust / V) for the stages whose time lies in the pulse 20 s <= t <= 23 s
 // (include/serl_b200.h).  Without GUST the offset is the constant 0 and the code is that of a build without the feature.
@@ -329,9 +297,9 @@ __device__ __forceinline__ real plant_gust_offset(int call, int s, real V)
     if (!on) return (real)0;
     return (real)(atan(PLANT_DIV((double)SERL_GUST_W, (double)V)) * 1.0);
 }
-template <bool STAB = false, bool TMF = false, bool GUST = false>
+template <bool STAB = false, bool GUST = false>
 static __device__ __noinline__ void plant_step(const real* pv, double* X, const double* U, const real* tab, bool nav = false,
-                                               const real* pv_post = nullptr, int call = 0, uint32_t taddr = 0, bool active = true)
+                                               const real* pv_post = nullptr, int call = 0)
 {
     const bool gust = GUST && (call & PLANT_CALL_GUST) != 0, gust_up = GUST && (call & PLANT_CALL_GUST_UP) != 0;
     if (GUST) call &= ~(PLANT_CALL_GUST | PLANT_CALL_GUST_UP);
@@ -343,50 +311,7 @@ static __device__ __noinline__ void plant_step(const real* pv, double* X, const 
 #pragma unroll
     for (int li = 0; li < NLIVE; ++li) x[li] = (real)X[LIVE[li]];
     double xl[NLIVE];
-    if (TMF && sizeof(real) == 8) {
-        real fc[NLIVE];                 // the stage just evaluated (local memory, L1-hot); older stages come from TMEM
-#pragma unroll
-        for (int s = 0; s < 6; ++s) {
-            const bool post = pv_post != nullptr && (call >= SERL_TRIGGER_CALLS || (s == 5 && call == SERL_TRIGGER_CALLS - 1));
-            if (GUST) { u[3] = gust ? plant_gust_offset(call, s, x[3]) : (real)0; if (gust_up) u[3] = -u[3]; }
-            if (STAB) plant_rhs_common_smem(x, u, fc, tab, post ? pv_post : pv);
-            else plant_rhs_common(x, u, fc, tab, post ? pv_post : pv);
-            double acc[NLIVE];
-            __syncwarp();
-            if (s > 0) {
-#pragma unroll
-                for (int j = 0; j < s; ++j) {
-                    uint32_t r[32];
-                    tmem_ld32(taddr + 32 * j, r);
-                    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-                    for (int li = 0; li < NLIVE; ++li) {
-                        const double fj = __hiloint2double((int)r[2 * li + 1], (int)r[2 * li]);
-                        if (j == 0) acc[li] = fj * (h * B[s][0]);
-                        else acc[li] += fj * (h * B[s][j]);
-                    }
-                }
-            }
-#pragma unroll
-            for (int li = 0; li < NLIVE; ++li) {
-                if (s == 0) acc[li] = (double)fc[li] * (h * B[0][0]);
-                else acc[li] += (double)fc[li] * (h * B[s][s]);
-                xl[li] = X[LIVE[li]] + acc[li];
-                x[li] = (real)xl[li];
-            }
-            if (s < 5) {
-                uint32_t r[32];
-#pragma unroll
-                for (int li = 0; li < NLIVE; ++li) {
-                    r[2 * li] = (uint32_t)__double2loint((double)fc[li]);
-                    r[2 * li + 1] = (uint32_t)__double2hiint((double)fc[li]);
-                }
-                r[28] = r[29] = r[30] = r[31] = 0u;
-                tmem_st32(taddr + 32 * s, r);
-                asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-            }
-        }
-    } else {
+    {
         real f[6][NLIVE];
 #pragma unroll
         for (int s = 0; s < 6; ++s) {
@@ -409,10 +334,8 @@ static __device__ __noinline__ void plant_step(const real* pv, double* X, const 
             X[8] = xn[0]; X[10] = xn[1]; X[11] = xn[2];
         }
     }
-    if (active) {
 #pragma unroll
-        for (int li = 0; li < NLIVE; ++li) X[LIVE[li]] = xl[li];
-    }
+    for (int li = 0; li < NLIVE; ++li) X[LIVE[li]] = xl[li];
 }
 
 // activations: IEEE-only sequences of actor_math.cuh (bit-reproducible on a CPU; see oracle/plant/actor_kernel_order.c)
@@ -546,18 +469,15 @@ static __device__ void env_reset(Env& e, const RolloutArgs& a, int env, float* o
 }
 
 // one CitationEnv.step (phlabenv.py:430-482) + the bookkeeping of Agent.evaluate (agent.py:85-118)
-// TMF (stage derivatives in tensor memory, see plant_step): the whole warp makes the call; lanes with active = false go
-// through the plant's collective transfers and change nothing.
-template <bool STAB = false, bool TMF = false, bool GUST = false>
-static __device__ void env_step(Env& e, const RolloutArgs& ar, size_t traj, int actor, bool replay, const float* a, float* obs,
-                                bool active = true, uint32_t taddr = 0)
+template <bool STAB = false, bool GUST = false>
+static __device__ void env_step(Env& e, const RolloutArgs& ar, size_t traj, int actor, bool replay, const float* a, float* obs)
 {
     const double bound = 10.0 * DEG2RAD;                       // phlabenv.py:208
     const double max_theta = 60.0 * DEG2RAD, max_phi = 75.0 * DEG2RAD;
     const double k_err = 6.0 / 3.141592653589793;              // phlabenv.py:226-231
     const double k_err4 = k_err * 4.0;
     double U[3], cmd[3], act_d[3];
-    if (ar.action_noise && active) {
+    if (ar.action_noise) {
         // action = clip(action + clipped_noise, -1, 1) in float64, then scale_action in float64 (agent.py:90-96)
         const float* nz = ar.action_noise + (traj * ar.horizon + e.k) * 3;
 #pragma unroll
@@ -576,13 +496,12 @@ static __device__ void env_step(Env& e, const RolloutArgs& ar, size_t traj, int 
         }
     }
     // a NaN action would be squashed to a bound by the plant's input saturation (as in the reference binary): report it
-    if (active && ar.status && !isfinite(act_d[0] + act_d[1] + act_d[2])) atomicOr(ar.status, SERL_STATUS_NONFINITE);
+    if (ar.status && !isfinite(act_d[0] + act_d[1] + act_d[2])) atomicOr(ar.status, SERL_STATUS_NONFINITE);
     apply_fault(e.fault, U, cmd);
     double xo[12];
 #pragma unroll
     for (int i = 0; i < 12; ++i) xo[i] = e.X[i];
-    plant_step<STAB, TMF, GUST>(e.pv, e.X, cmd, e.tab, ar.trace != nullptr, e.pv_post, (e.k + 1) | (GUST && (e.gust & 1) ? PLANT_CALL_GUST | ((e.gust & 2) ? PLANT_CALL_GUST_UP : 0) : 0), taddr, active);
-    if (!active) return;
+    plant_step<STAB, GUST>(e.pv, e.X, cmd, e.tab, ar.trace != nullptr, e.pv_post, (e.k + 1) | (GUST && (e.gust & 1) ? PLANT_CALL_GUST | ((e.gust & 2) ? PLANT_CALL_GUST_UP : 0) : 0));
     sensor_noise(ar, traj, e.k + 1, xo);
 
     const double t = e.t;

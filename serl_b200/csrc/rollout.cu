@@ -1,4 +1,4 @@
-// K1 — fused population rollout for sm_100a (+ K6 smoothness metric, batched plant step).
+// K1 — fused population rollout for sm_90a (+ K6 smoothness metric, batched plant step).
 //
 // One lane = one (actor, env) trajectory; one warp = 32 envs of one actor; one CTA = 1-2 actors x 128 envs with their
 // fp32 genomes (and the plant tables) staged once in shared memory.  Per step a warp runs, entirely on chip:
@@ -12,10 +12,10 @@
 //
 // Two actor implementations:
 //   rollout_kernel_persist<H, TABS, GUST>  persistent grid, one CTA per SM.  The MLP is a register-tiled GEMM inside a warp
-//                           (lane = 1/4 of the output neurons x 4 envs, packed FFMA2, activations exchanged with warp
+//                           (lane = 1/4 of the output neurons x 4 envs, float2 pairs, activations exchanged with warp
 //                           shuffles, weights broadcast from shared memory; h in {32,64,72,96,128}).  The CTA's warps take
 //                           their steps in lockstep (one barrier per step: shared instruction fetch), genomes arrive by bulk
-//                           TMA copies, the ode5 stage derivatives live in tensor memory.
+//                           TMA copies.
 //   rollout_kernel_simple   every thread runs the whole MLP for its env (any h that fits); cross-check / fallback shape.
 #include "plant_env.cuh"
 
@@ -89,7 +89,7 @@ __device__ void actor_forward_simple(const float* __restrict__ w, const serl_act
 // The activation of neuron k for env 4g+c lives in lane (g, og = k/TM), register in[k%TM][c]; the next layer
 // fetches it with one shuffle per (k, c).  Reductions over neurons are xor-butterflies over the two og bits, so
 // the four lanes of a group hold bit-identical means / deviations.
-// All MLP arithmetic uses the packed FP32 FMA of sm_100 (FFMA2: two IEEE-rn fmas per issued instruction); a float2
+// All MLP arithmetic is written on float2 pairs (am_fma2: two independent IEEE-rn fmas); a float2
 // register pair holds two consecutive output neurons (m, m+1) of one env, exactly what one LDS.64 of the transposed
 // weight row delivers, and the activation of the source neuron is broadcast into both halves.
 template <int H>
@@ -121,10 +121,10 @@ __device__ __forceinline__ void warp_layer(const float* __restrict__ Wt, const f
 #pragma unroll
             for (int m2 = 0; m2 < TM2; ++m2) {
                 const float2 w2 = wp[m2];
-                acc[m2][0] = __ffma2_rn(w2, b0, acc[m2][0]);
-                acc[m2][1] = __ffma2_rn(w2, b1, acc[m2][1]);
-                acc[m2][2] = __ffma2_rn(w2, b2, acc[m2][2]);
-                acc[m2][3] = __ffma2_rn(w2, b3, acc[m2][3]);
+                acc[m2][0] = am_fma2(w2, b0, acc[m2][0]);
+                acc[m2][1] = am_fma2(w2, b1, acc[m2][1]);
+                acc[m2][2] = am_fma2(w2, b2, acc[m2][2]);
+                acc[m2][3] = am_fma2(w2, b3, acc[m2][3]);
             }
         }
     }
@@ -165,8 +165,8 @@ __device__ __noinline__ void actor_forward_warp(const float* __restrict__ w, int
 #pragma unroll
         for (int m2 = 0; m2 < TM2; ++m2) {
             const float2 w2 = wp[m2];
-            acc[m2][0] = __ffma2_rn(w2, b0v, acc[m2][0]); acc[m2][1] = __ffma2_rn(w2, b1v, acc[m2][1]);
-            acc[m2][2] = __ffma2_rn(w2, b2v, acc[m2][2]); acc[m2][3] = __ffma2_rn(w2, b3v, acc[m2][3]);
+            acc[m2][0] = am_fma2(w2, b0v, acc[m2][0]); acc[m2][1] = am_fma2(w2, b1v, acc[m2][1]);
+            acc[m2][2] = am_fma2(w2, b2v, acc[m2][2]); acc[m2][3] = am_fma2(w2, b3v, acc[m2][3]);
         }
     }
 #pragma unroll
@@ -276,7 +276,7 @@ __global__ void genome_layout_kernel(const float* __restrict__ w, float* __restr
 // one task, some whole tasks, and the head of another.  A slot flies the head segment FIRST and publishes the
 // trajectories' state in HBM (Handoff), then its whole tasks, and LAST the tail segment, whose first part the previous
 // slot published long before: no slot ever waits in practice, and all SMs finish together (512 actors x 128 envs on
-// 148 SMs x 2 slots = 1.73 tasks per slot: two full rounds without the split).  When there are fewer tasks than
+// 132 SMs x 2 slots = 1.94 tasks per slot: two full rounds without the split).  When there are fewer tasks than
 // slots every task is flown whole by one slot.  The genome of a slot is swapped by ONE elected thread with a bulk TMA copy;
 // the slot's warps meet at its named barrier for that and for the slot-uniform decisions of the lockstep loop (see there).
 // TABS: plant tables staged in shared memory (true) or read from global memory through L1 (false: h = 128, whose
@@ -289,7 +289,6 @@ rollout_kernel_persist(RolloutArgs ar)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];     // same alignment as plant_smem_tab (plant_env.cuh)
     __shared__ uint64_t gbar[4];                       // one mbarrier per genome slot
-    __shared__ uint32_t tmem_slot;                     // base address of the CTA's tensor memory (stage derivatives)
     if (TABS) plant_tab_check(smem_raw);
     real* tab_s = reinterpret_cast<real*>(smem_raw);
     constexpr int TABN = PT_TOTAL + SERL_PLANT_COUNT * PLANT_NPV;      // tables + per-variant parameter rows
@@ -310,18 +309,7 @@ rollout_kernel_persist(RolloutArgs ar)
         for (int i = 0; i < ar.apc; ++i) mbar_init(&gbar[i], 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    // Tensor memory for the ode5 stage derivatives (plant_env.cuh): the whole 512 columns, allocated by warp 0.  Traced
-    // launches (single episodes; the navigation integrator wants all six stages) and the float build keep local memory.
-    const bool use_tmem = sizeof(real) == 8 && ar.trace == nullptr;
-    if (use_tmem && warp == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "r"(512) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = use_tmem ? *reinterpret_cast<volatile uint32_t*>(&tmem_slot) : 0u;
-    const uint32_t taddr = tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + (uint32_t)((warp >> 2) * PLANT_TMEM_COLS_PER_WARP);
     float* w = wbase + (size_t)slot_l * ar.P4;
     const int slot_threads = wps * 32;
     const int actfn = ar.sh.activation;
@@ -474,16 +462,8 @@ rollout_kernel_persist(RolloutArgs ar)
             if (actfn == SERL_ACT_TANH) actor_forward_warp<H, SERL_ACT_TANH>(w, L, lane, obs, a);
             else if (actfn == SERL_ACT_ELU) actor_forward_warp<H, SERL_ACT_ELU>(w, L, lane, obs, a);
             else actor_forward_warp<H, SERL_ACT_LEAKY_RELU>(w, L, lane, obs, a);
-            // with the stage derivatives in tensor memory the plant's transfers are warp-collective: every lane steps,
-            // lanes whose trajectory is over change nothing
-            if (use_tmem) env_step<TABS, true, GUST>(e, ar, traj, actor, replay, a, obs, mine, taddr);
-            else if (mine) env_step<TABS, false, GUST>(e, ar, traj, actor, replay, a, obs);
+            if (mine) env_step<TABS, GUST>(e, ar, traj, actor, replay, a, obs);
         }
-    }
-    if (use_tmem) {                                    // every warp has left the loop (it ends at a CTA barrier)
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncthreads();
-        if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512) : "memory");
     }
 }
 
@@ -512,7 +492,7 @@ rollout_kernel_simple(RolloutArgs ar)
     const bool replay = ar.replay != nullptr && env == ar.replay_env;
     while (!e.done) {
         actor_forward_simple(w, ar.sh, bufA, bufB, tid, 128, obs, a);
-        env_step<false, false, true>(e, ar, traj, actor, replay, a, obs);       // (the gust schedule costs nothing that matters here)
+        env_step<false, true>(e, ar, traj, actor, replay, a, obs);       // (the gust schedule costs nothing that matters here)
     }
     ar.returns[traj] = e.ret;
     ar.steps[traj] = e.k;
@@ -581,7 +561,7 @@ __global__ void plant_step_kernel(double* __restrict__ X, const double* __restri
     for (int k = 0; k < NX; ++k) x[k] = X[(size_t)i * NX + k];
     u[0] = cmd[3 * i]; u[1] = cmd[3 * i + 1]; u[2] = cmd[3 * i + 2];
     const int post = (variant[i] >> 16) & 0xff;
-    plant_step<false, false, true>(plant_pv[variant[i] & 0xff], x, u, plant_tables_blob, false, post ? plant_pv[post] : nullptr,
+    plant_step<false, true>(plant_pv[variant[i] & 0xff], x, u, plant_tables_blob, false, post ? plant_pv[post] : nullptr,
                                    (call ? call[i] : 0) | ((variant[i] & SERL_MODE_GUST) ? PLANT_CALL_GUST : 0) |
                                        ((variant[i] & SERL_MODE_GUST_UP) ? PLANT_CALL_GUST_UP : 0));
 #pragma unroll
@@ -963,7 +943,7 @@ static int device_sms()
     if (num_sms == 0) {
         int dev = 0;
         cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 148;
+        if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 132;
     }
     return num_sms;
 }

@@ -1,46 +1,41 @@
 // K1-TC — population rollout for WIDE two-hidden-layer actors (BASELINE config 5: hidden = [400,300] / [128,128]) on the
-// 5th-generation tensor cores of sm_100a.
+// tensor cores of sm_90a (warpgroup MMA, wgmma).
 //
 //   actor  Linear(7,w1) -> act -> Linear(w1,w2) -> LayerNorm(w2) -> act -> Linear(w2,3) -> tanh
 //          (the two-hidden-layer generalisation of base/core/genetic_agent.py:78-101; LayerNorm base/core/mod_utils.py:47-50)
 //
-// One CTA per SM = 256 threads = two GROUPS of 128 threads; a group = 128 envs of one actor (thread = env = row of the layer
-// GEMM = TMEM lane).  The two groups run independent task loops, share the plant tables in shared memory, the weight ring,
-// the TMEM accumulator and the tensor core, and take turns on them (a shared-memory lock): while one group streams its W1
-// slabs through the tensor core the other integrates its plant step.  Per step of a group:
-//   layer 1   on CUDA cores, 8 neurons at a time: every thread computes its env's activations and writes them, split
-//             into TF32 hi + lo parts, as one K-slab of the A operand in shared memory (UMMA canonical K-major layout,
+// One CTA per SM = 256 threads = two GROUPS of 128 threads (one warpgroup each); a group = 128 envs of one actor
+// (thread = env).  The two groups run independent task loops, share the plant tables in shared memory and the A / W1 rings,
+// and take turns on the rings (a shared-memory lock): while one group streams its W1 slabs through the tensor cores the
+// other integrates its plant step.  Per step of a group, for each half of 64 envs (the M of one wgmma):
+//   layer 1   on CUDA cores, 8 neurons at a time (two threads per env, 4 neurons each): the activations, split into
+//             TF32 hi + lo parts, are written as one K-slab of the A operand in shared memory (canonical K-major layout,
 //             no swizzle);
-//   layer 2   D[128 x w2] += A[128 x 8] . W1^T[8 x w2]  by tcgen05.mma (kind::tf32, M = 128, N <= 256 per instruction,
-//             fp32 accumulator in TENSOR MEMORY), three products per slab (hi.hi + hi.lo + lo.hi = "3xTF32", fp32-level
-//             accuracy); the W1 K-slabs (pre-split and pre-tiled once per launch) are STREAMED from L2 into a 3-stage
-//             shared-memory ring by bulk TMA copies (cp.async.bulk + mbarrier complete_tx) — a [400,300] genome is 500 KB
-//             and never fits on chip; tcgen05.commit hands each ring slot back when its MMAs have read it;
-//   epilogue  tcgen05.ld brings the thread's accumulator row out of TMEM 16 columns at a time: bias, LayerNorm (the whole
-//             row lives in one thread: no shuffles), activation, and the 3-row output layer folded into the same pass;
+//   layer 2   D[64 x w2] += A[64 x 8] . W1^T[8 x w2]  by wgmma.mma_async m64n64k8 .tf32 (fp32 accumulator in registers,
+//             n2pad / 2 per thread), three products per slab (hi.hi + hi.lo + lo.hi = "3xTF32", fp32-level accuracy); the
+//             W1 K-slabs (pre-split and pre-tiled once per launch) are STREAMED from L2 into a 4-stage shared-memory ring by
+//             bulk TMA copies (cp.async.bulk + mbarrier complete_tx), two stages ahead — a [400,300] genome is 500 KB and
+//             never fits on chip; wgmma.wait_group tells when a ring slot's MMAs have read it;
+//   epilogue  from the accumulator fragment (a row lives in the 4 lanes of a quad): bias, LayerNorm (quad shuffles for the
+//             row sums), activation, and the 3-row output layer folded into the same pass;
 //   plant     CitationEnv.step + the ode5 plant step on CUDA cores (plant_env.cuh), exactly as in K1.
-// (Round-2 history: the first version ran two 128-thread CTAs per SM with the plant tables read through L1; at [400,300]
-// the two weight rings left ~50 KB of L1 and the plant's table / local-memory traffic thrashed it — 26 % long-scoreboard
-// stalls, 1.1e8 env-steps/s.  Sharing one ring, one accumulator and shared-memory tables between two groups fixed that.)
 //
 // Numerics: tensor-core accumulation order is not reproducible on a CPU, so this path is checked against the torch fp32
 // oracle with a tolerance (tests/test_wide_actor_gpu.py), not bit for bit like K1.
 #include "plant_env.cuh"
 
-#define TC_THREADS 128
-#ifndef TC_STAGES
-#define TC_STAGES 3
-#endif
-#ifndef TC_KSLAB
-#define TC_KSLAB 8                 // K values per pipeline stage (a multiple of 8 = the tcgen05.mma K step for TF32)
-#endif
+#define TC_THREADS 128             // a group: one warpgroup
+#define TC_M 64                    // rows (envs) of one wgmma
+#define TC_STAGES 4
+#define TC_KSLAB 8                 // K values per pipeline stage (the wgmma K step for TF32)
 #define TC_CH (TC_KSLAB / 4)        // 16-byte K chunks (4 TF32 values) per stage
+#define TC_NCH 64                  // accumulator columns per wgmma
+#define TC_MAXN 320                // largest padded w2
 
 struct TcArgs {
     RolloutArgs r;                 // env / output part (weights, wt, P4, apc ... unused)
-    int w1, w2, n2pad;             // layer widths (w1 already padded to a multiple of TC_KSLAB with zero neurons); w2 padded to 16
+    int w1, w2, n2pad;             // layer widths (w1 already padded to a multiple of TC_KSLAB with zero neurons); w2 padded to TC_NCH
     int w1_real;
-    int tmem_cols;                 // TMEM columns to allocate (power of two >= 32)
     int small_floats;              // per-actor small parameter block (floats, multiple of 4)
     int stage_floats;              // per-stage W1 slab: hi[2][n2pad][4] + lo[2][n2pad][4]
     const float* small;            // [pop][small_floats]
@@ -101,56 +96,39 @@ __global__ void tc_layout_kernel(const float* __restrict__ w, int pop, int P, in
     }
 }
 
-// ---- tcgen05 primitives ---------------------------------------------------------------------------------------
+// ---- wgmma primitives -----------------------------------------------------------------------------------------
 // shared-memory matrix descriptor, K-major, no swizzle: core matrix = 8 rows x 16 bytes (contiguous 128 B);
 // SBO = byte distance between 8-row groups, LBO = byte distance between the two 16-byte K chunks of one MMA K step
-__device__ __forceinline__ uint64_t umma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes)
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes)
 {
-    return (uint64_t)((smem_addr & 0x3ffffu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-           (1ull << 46);          // descriptor version 1 (sm_100), layout type 0 = no swizzle
+    return (uint64_t)((smem_addr & 0x3ffffu) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32);
 }
-// instruction descriptor: D = F32, A = B = TF32, both K-major, M = 128, N = n
-__device__ __forceinline__ uint32_t umma_idesc_tf32(int n)
-{
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate)
+// D[64 x 64] (+)= A[64 x 8] . B[64 x 8]^T, TF32 inputs, FP32 accumulator in registers (the m64n64 fragment: lane l of warp w
+// of the warpgroup holds rows 16w + l/4 and 16w + l/4 + 8, columns 8i + 2(l%4) + {0,1}, i = 0..7, as d[4i + {0,1,2,3}])
+__device__ __forceinline__ void wgmma_tf32_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate)
 {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t"
-        "}\n" ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate), "r"(0u) : "memory");
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint64_t* bar)
-{
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v)
-{
-    uint32_t r[16];
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-                 : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-                   "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-                 : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 struct TcCtx {
     const float* small;            // smem: small parameter block of the current actor
-    float* a_ring;                 // smem: TC_STAGES x { hi[2][128][4], lo[2][128][4] }
+    float* io;                     // smem: the group's observations [128][8] and actions [128][4]
+    float* a_ring;                 // smem: TC_STAGES x { hi[2][64][4], lo[2][64][4] }
     float* b_ring;                 // smem: TC_STAGES x stage_floats
     uint64_t* full_b;              // [TC_STAGES] TMA landed
-    uint64_t* free_s;              // [TC_STAGES] MMAs of the slot retired
-    uint64_t* acc_bar;             // accumulator complete
-    uint32_t* tmem_slot;           // smem word tcgen05.alloc writes
     uint32_t g;                    // stages issued so far (valid while the group holds the lock)
-    uint32_t steps;                // accumulators completed so far (same)
-    uint32_t tmem;                 // TMEM base address
-    uint32_t* shared_state;        // smem: {lock, g, steps} shared by the two groups
+    uint32_t* shared_state;        // smem: {lock, g} shared by the two groups
     int grp, gtid;                 // group of this thread (0/1), thread index inside the group
 };
 
@@ -162,7 +140,7 @@ __device__ __forceinline__ bool group_any(int grp, bool pred)
                  : "=r"(r) : "r"((uint32_t)pred), "r"(3 + grp), "r"(TC_THREADS) : "memory");
     return r != 0;
 }
-// the tensor core, its accumulator and the A / W1 rings belong to one group at a time
+// the A / W1 rings and their barriers belong to one group at a time
 __device__ __forceinline__ void tc_acquire(TcCtx& c)
 {
     if (c.gtid == 0) {
@@ -171,179 +149,196 @@ __device__ __forceinline__ void tc_acquire(TcCtx& c)
     }
     group_sync(c.grp);
     c.g = *reinterpret_cast<volatile uint32_t*>(&c.shared_state[1]);
-    c.steps = *reinterpret_cast<volatile uint32_t*>(&c.shared_state[2]);
 }
 __device__ __forceinline__ void tc_release(TcCtx& c)
 {
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    group_sync(c.grp);                       // every warp of the group has read its TMEM lanes
+    group_sync(c.grp);                       // every warp of the group has retired its MMAs
     if (c.gtid == 0) {
         c.shared_state[1] = c.g;
-        c.shared_state[2] = c.steps;
         __threadfence_block();
         atomicExch(&c.shared_state[0], 0u);
     }
 }
 
-// one actor forward for the 128 envs of the CTA; every thread passes its own observation and receives its own action
+// one actor forward for the 128 envs of the group; every thread passes its own observation and receives its own action.
+// The group's rows are done in two halves of TC_M = 64 (the M of one wgmma); each half streams all W1 slabs, so the
+// accumulator of a thread is n2pad / 2 registers.
 template <int ACT>
 __device__ __forceinline__ void tc_actor_forward(TcCtx& c, const TcArgs& ar, const float* tiles_actor, const float* obs, float* action)
 {
-    const int tid = c.gtid, warp = tid >> 5;          // group-local: warp = TMEM lane quadrant of this thread
-    const int w1 = ar.w1, w2 = ar.w2, n2pad = ar.n2pad;
-    const int n_stages = w1 / TC_KSLAB;
+    const int tid = c.gtid, warp = tid >> 5, lane = tid & 31;
+    const int w2 = ar.w2, n2pad = ar.n2pad, nch = n2pad / TC_NCH;
+    const int n_stages = ar.w1 / TC_KSLAB, total = 2 * n_stages;
     const uint32_t stage_bytes = (uint32_t)ar.stage_floats * 4u;
-    constexpr int A_STAGE_FLOATS = 2 * TC_CH * TC_THREADS * 4;             // hi + lo, TC_CH chunks x 128 rows x 4 floats
+    constexpr int A_STAGE_FLOATS = 2 * TC_CH * TC_M * 4;                   // hi + lo, TC_CH chunks x 64 rows x 4 floats
     const float* W0p = c.small;
-    tc_acquire(c);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+    float* obs_s = c.io;
+    float* act_s = c.io + TC_THREADS * 8;
+#pragma unroll
+    for (int k = 0; k < 7; ++k) obs_s[tid * 8 + k] = obs[k];
+    tc_acquire(c);                                                         // (its barrier publishes obs_s)
     const uint32_t g0 = c.g;
-    // W1 slabs of the first stages of this step (their slots were released by the previous step's MMAs)
+    // W1 slabs of the first two stages (their slots' MMAs retired before the lock was released)
     if (tid == 0) {
-        for (int s = 0; s < TC_STAGES - 1 && s < n_stages; ++s) {
-            const uint32_t g = g0 + s, slot = g % TC_STAGES;
-            if (g >= TC_STAGES) mbar_wait(&c.free_s[slot], ((g / TC_STAGES) + 1) & 1);
-            mbar_expect_tx(&c.full_b[slot], stage_bytes);
-            tma_bulk_g2s(c.b_ring + (size_t)slot * ar.stage_floats, tiles_actor + (size_t)s * ar.stage_floats, stage_bytes, &c.full_b[slot]);
+        for (int q = 0; q < 2 && q < total; ++q) {
+            const uint32_t sl = (g0 + q) % TC_STAGES;
+            mbar_expect_tx(&c.full_b[sl], stage_bytes);
+            tma_bulk_g2s(c.b_ring + (size_t)sl * ar.stage_floats, tiles_actor + (size_t)(q % n_stages) * ar.stage_floats, stage_bytes, &c.full_b[sl]);
         }
     }
-    const uint32_t idesc0 = umma_idesc_tf32(n2pad <= 256 ? n2pad : 256);
-    const uint32_t idesc1 = umma_idesc_tf32(n2pad <= 256 ? 16 : n2pad - 256);
-    for (int s = 0; s < n_stages; ++s) {
-        const uint32_t g = g0 + s, slot = g % TC_STAGES;
-        // the slot's previous MMAs must have read A (and B) before it is overwritten
-        if (g >= TC_STAGES) mbar_wait(&c.free_s[slot], ((g / TC_STAGES) + 1) & 1);
-        // layer 1: this env's 8 activations of the slab, split into TF32 hi / lo, as A rows
-        float* a_hi = c.a_ring + (size_t)slot * A_STAGE_FLOATS;
-        float* a_lo = a_hi + TC_CH * TC_THREADS * 4;
-#pragma unroll
-        for (int j = 0; j < TC_CH; ++j) {
-            float h[4];
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                const float4 wa = *reinterpret_cast<const float4*>(W0p + (size_t)(s * TC_KSLAB + j * 4 + kk) * 8);
-                const float4 wb = *reinterpret_cast<const float4*>(W0p + (size_t)(s * TC_KSLAB + j * 4 + kk) * 8 + 4);
-                float acc = wb.w;                                    // bias
-                acc = __fmaf_rn(wa.x, obs[0], acc); acc = __fmaf_rn(wa.y, obs[1], acc); acc = __fmaf_rn(wa.z, obs[2], acc);
-                acc = __fmaf_rn(wa.w, obs[3], acc); acc = __fmaf_rn(wb.x, obs[4], acc); acc = __fmaf_rn(wb.y, obs[5], acc);
-                acc = __fmaf_rn(wb.z, obs[6], acc);
-                h[kk] = acc;
-            }
-            const float2 p0 = am_act2<ACT>(make_float2(h[0], h[1])), p1 = am_act2<ACT>(make_float2(h[2], h[3]));
-            const float4 hi = make_float4(rn_tf32(p0.x), rn_tf32(p0.y), rn_tf32(p1.x), rn_tf32(p1.y));
-            const float4 lo = make_float4(rn_tf32(p0.x - hi.x), rn_tf32(p0.y - hi.y), rn_tf32(p1.x - hi.z), rn_tf32(p1.y - hi.w));
-            *reinterpret_cast<float4*>(a_hi + ((size_t)j * TC_THREADS + tid) * 4) = hi;
-            *reinterpret_cast<float4*>(a_lo + ((size_t)j * TC_THREADS + tid) * 4) = lo;
-        }
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy writes of A -> tensor-core (async proxy) reads
-        group_sync(c.grp);
-        if (tid == 0) {
-            mbar_wait(&c.full_b[slot], (g / TC_STAGES) & 1);               // W1 slab landed
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t a_hi_addr = smem_u32(a_hi), a_lo_addr = smem_u32(a_lo);
-            const uint32_t b_hi_addr = smem_u32(c.b_ring + (size_t)slot * ar.stage_floats);
-            const uint32_t b_lo_addr = b_hi_addr + (uint32_t)TC_CH * (uint32_t)n2pad * 16u;
-            const uint32_t lbo_a = TC_THREADS * 16, lbo_b = (uint32_t)n2pad * 16;
-#pragma unroll
-            for (int ks = 0; ks < TC_KSLAB / 8; ++ks) {                         // one K step = two 16-byte chunks
-                const uint32_t ao = (uint32_t)(2 * ks) * lbo_a, bo2 = (uint32_t)(2 * ks) * lbo_b;
-                const uint64_t dah = umma_desc(a_hi_addr + ao, lbo_a, 128), dal = umma_desc(a_lo_addr + ao, lbo_a, 128);
-                const uint32_t acc0 = (s > 0 || ks > 0) ? 1u : 0u;
-                // N part 0 (columns 0 .. min(n2pad,256))
-                umma_tf32(c.tmem, dah, umma_desc(b_hi_addr + bo2, lbo_b, 128), idesc0, acc0);
-                umma_tf32(c.tmem, dah, umma_desc(b_lo_addr + bo2, lbo_b, 128), idesc0, 1u);
-                umma_tf32(c.tmem, dal, umma_desc(b_hi_addr + bo2, lbo_b, 128), idesc0, 1u);
-                if (n2pad > 256) {                                             // N part 1 (columns 256 .. n2pad)
-                    umma_tf32(c.tmem + 256, dah, umma_desc(b_hi_addr + bo2 + 256 * 16, lbo_b, 128), idesc1, acc0);
-                    umma_tf32(c.tmem + 256, dah, umma_desc(b_lo_addr + bo2 + 256 * 16, lbo_b, 128), idesc1, 1u);
-                    umma_tf32(c.tmem + 256, dal, umma_desc(b_hi_addr + bo2 + 256 * 16, lbo_b, 128), idesc1, 1u);
-                }
-            }
-            umma_commit(&c.free_s[slot]);                                      // slot reusable when these MMAs retire
-            if (s == n_stages - 1) umma_commit(c.acc_bar);
-            // prefetch the slab TC_STAGES-1 ahead into the slot stage g-1 used
-            const int sn = s + TC_STAGES - 1;
-            if (sn < n_stages) {
-                const uint32_t gn = g + TC_STAGES - 1, sl = gn % TC_STAGES;
-                if (gn >= TC_STAGES) mbar_wait(&c.free_s[sl], ((gn / TC_STAGES) + 1) & 1);
-                mbar_expect_tx(&c.full_b[sl], stage_bytes);
-                tma_bulk_g2s(c.b_ring + (size_t)sl * ar.stage_floats, tiles_actor + (size_t)sn * ar.stage_floats, stage_bytes, &c.full_b[sl]);
-            }
-        }
-    }
-    c.g = g0 + n_stages;
-    // ---- epilogue: this thread's accumulator row (TMEM lane = thread) ----
-    mbar_wait(c.acc_bar, c.steps & 1);
-    c.steps += 1;
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const float* b1 = c.small + w1 * 8;
+    const int rr = tid & (TC_M - 1), jj = tid >> 6;                         // layer 1: row rr of the half, K chunk jj of the slab
+    const float* b1 = c.small + ar.w1 * 8;
     const float* gamma = b1 + n2pad;
     const float* beta = gamma + n2pad;
     const float* Wo = beta + n2pad;
     const float* bo = Wo + 3 * n2pad;
-    const uint32_t trow = c.tmem + ((uint32_t)(warp * 32) << 16);
-    const int n_chunks = n2pad / 16;
-    float v[16];
-#ifdef TC_EPI2
-    // mean and variance in ONE pass over the accumulator row, shifted by its first element (no cancellation problem:
-    // |mean - x0| is of the order of the row's own spread)
-    float x0 = 0.f, s1 = 0.f, s2 = 0.f;
-    for (int ch = 0; ch < n_chunks; ++ch) {
-        tmem_ld16(trow + ch * 16, v);
-        if (ch == 0) x0 = __fadd_rn(v[0], b1[0]);
+    float acc[TC_MAXN / 2];
+    for (int h = 0; h < 2; ++h) {
+        float ob[7];
 #pragma unroll
-        for (int i = 0; i < 16; ++i)
-            if (ch * 16 + i < w2) { const float d = __fadd_rn(__fadd_rn(v[i], b1[ch * 16 + i]), -x0); s1 = __fadd_rn(s1, d); s2 = __fmaf_rn(d, d, s2); }
-    }
-    const float mean = __fadd_rn(x0, __fdiv_rn(s1, (float)w2));
-    const float ss = fmaxf(__fmaf_rn(-s1, __fdiv_rn(s1, (float)w2), s2), 0.f);
-#else
-    float sum = 0.f;
-    for (int ch = 0; ch < n_chunks; ++ch) {
-        tmem_ld16(trow + ch * 16, v);
+        for (int k = 0; k < 7; ++k) ob[k] = obs_s[(h * TC_M + rr) * 8 + k];
+        for (int s = 0; s < n_stages; ++s) {
+            const int q = h * n_stages + s;
+            const uint32_t g = g0 + q, slot = g % TC_STAGES;
+            // the slot's previous MMAs (stage g - TC_STAGES) retired: every thread waited for stage g - 3 before the
+            // barrier of stage g - 1
+            float* a_hi = c.a_ring + (size_t)slot * A_STAGE_FLOATS;
+            float* a_lo = a_hi + TC_CH * TC_M * 4;
+            float hv[4];
 #pragma unroll
-        for (int i = 0; i < 16; ++i)
-            if (ch * 16 + i < w2) sum = __fadd_rn(sum, __fadd_rn(v[i], b1[ch * 16 + i]));
-    }
-    const float mean = __fdiv_rn(sum, (float)w2);
-    float ss = 0.f;
-    for (int ch = 0; ch < n_chunks; ++ch) {
-        tmem_ld16(trow + ch * 16, v);
+            for (int kk = 0; kk < 4; ++kk) {
+                const float4 wa = *reinterpret_cast<const float4*>(W0p + (size_t)(s * TC_KSLAB + jj * 4 + kk) * 8);
+                const float4 wb = *reinterpret_cast<const float4*>(W0p + (size_t)(s * TC_KSLAB + jj * 4 + kk) * 8 + 4);
+                float a = wb.w;                                              // bias
+                a = __fmaf_rn(wa.x, ob[0], a); a = __fmaf_rn(wa.y, ob[1], a); a = __fmaf_rn(wa.z, ob[2], a);
+                a = __fmaf_rn(wa.w, ob[3], a); a = __fmaf_rn(wb.x, ob[4], a); a = __fmaf_rn(wb.y, ob[5], a);
+                a = __fmaf_rn(wb.z, ob[6], a);
+                hv[kk] = a;
+            }
+            const float2 p0 = am_act2<ACT>(make_float2(hv[0], hv[1])), p1 = am_act2<ACT>(make_float2(hv[2], hv[3]));
+            const float4 hi = make_float4(rn_tf32(p0.x), rn_tf32(p0.y), rn_tf32(p1.x), rn_tf32(p1.y));
+            const float4 lo = make_float4(rn_tf32(p0.x - hi.x), rn_tf32(p0.y - hi.y), rn_tf32(p1.x - hi.z), rn_tf32(p1.y - hi.w));
+            *reinterpret_cast<float4*>(a_hi + ((size_t)jj * TC_M + rr) * 4) = hi;
+            *reinterpret_cast<float4*>(a_lo + ((size_t)jj * TC_M + rr) * 4) = lo;
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");      // generic-proxy writes of A -> wgmma (async proxy) reads
+            group_sync(c.grp);
+            // prefetch stage g + 2 into the slot of stage g - 2, retired by every thread before this barrier
+            if (tid == 0 && q + 2 < total) {
+                const uint32_t sl = (g + 2) % TC_STAGES;
+                mbar_expect_tx(&c.full_b[sl], stage_bytes);
+                tma_bulk_g2s(c.b_ring + (size_t)sl * ar.stage_floats, tiles_actor + (size_t)((q + 2) % n_stages) * ar.stage_floats,
+                             stage_bytes, &c.full_b[sl]);
+            }
+            mbar_wait(&c.full_b[slot], (g / TC_STAGES) & 1);               // W1 slab landed
+            const uint32_t a_hi_addr = smem_u32(a_hi), a_lo_addr = smem_u32(a_lo);
+            const uint32_t b_hi_addr = smem_u32(c.b_ring + (size_t)slot * ar.stage_floats);
+            const uint32_t b_lo_addr = b_hi_addr + (uint32_t)TC_CH * (uint32_t)n2pad * 16u;
+            const uint32_t lbo_a = TC_M * 16, lbo_b = (uint32_t)n2pad * 16;
+            const uint64_t dah = wgmma_desc(a_hi_addr, lbo_a, 128), dal = wgmma_desc(a_lo_addr, lbo_a, 128);
+            const uint32_t acc0 = s > 0 ? 1u : 0u;
+            wgmma_fence();
 #pragma unroll
-        for (int i = 0; i < 16; ++i)
-            if (ch * 16 + i < w2) { const float d = __fadd_rn(__fadd_rn(v[i], b1[ch * 16 + i]), -mean); ss = __fmaf_rn(d, d, ss); }
-    }
-#endif
-    const float inv = __fdiv_rn(1.0f, __fadd_rn(__fsqrt_rn(__fdiv_rn(ss, (float)(w2 - 1))), 1e-6f));
-    float o0 = 0.f, o1 = 0.f, o2 = 0.f;
-    for (int ch = 0; ch < n_chunks; ++ch) {
-        tmem_ld16(trow + ch * 16, v);
+            for (int cc = 0; cc < TC_MAXN / TC_NCH; ++cc) {
+                if (cc < nch) {                                              // hi.hi + hi.lo + lo.hi ("3xTF32")
+                    float (&d)[32] = *reinterpret_cast<float (*)[32]>(acc + cc * 32);
+                    const uint32_t bo2 = (uint32_t)(cc * TC_NCH) * 16u;
+                    wgmma_tf32_n64(d, dah, wgmma_desc(b_hi_addr + bo2, lbo_b, 128), acc0);
+                    wgmma_tf32_n64(d, dah, wgmma_desc(b_lo_addr + bo2, lbo_b, 128), 1u);
+                    wgmma_tf32_n64(d, dal, wgmma_desc(b_hi_addr + bo2, lbo_b, 128), 1u);
+                }
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                                                 // stage g - 1 retired
+        }
+        wgmma_wait<0>();
+        // ---- epilogue of the half: rows r0 and r0 + 8 of the thread's warp, spread over the 4 lanes of a quad ----
+        const int r0 = warp * 16 + (lane >> 2), cq = (lane & 3) * 2;
+        float s0 = 0.f, s1 = 0.f;
 #pragma unroll
-        for (int i = 0; i < 16; i += 2) {
-            const int j = ch * 16 + i;
-            const float d0 = __fadd_rn(__fadd_rn(v[i], b1[j]), -mean), d1 = __fadd_rn(__fadd_rn(v[i + 1], b1[j + 1]), -mean);
-            const float2 y = am_act2<ACT>(make_float2(__fmaf_rn(__fmul_rn(gamma[j], d0), inv, beta[j]),
-                                                      __fmaf_rn(__fmul_rn(gamma[j + 1], d1), inv, beta[j + 1])));
-            // padded columns carry zero weights in Wo, so they add nothing
-            o0 = __fmaf_rn(Wo[j], y.x, o0); o0 = __fmaf_rn(Wo[j + 1], y.y, o0);
-            o1 = __fmaf_rn(Wo[n2pad + j], y.x, o1); o1 = __fmaf_rn(Wo[n2pad + j + 1], y.y, o1);
-            o2 = __fmaf_rn(Wo[2 * n2pad + j], y.x, o2); o2 = __fmaf_rn(Wo[2 * n2pad + j + 1], y.y, o2);
+        for (int cc = 0; cc < TC_MAXN / TC_NCH; ++cc) {
+            if (cc < nch) {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    const int j = cc * TC_NCH + i * 8 + cq;
+                    float* d = acc + cc * 32 + i * 4;
+                    d[0] = __fadd_rn(d[0], b1[j]); d[1] = __fadd_rn(d[1], b1[j + 1]);
+                    d[2] = __fadd_rn(d[2], b1[j]); d[3] = __fadd_rn(d[3], b1[j + 1]);
+                    s0 = __fadd_rn(s0, __fadd_rn(d[0], d[1]));           // padded columns hold 0 (zero weights and bias)
+                    s1 = __fadd_rn(s1, __fadd_rn(d[2], d[3]));
+                }
+            }
+        }
+        s0 = __fadd_rn(s0, __shfl_xor_sync(0xffffffffu, s0, 1)); s0 = __fadd_rn(s0, __shfl_xor_sync(0xffffffffu, s0, 2));
+        s1 = __fadd_rn(s1, __shfl_xor_sync(0xffffffffu, s1, 1)); s1 = __fadd_rn(s1, __shfl_xor_sync(0xffffffffu, s1, 2));
+        const float mean0 = __fdiv_rn(s0, (float)w2), mean1 = __fdiv_rn(s1, (float)w2);
+        float v0 = 0.f, v1 = 0.f;
+#pragma unroll
+        for (int cc = 0; cc < TC_MAXN / TC_NCH; ++cc) {
+            if (cc < nch) {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    const int j = cc * TC_NCH + i * 8 + cq;
+                    const float* d = acc + cc * 32 + i * 4;
+                    const float m0 = j < w2 ? 1.f : 0.f, m1 = j + 1 < w2 ? 1.f : 0.f;
+                    const float e00 = __fmul_rn(m0, __fadd_rn(d[0], -mean0)), e01 = __fmul_rn(m1, __fadd_rn(d[1], -mean0));
+                    const float e10 = __fmul_rn(m0, __fadd_rn(d[2], -mean1)), e11 = __fmul_rn(m1, __fadd_rn(d[3], -mean1));
+                    v0 = __fmaf_rn(e00, e00, v0); v0 = __fmaf_rn(e01, e01, v0);
+                    v1 = __fmaf_rn(e10, e10, v1); v1 = __fmaf_rn(e11, e11, v1);
+                }
+            }
+        }
+        v0 = __fadd_rn(v0, __shfl_xor_sync(0xffffffffu, v0, 1)); v0 = __fadd_rn(v0, __shfl_xor_sync(0xffffffffu, v0, 2));
+        v1 = __fadd_rn(v1, __shfl_xor_sync(0xffffffffu, v1, 1)); v1 = __fadd_rn(v1, __shfl_xor_sync(0xffffffffu, v1, 2));
+        const float inv0 = __fdiv_rn(1.0f, __fadd_rn(__fsqrt_rn(__fdiv_rn(v0, (float)(w2 - 1))), 1e-6f));
+        const float inv1 = __fdiv_rn(1.0f, __fadd_rn(__fsqrt_rn(__fdiv_rn(v1, (float)(w2 - 1))), 1e-6f));
+        float o[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+        for (int cc = 0; cc < TC_MAXN / TC_NCH; ++cc) {
+            if (cc < nch) {
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    const int j = cc * TC_NCH + i * 8 + cq;
+                    const float* d = acc + cc * 32 + i * 4;
+                    // padded columns carry zero weights in Wo, so they add nothing
+                    const float2 y0 = am_act2<ACT>(make_float2(__fmaf_rn(__fmul_rn(gamma[j], __fadd_rn(d[0], -mean0)), inv0, beta[j]),
+                                                               __fmaf_rn(__fmul_rn(gamma[j + 1], __fadd_rn(d[1], -mean0)), inv0, beta[j + 1])));
+                    const float2 y1 = am_act2<ACT>(make_float2(__fmaf_rn(__fmul_rn(gamma[j], __fadd_rn(d[2], -mean1)), inv1, beta[j]),
+                                                               __fmaf_rn(__fmul_rn(gamma[j + 1], __fadd_rn(d[3], -mean1)), inv1, beta[j + 1])));
+#pragma unroll
+                    for (int k = 0; k < 3; ++k) {
+                        o[0][k] = __fmaf_rn(Wo[k * n2pad + j], y0.x, o[0][k]); o[0][k] = __fmaf_rn(Wo[k * n2pad + j + 1], y0.y, o[0][k]);
+                        o[1][k] = __fmaf_rn(Wo[k * n2pad + j], y1.x, o[1][k]); o[1][k] = __fmaf_rn(Wo[k * n2pad + j + 1], y1.y, o[1][k]);
+                    }
+                }
+            }
+        }
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                o[r][k] = __fadd_rn(o[r][k], __shfl_xor_sync(0xffffffffu, o[r][k], 1));
+                o[r][k] = __fadd_rn(o[r][k], __shfl_xor_sync(0xffffffffu, o[r][k], 2));
+            }
+        if ((lane & 3) == 0) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                act_s[(h * TC_M + r0) * 4 + k] = am_tanh1(__fadd_rn(o[0][k], bo[k]));
+                act_s[(h * TC_M + r0 + 8) * 4 + k] = am_tanh1(__fadd_rn(o[1][k], bo[k]));
+            }
         }
     }
-    action[0] = am_tanh1(__fadd_rn(o0, bo[0]));
-    action[1] = am_tanh1(__fadd_rn(o1, bo[1]));
-    action[2] = am_tanh1(__fadd_rn(o2, bo[2]));
-    // every warp has read its TMEM lanes: hand the tensor core, the accumulator and the rings to the other group
-    tc_release(c);
+    c.g = g0 + total;
+    tc_release(c);                                                           // (its barrier publishes act_s)
+    action[0] = act_s[tid * 4]; action[1] = act_s[tid * 4 + 1]; action[2] = act_s[tid * 4 + 2];
 }
 
 constexpr int TC_TABN = PT_TOTAL + SERL_PLANT_COUNT * PLANT_NPV;      // plant tables + per-variant parameter rows
 constexpr int TC_TABN2 = (TC_TABN + 15) & ~15;                          // keeps the float regions 128-byte aligned
+constexpr int TC_IO_FLOATS = TC_THREADS * 12;                           // per group: observations [128][8], actions [128][4]
 
-__device__ __forceinline__ void tc_setup(TcCtx& c, const TcArgs& ar, unsigned char* smem_raw, uint64_t* bars, uint32_t* tmem_slot,
-                                         uint32_t* shared_state)
+__device__ __forceinline__ void tc_setup(TcCtx& c, const TcArgs& ar, unsigned char* smem_raw, uint64_t* bars, uint32_t* shared_state)
 {
-    constexpr int A_STAGE_FLOATS = 2 * TC_CH * TC_THREADS * 4;
+    constexpr int A_STAGE_FLOATS = 2 * TC_CH * TC_M * 4;
     real* tab_s = reinterpret_cast<real*>(smem_raw);
     for (int i = threadIdx.x; i < PT_TOTAL; i += blockDim.x) tab_s[i] = plant_tables_blob[i];
     for (int i = threadIdx.x; i < SERL_PLANT_COUNT * PLANT_NPV; i += blockDim.x) tab_s[PT_TOTAL + i] = (&plant_pv[0][0])[i];
@@ -352,33 +347,18 @@ __device__ __forceinline__ void tc_setup(TcCtx& c, const TcArgs& ar, unsigned ch
     c.grp = threadIdx.x >> 7;
     c.gtid = threadIdx.x & (TC_THREADS - 1);
     c.small = f + (size_t)c.grp * small_pad;
-    c.a_ring = f + 2 * (size_t)small_pad;
+    c.io = f + 2 * (size_t)small_pad + (size_t)c.grp * TC_IO_FLOATS;
+    c.a_ring = f + 2 * (size_t)small_pad + 2 * TC_IO_FLOATS;
     c.b_ring = c.a_ring + TC_STAGES * A_STAGE_FLOATS;
-    c.full_b = bars; c.free_s = bars + TC_STAGES; c.acc_bar = bars + 2 * TC_STAGES;
-    c.tmem_slot = tmem_slot;
+    c.full_b = bars;
     c.shared_state = shared_state;
-    c.g = 0; c.steps = 0; c.tmem = 0;
+    c.g = 0;
     if (threadIdx.x == 0) {
-        for (int i = 0; i < 2 * TC_STAGES + 1; ++i) mbar_init(&bars[i], 1);
-        shared_state[0] = shared_state[1] = shared_state[2] = 0;
+        for (int i = 0; i < TC_STAGES; ++i) mbar_init(&bars[i], 1);
+        shared_state[0] = shared_state[1] = 0;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    if ((threadIdx.x >> 5) == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "r"(ar.tmem_cols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    c.tmem = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
-}
-
-__device__ __forceinline__ void tc_teardown(TcCtx& c, const TcArgs& ar)
-{
-    __syncthreads();
-    if ((threadIdx.x >> 5) == 0)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(c.tmem), "r"(ar.tmem_cols) : "memory");
 }
 
 __device__ __forceinline__ void tc_load_small(TcCtx& c, const TcArgs& ar, int actor)
@@ -395,12 +375,11 @@ __global__ void __launch_bounds__(2 * TC_THREADS, 1)
 rollout_kernel_tc(TcArgs ar)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    __shared__ uint64_t bars[2 * TC_STAGES + 1];
-    __shared__ uint32_t tmem_slot;
-    __shared__ uint32_t shared_state[4];
+    __shared__ uint64_t bars[TC_STAGES];
+    __shared__ uint32_t shared_state[2];
     TcCtx c;
     plant_tab_check(smem_raw);
-    tc_setup(c, ar, smem_raw, bars, &tmem_slot, shared_state);
+    tc_setup(c, ar, smem_raw, bars, shared_state);
     const RolloutArgs& r = ar.r;
     const real* tab = reinterpret_cast<const real*>(smem_raw);
     const real* pv_base = tab + PT_TOTAL;
@@ -436,7 +415,7 @@ rollout_kernel_tc(TcArgs ar)
         while (group_any(c.grp, !e.done)) {
             tc_actor_forward<ACT>(c, ar, tiles_actor, obs, a);
             if (!e.done) {
-                if (any_gust) env_step<true, false, true>(e, r, traj, actor, replay, a, obs);
+                if (any_gust) env_step<true, true>(e, r, traj, actor, replay, a, obs);
                 else env_step<true>(e, r, traj, actor, replay, a, obs);
             }
         }
@@ -446,7 +425,6 @@ rollout_kernel_tc(TcArgs ar)
             if (r.status && !isfinite(e.ret + e.X[3] + e.X[7] + e.X[9])) atomicOr(r.status, SERL_STATUS_NONFINITE);
         }
     }
-    tc_teardown(c, ar);
 }
 
 // Actor.forward for a batch through the same tensor-core device code (parity tests of the GEMM path)
@@ -455,11 +433,10 @@ __global__ void __launch_bounds__(2 * TC_THREADS, 1)
 actor_forward_tc_kernel(TcArgs ar)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    __shared__ uint64_t bars[2 * TC_STAGES + 1];
-    __shared__ uint32_t tmem_slot;
-    __shared__ uint32_t shared_state[4];
+    __shared__ uint64_t bars[TC_STAGES];
+    __shared__ uint32_t shared_state[2];
     TcCtx c;
-    tc_setup(c, ar, smem_raw, bars, &tmem_slot, shared_state);
+    tc_setup(c, ar, smem_raw, bars, shared_state);
     tc_load_small(c, ar, 0);
     const int tid = c.gtid;
     for (int base = (blockIdx.x * 2 + c.grp) * TC_THREADS; base < ar.n_obs; base += 2 * gridDim.x * TC_THREADS) {
@@ -470,7 +447,6 @@ actor_forward_tc_kernel(TcArgs ar)
         tc_actor_forward<ACT>(c, ar, ar.tiles, obs, a);
         if (i < ar.n_obs) { ar.act_out[(size_t)i * 3] = a[0]; ar.act_out[(size_t)i * 3 + 1] = a[1]; ar.act_out[(size_t)i * 3 + 2] = a[2]; }
     }
-    tc_teardown(c, ar);
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------
@@ -502,6 +478,14 @@ extern "C" int64_t serl_actor_num_params_wide(const int32_t* widths, int32_t n_w
     return P + 3 * (int64_t)widths[n_widths - 1] + 3;
 }
 
+static int device_sms()
+{
+    int sms = 0, dev = 0;
+    cudaGetDevice(&dev);
+    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
+    return sms;
+}
+
 static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t* widths, int n_widths, cudaStream_t s, size_t* smem_out)
 {
     if (n_widths != 2) return serl_fail(SERL_ERR_UNSUPPORTED, "wide actors: the tensor-core path implements two hidden layers [w1, w2]");
@@ -510,10 +494,7 @@ static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t
         return serl_fail(SERL_ERR_UNSUPPORTED, "wide actors: need w1 % 8 == 0, 8 <= w1 <= 1024, 8 <= w2 <= 320");
     ar.w1_real = w1;
     ar.w1 = (w1 + TC_KSLAB - 1) / TC_KSLAB * TC_KSLAB;
-    ar.w2 = w2; ar.n2pad = (w2 + 15) & ~15;
-    int cols = 32;
-    while (cols < ar.n2pad) cols <<= 1;
-    ar.tmem_cols = cols;
+    ar.w2 = w2; ar.n2pad = (w2 + TC_NCH - 1) / TC_NCH * TC_NCH;
     ar.small_floats = (tc_small_floats(ar.w1, ar.n2pad) + 3) & ~3;
     ar.stage_floats = 2 * TC_CH * ar.n2pad * 4;
     const int P = (int)serl_actor_num_params_wide(widths, n_widths);
@@ -530,9 +511,9 @@ static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t
     const int grid = (int)((total + 255) / 256 < 8192 ? (total + 255) / 256 : 8192);
     tc_layout_kernel<<<grid, 256, 0, s>>>(d_weights, pop, P, ar.w1, w1, w2, ar.n2pad, ar.small_floats, ar.stage_floats, small, tiles);
     serl_count_launch();
-    constexpr int A_STAGE_FLOATS = 2 * TC_CH * TC_THREADS * 4;
+    constexpr int A_STAGE_FLOATS = 2 * TC_CH * TC_M * 4;
     *smem_out = (size_t)TC_TABN2 * sizeof(real) +
-                (size_t)(2 * ((ar.small_floats + 31) & ~31) + TC_STAGES * A_STAGE_FLOATS + TC_STAGES * ar.stage_floats) * 4;
+                (size_t)(2 * ((ar.small_floats + 31) & ~31) + 2 * TC_IO_FLOATS + TC_STAGES * A_STAGE_FLOATS + TC_STAGES * ar.stage_floats) * 4;
     if (*smem_out > 227 * 1024 - 256) return serl_fail(SERL_ERR_UNSUPPORTED, "wide actors: tables + parameters + rings exceed the shared memory of an SM");
     return SERL_OK;
 }
@@ -558,9 +539,7 @@ int rollout_tc_impl(const serl_rollout_desc& d, const int32_t* widths, int n_wid
     if (rc != SERL_OK) return rc;
     ar.n_chunks = (d.n_envs + TC_THREADS - 1) / TC_THREADS;
     ar.n_tasks = (long long)d.pop * ar.n_chunks;
-    int sms = 148, dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    int sms = device_sms();
     if (d.sm_limit > 0 && d.sm_limit < sms) sms = d.sm_limit;
     const long long grid = (ar.n_tasks + 1) / 2 < sms ? (ar.n_tasks + 1) / 2 : sms;
     cudaError_t e;
@@ -588,7 +567,8 @@ extern "C" int serl_actor_forward_wide(const float* d_genome, const int32_t* wid
     if (rc != SERL_OK) return rc;
     ar.obs_in = d_obs; ar.act_out = d_actions; ar.n_obs = n;
     const int blocks = (n + 2 * TC_THREADS - 1) / (2 * TC_THREADS);
-    const int grid = blocks < 148 ? blocks : 148;
+    const int sms = device_sms();
+    const int grid = blocks < sms ? blocks : sms;
     cudaError_t e;
 #define TC_LAUNCH(A) do { e = cudaFuncSetAttribute(actor_forward_tc_kernel<A>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
         if (e == cudaSuccess) { actor_forward_tc_kernel<A><<<grid, 2 * TC_THREADS, smem, s>>>(ar); e = cudaGetLastError(); } } while (0)

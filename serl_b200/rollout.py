@@ -145,7 +145,7 @@ def num_params_wide(widths):
 
 
 def actor_forward_wide(genome, widths, activation, obs):
-    """forward pass of a wide [w1, w2] actor for a batch of observations through the tensor-core device code (tcgen05 3xTF32)."""
+    """forward pass of a wide [w1, w2] actor for a batch of observations through the tensor-core device code (wgmma 3xTF32)."""
     if not genome.is_cuda:
         raise _native.NativeError('actor_forward_wide needs CUDA tensors (no CPU fallback)')
     assert genome.dtype == torch.float32 and genome.is_contiguous() and genome.numel() == num_params_wide(widths)

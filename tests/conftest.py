@@ -9,12 +9,12 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100)')
     config.addinivalue_line('markers', 'refbin: needs the reference plant binaries under oracle/_ref')
 
 
 def pytest_collection_modifyitems(config, items):
-    """GPU tests go through the in-tree C-ABI library; build it (nvcc, sm_100a) if the snapshot arrived without it."""
+    """GPU tests go through the in-tree C-ABI library; build it (nvcc, sm_90a) if the tree arrived without it."""
     if any('gpu' in item.keywords for item in items):
         try:
             import torch

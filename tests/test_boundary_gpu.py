@@ -55,39 +55,37 @@ def test_plant_step_kernel_matches_oracle(variant):
     assert np.allclose(got[:, live], ref[:, live], rtol=1e-11, atol=1e-12)
 
 
-@pytest.mark.skipif(not os.path.exists(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), 'oracle', '_ref', 'citation_gust.so')),
-                    reason='needs the reference gust binary under oracle/_ref')
 @pytest.mark.parametrize('build', ['gust', 'test'])
 def test_timed_plant_step_api_flies_the_gust_pulse_like_the_binary(build):
     """serl_plant_step_timed with SERL_MODE_GUST (the per-step path of CitationEnv in 'gust' mode): one-step predictions from
-    the binary's own states through both edges of the pulse (native calls 1996..2003, 2296..2303) and in its middle."""
+    the binary's own states through both edges of the pulse (native calls 1996..2003, 2296..2303) and in its middle.  The
+    binary's states before and after each of those calls are stored in tests/golden/refbin_kat.npz."""
     from serl_b200 import _native, rollout
     L = _native.lib()
     dev = torch.device('cuda:0')
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    pl = OP.RefPlant(build)          # envs/test: the same pulse with the opposite sign
-    X = pl.initial_state()
+    kat = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'refbin_kat.npz'))
+    X0, X1 = kat['timed_%s_X0' % build], kat['timed_%s_X1' % build]          # envs/test: the same pulse with the opposite sign
     var = torch.tensor([rollout.mode_code(build) & ~0xff00], dtype=torch.int32, device=dev)
     live = [0, 1, 2, 3, 4, 5, 6, 7, 9, 12, 15, 16, 17, 18]
     worst, changed = 0.0, 0
-    for k in range(2306):
+    ks = [k for k in range(2306) if 1996 <= k <= 2003 or 2296 <= k <= 2303 or k == 2150]
+    assert len(ks) == len(X0)
+    for w, k in enumerate(ks):
         cmd = 0.02 * np.sin(0.01 * k + np.arange(3))
-        window = 1996 <= k <= 2003 or 2296 <= k <= 2303 or k == 2150
-        if window:
-            Xd = torch.as_tensor(X[None].copy(), device=dev)
-            d = torch.as_tensor(cmd[None].copy(), device=dev)
-            call = torch.tensor([k], dtype=torch.int32, device=dev)
-            _native.check(L.serl_plant_step_timed(ctypes.c_void_p(Xd.data_ptr()), ctypes.c_void_p(d.data_ptr()), ctypes.c_void_p(var.data_ptr()),
-                                                  ctypes.c_void_p(call.data_ptr()), 1, st), 'serl_plant_step_timed')
-            call0 = torch.tensor([0], dtype=torch.int32, device=dev)
-            Xn = torch.as_tensor(X[None].copy(), device=dev)
-            _native.check(L.serl_plant_step_timed(ctypes.c_void_p(Xn.data_ptr()), ctypes.c_void_p(d.data_ptr()), ctypes.c_void_p(var.data_ptr()),
-                                                  ctypes.c_void_p(call0.data_ptr()), 1, st), 'serl_plant_step_timed')
-        _, X = pl.step(X, np.concatenate([cmd, np.zeros(7)]))
-        if window:
-            got = Xd.cpu().numpy()[0]
-            worst = max(worst, np.abs(got[live] - X[live]).max())
-            changed += int(np.abs(Xn.cpu().numpy()[0][live] - X[live]).max() > 1e-6)        # the same step outside the pulse (call 0)
+        Xd = torch.as_tensor(X0[w][None].copy(), device=dev)
+        d = torch.as_tensor(cmd[None].copy(), device=dev)
+        call = torch.tensor([k], dtype=torch.int32, device=dev)
+        _native.check(L.serl_plant_step_timed(ctypes.c_void_p(Xd.data_ptr()), ctypes.c_void_p(d.data_ptr()), ctypes.c_void_p(var.data_ptr()),
+                                              ctypes.c_void_p(call.data_ptr()), 1, st), 'serl_plant_step_timed')
+        call0 = torch.tensor([0], dtype=torch.int32, device=dev)
+        Xn = torch.as_tensor(X0[w][None].copy(), device=dev)
+        _native.check(L.serl_plant_step_timed(ctypes.c_void_p(Xn.data_ptr()), ctypes.c_void_p(d.data_ptr()), ctypes.c_void_p(var.data_ptr()),
+                                              ctypes.c_void_p(call0.data_ptr()), 1, st), 'serl_plant_step_timed')
+        X = X1[w]
+        got = Xd.cpu().numpy()[0]
+        worst = max(worst, np.abs(got[live] - X[live]).max())
+        changed += int(np.abs(Xn.cpu().numpy()[0][live] - X[live]).max() > 1e-6)        # the same step outside the pulse (call 0)
     assert worst < 1e-9, worst
     assert changed >= 10
 

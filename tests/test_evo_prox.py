@@ -1,16 +1,42 @@
-"""N3: proximal / safe mutation batched over the population (serl_b200/evo_prox.py) against (a) the reference module itself
-(base/core/mod_neuro_evo.py:183-252, imported in the build container) and (b) a per-actor autograd restatement."""
+"""N3: proximal / safe mutation batched over the population (serl_b200/evo_prox.py) against (a) what the reference module
+itself (base/core/mod_neuro_evo.py:183-252, base/core/genetic_agent.py:22-60) computed on the same seeded inputs, stored by
+tests/golden/make_golden_evo_ref.py, and (b) a per-actor autograd restatement."""
 import os
-import sys
-import types
 
 import numpy as np
-import pytest
 import torch
 
+from oracle import actor as OA
 from serl_b200 import evo, evo_prox
 
-REF = '/root/reference/base'
+SHAPE = (7, 3, 72, 3)                      # the reference's default actor: hidden 72, 3 layers, tanh
+SAMPLE_COLS = np.sort(np.random.RandomState(0).choice(OA.num_params(*SHAPE), 512, replace=False))     # stored genome columns
+
+
+def stored():
+    return np.load(os.path.join(os.path.dirname(__file__), 'golden', 'evo_ref_kat.npz'))
+
+
+def proximal_inputs(mag):
+    """three actors initialised in the reference's order under seed 0, their state batches, the Gaussian draws"""
+    torch.manual_seed(0)
+    G = torch.stack([torch.from_numpy(OA.flatten(OA.Actor())) for _ in range(3)])
+    states = torch.randn(3, 32, 7) * 0.1
+    nw = int(evo_prox.weight_mask(SHAPE, G.device).sum())          # the draw covers the weight matrices only
+    deltas = []
+    for k in range(3):
+        torch.manual_seed(100 + k)
+        deltas.append(torch.distributions.Normal(torch.zeros(nw), torch.ones(nw) * mag).sample())
+    return G, states, torch.stack(deltas)
+
+
+def distillation_inputs():
+    """children, first and second parents (initialised in that order under seed 0), the critic's layer, the states"""
+    torch.manual_seed(0)
+    G0, G1, G2 = (torch.stack([torch.from_numpy(OA.flatten(OA.Actor())) for _ in range(3)]) for _ in range(3))
+    lin = torch.nn.Linear(10, 2)
+    states = torch.randn(3, 40, 7) * 0.2
+    return G0, G1, G2, lin, states
 
 
 def per_actor_reference(genome, states, shape, activation, mag, delta):
@@ -50,101 +76,43 @@ def test_batched_equals_per_actor_restatement():
     assert torch.equal(G2[:, ~m], G[:, ~m])
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason='needs the reference tree (build container only)')
-def test_batched_proximal_mutation_equals_the_reference_module(tmp_path, monkeypatch):
-    monkeypatch.chdir(tmp_path)
-    saved = {k: sys.modules.pop(k) for k in list(sys.modules) if k == 'core' or k.startswith('core.') or k == 'parameters'}
-    sys.path.insert(0, REF)
-    try:
-        from core import mod_neuro_evo as ref_ne, genetic_agent as ref_ga
-        from parameters import Parameters as RefP
-        import torch.distributions as dist
-        args = RefP(types.SimpleNamespace(pop_size=4, mut_type='proximal', env='x', frames=1, seed=1, disable_cuda=True))
-        args.state_dim, args.action_dim, args.device = 7, 3, torch.device('cpu')
-        torch.manual_seed(0)
-        genes = [ref_ga.GeneticAgent(args) for _ in range(3)]
-        shape = (7, 3, args.hidden_size, args.num_layers)
-        G = torch.stack([torch.cat([p.data.reshape(-1) for p in g.actor.parameters()]) for g in genes])
-        states = torch.randn(3, 32, 7) * 0.1
-        ssne = ref_ne.SSNE(args, None, None)
-
-        class FakeBuf:
-            def __init__(self, st):
-                self.st = st
-
-            def __len__(self):
-                return 32
-
-            def sample(self, n):
-                return (self.st, None, None, None, None)
-        deltas = []
-        for k, g in enumerate(genes):
-            g.buffer = FakeBuf(states[k])
-            tot = g.actor.count_parameters()
-            torch.manual_seed(100 + k)
-            deltas.append(dist.Normal(torch.zeros(tot), torch.ones(tot) * args.mutation_mag).sample())
-            torch.manual_seed(100 + k)
-            ssne.proximal_mutate(g, mag=args.mutation_mag)
-        G_ref = torch.stack([torch.cat([p.data.reshape(-1) for p in g.actor.parameters()]) for g in genes])
-    finally:
-        sys.path.remove(REF)
-        for k in [k for k in sys.modules if k == 'core' or k.startswith('core.') or k == 'parameters']:
-            del sys.modules[k]
-        sys.modules.update(saved)
+def test_batched_proximal_mutation_equals_the_reference_module():
+    KAT = stored()
+    mag = float(KAT['prox_mag'])
+    G, states, deltas = proximal_inputs(mag)
     G2 = G.clone()
-    evo_prox.proximal_mutate_batched(G2, [0, 1, 2], states, shape, args.activation_actor, args.mutation_mag, delta=torch.stack(deltas))
-    assert (G_ref - G).abs().max() > 0.1
-    assert (G2 - G_ref).abs().max().item() <= 1e-6
+    evo_prox.proximal_mutate_batched(G2, [0, 1, 2], states, SHAPE, 'tanh', mag, delta=deltas)
+    G_ref = torch.from_numpy(KAT['prox_G_ref'])
+    assert float(KAT['prox_moved']) > 0.1
+    assert (G2 - G).abs().max() > 0.1
+    assert (G2[:, SAMPLE_COLS] - G_ref).abs().max().item() <= 1e-6
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason='needs the reference tree (build container only)')
-def test_batched_distillation_step_equals_the_reference_update_parameters(tmp_path, monkeypatch):
+def test_batched_distillation_step_equals_the_reference_update_parameters():
     """one Q-filtered behaviour-cloning Adam step (base/core/genetic_agent.py:22-60) for three children at once."""
     from serl_b200 import evo_distil
-    monkeypatch.chdir(tmp_path)
-    saved = {k: sys.modules.pop(k) for k in list(sys.modules) if k == 'core' or k.startswith('core.') or k == 'parameters'}
-    sys.path.insert(0, REF)
-    try:
-        from core import genetic_agent as ref_ga
-        from parameters import Parameters as RefP
-        args = RefP(types.SimpleNamespace(pop_size=4, mut_type='proximal', env='x', frames=1, seed=1, disable_cuda=True))
-        args.state_dim, args.action_dim, args.device = 7, 3, torch.device('cpu')
-        torch.manual_seed(0)
-        kids = [ref_ga.GeneticAgent(args) for _ in range(3)]
-        p1s = [ref_ga.GeneticAgent(args) for _ in range(3)]
-        p2s = [ref_ga.GeneticAgent(args) for _ in range(3)]
-        flat = lambda g: torch.cat([p.data.reshape(-1) for p in g.actor.parameters()])
-        lin = torch.nn.Linear(10, 2)
+    KAT = stored()
+    G0, G1, G2, lin, states = distillation_inputs()
 
-        def critic(s, a):
-            q = lin(torch.cat((s, a), 1))
-            return q[:, :1], q[:, 1:]
-        states = torch.randn(3, 40, 7) * 0.2
-        shape = (7, 3, args.hidden_size, args.num_layers)
-        G0 = torch.stack([flat(k) for k in kids])
-        G1, G2 = torch.stack([flat(p) for p in p1s]), torch.stack([flat(p) for p in p2s])
-        mse_ref = [kids[c].update_parameters((states[c], None, None, None, None), p1s[c].actor, p2s[c].actor, critic) for c in range(3)]
-        G_ref = torch.stack([flat(k) for k in kids])
-    finally:
-        sys.path.remove(REF)
-        for k in [k for k in sys.modules if k == 'core' or k.startswith('core.') or k == 'parameters']:
-            del sys.modules[k]
-        sys.modules.update(saved)
+    def critic(s, a):
+        q = lin(torch.cat((s, a), 1))
+        return q[:, :1], q[:, 1:]
     child = G0.clone().requires_grad_(True)
     opt = torch.optim.Adam([child], lr=1e-3)
     with torch.no_grad():
-        a1 = evo_prox.actor_forward_batched(G1, states, shape, 'tanh')
-        a2 = evo_prox.actor_forward_batched(G2, states, shape, 'tanh')
+        a1 = evo_prox.actor_forward_batched(G1, states, SHAPE, 'tanh')
+        a2 = evo_prox.actor_forward_batched(G2, states, SHAPE, 'tanh')
         fl = states.reshape(120, 7)
         q1 = torch.min(*critic(fl, a1.reshape(120, 3))).reshape(3, 40)
         q2 = torch.min(*critic(fl, a2.reshape(120, 3))).reshape(3, 40)
     opt.zero_grad()
-    loss, mse = evo_distil.cloning_loss(evo_prox.actor_forward_batched(child, states, shape, 'tanh'), a1, a2, q1, q2)
+    loss, mse = evo_distil.cloning_loss(evo_prox.actor_forward_batched(child, states, SHAPE, 'tanh'), a1, a2, q1, q2)
     loss.backward()
     opt.step()
-    assert (G_ref - G0).abs().max() > 1e-4
-    assert (child.detach() - G_ref).abs().max().item() <= 2e-6
-    assert np.allclose(mse.numpy(), np.asarray(mse_ref), rtol=1e-4)
+    G_ref = torch.from_numpy(KAT['distil_G_ref'])
+    assert float(KAT['distil_moved']) > 1e-4
+    assert (child.detach()[:, SAMPLE_COLS] - G_ref).abs().max().item() <= 2e-6
+    assert np.allclose(mse.numpy(), KAT['distil_mse'], rtol=1e-4)
 
 
 def test_sort_groups_by_fitness_order():

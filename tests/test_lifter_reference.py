@@ -1,26 +1,25 @@
-"""Container-only checks of the lifter's hand-restated helper semantics against the exported functions of the reference
-binary itself (rt_GetLookupIndex @0xf470, rt_Lookup @0xf530, rt_Lookup2D_Normal @0xf590), including exact ties, and of the
-branch-free breakpoint count the generated code uses."""
+"""The lifter's hand-restated helper semantics against the exported functions of the reference binary
+(rt_GetLookupIndex @0xf470, rt_Lookup @0xf530, rt_Lookup2D_Normal @0xf590), including exact ties, and the branch-free
+breakpoint count the generated code uses.  The binary's answers are stored in tests/golden/refbin_kat.npz
+(make_golden_refbin.py calls load_binary_lookups / index_cases / formula_cases below on the binary)."""
 import ctypes
 import os
 import shutil
 import sys
+import tempfile
 
 import numpy as np
-import pytest
 
-REF = '/root/reference/envs/h2000_v90/_citation.cpython-38-x86_64-linux-gnu.so'
-pytestmark = pytest.mark.skipif(not os.path.exists(REF), reason='needs the reference tree (build container only)')
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, 'tools', 'lift'))
 D = ctypes.c_double
+KAT = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'refbin_kat.npz'))
 
 
-@pytest.fixture(scope='module')
-def lib(tmp_path_factory):
-    p = tmp_path_factory.mktemp('ref') / 'c.so'
-    shutil.copy(REF, p)
-    L = ctypes.CDLL(str(p))
+def load_binary_lookups(so):
+    p = os.path.join(tempfile.mkdtemp(), 'c.so')
+    shutil.copy(so, p)
+    L = ctypes.CDLL(p)
     L.rt_GetLookupIndex.restype = ctypes.c_int
     L.rt_GetLookupIndex.argtypes = [ctypes.POINTER(D), ctypes.c_int, D]
     L.rt_Lookup.restype = D
@@ -48,18 +47,17 @@ def count_rule(x, u):
     return sum((xj <= u) if xj < 0 else (xj < u) for xj in x[1:-1])
 
 
-def test_lookup_index_restatements_equal_the_binary(lib):
-    import symtrace as S
+def index_cases(lib=None):
+    """(breakpoints, probe, the binary's index or None) in a fixed order"""
     rng = np.random.RandomState(0)
     for x in axes(rng):
         arr = (D * len(x))(*x)
         for u in probes(x, rng):
-            ref = lib.rt_GetLookupIndex(arr, len(x), float(u))
-            assert S.Tracer.lookup_index(list(x), float(u)) == ref, (list(x), u)
-            assert count_rule(x, u) == ref, (list(x), u)
+            yield x, u, (lib.rt_GetLookupIndex(arr, len(x), float(u)) if lib else None)
 
 
-def test_lookup_formulas_equal_the_binary(lib):
+def formula_cases(lib=None):
+    """(the binary's 2-D lookup, its 1-D lookup, my 2-D value, my 1-D value) in a fixed order"""
     import symtrace as S
     rng = np.random.RandomState(1)
     li = S.Tracer.lookup_index
@@ -74,8 +72,26 @@ def test_lookup_formulas_equal_the_binary(lib):
             a = (zs[ix + 1 + nx * iy] - zs[ix + nx * iy]) / dx * ux + zs[ix + nx * iy]
             b = (zs[ix + 1 + nx * (iy + 1)] - zs[ix + nx * (iy + 1)]) / dx * ux + zs[ix + nx * (iy + 1)]
             mine = (b - a) / (ys[iy + 1] - ys[iy]) * (y - ys[iy]) + a
-            assert mine == lib.rt_Lookup2D_Normal(X, nx, Y, ny, Z, x, y)           # bit-exact
             i = li(list(xs), x)
             zz = zs[:nx]
             mine1 = (zz[i + 1] - zz[i]) / (xs[i + 1] - xs[i]) * (x - xs[i]) + zz[i]
-            assert mine1 == lib.rt_Lookup(X, nx, x, (D * nx)(*zz))
+            ref2 = lib.rt_Lookup2D_Normal(X, nx, Y, ny, Z, x, y) if lib else None
+            ref1 = lib.rt_Lookup(X, nx, x, (D * nx)(*zz)) if lib else None
+            yield ref2, ref1, mine, mine1
+
+
+def test_lookup_index_restatements_equal_the_binary():
+    import symtrace as S
+    cases = list(index_cases())
+    assert len(cases) == len(KAT['lookup_index'])
+    for (x, u, _), ref in zip(cases, KAT['lookup_index']):
+        assert S.Tracer.lookup_index(list(x), float(u)) == ref, (list(x), u)
+        assert count_rule(x, u) == ref, (list(x), u)
+
+
+def test_lookup_formulas_equal_the_binary():
+    cases = list(formula_cases())
+    assert len(cases) == len(KAT['lookup2d'])
+    for (_, _, mine, mine1), ref2, ref1 in zip(cases, KAT['lookup2d'], KAT['lookup1d']):
+        assert mine == ref2           # bit-exact
+        assert mine1 == ref1

@@ -1,5 +1,5 @@
 """BASELINE config 5: wide two-hidden-layer actors ([400,300], [128,128]) on the tensor-core rollout kernel
-(csrc/rollout_tc.cu: tcgen05.mma kind::tf32 as 3xTF32, TMEM accumulator, TMA-streamed weight slabs).
+(csrc/rollout_tc.cu: wgmma .tf32 as 3xTF32, register accumulators, TMA-streamed weight slabs).
 
 The tensor core's accumulation order cannot be restated on a CPU, so this path is compared with the torch fp32 oracle
 (oracle/actor.py WideActor = the reference's Actor form with a width list) within a tolerance:
@@ -70,7 +70,7 @@ def test_wide_closed_loop_against_the_c_episode_port(widths):
 
 def test_config5_shape_many_ctas_deterministic():
     """pop x 256 envs: two 128-env chunks per actor, more CTAs than resident slots, identical genomes -> identical bits
-    (two CTAs per SM share the tensor core and, for w2 > 256, take turns on the TMEM columns)."""
+    (the two groups of a CTA take turns on the shared weight ring)."""
     from serl_b200 import rollout
     dev = torch.device('cuda:0')
     for widths in ([400, 300], [128, 128]):
