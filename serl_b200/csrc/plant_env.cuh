@@ -182,6 +182,10 @@ __device__ __forceinline__ double plant_cos_fast(double x) { double s, c; plant_
 // the right-hand side works on the 14 live continuous states only: rtX index -> position in the compact arrays
 #define PLANT_XI(i) ((i) < 8 ? (i) : ((i) == 9 ? 8 : ((i) == 12 ? 9 : (i) - 5)))
 #include PLANT_GEN(plant_ic.h)
+// The generated right-hand sides are inlined into the by-value wrappers plant_rhs_regs / plant_rhs_regs_smem below.
+#undef PLANT_FN
+#define PLANT_FN static __device__ __forceinline__
+#define PLANT_RHS_COMMON_NAME plant_rhs_common
 #include PLANT_GEN(plant_rhs_common.h)     // ONE function for every plant variant + per-variant parameter rows
 // Second instance of the same generated text for kernels that stage the tables (+ parameter rows) at the START of their
 // dynamic shared memory: tables and parameter rows are read as plant_smem_tab[...] — the compiler sees the shared address
@@ -212,6 +216,8 @@ __device__ __forceinline__ int plant_smem_index(const real* p)          // eleme
 #undef PLANT_RHS_COMMON_NAME
 #undef PLANT_TAB
 #undef PLANT_PV
+#undef PLANT_FN
+#define PLANT_FN static __device__ __noinline__
 #define PLANT_TAB(name) (plant_tab + PT_OFF_##name)
 #define PLANT_PV(k) plant_pvrow[k]
 #undef PLANT_XI
@@ -222,6 +228,29 @@ __device__ __forceinline__ int plant_smem_index(const real* p)          // eleme
 #define NX 19
 #define NLIVE 14
 #define MAX_CTA_THREADS 256
+
+// State vectors travel BY VALUE between the out-of-line plant functions: the struct arguments and results of a
+// __noinline__ function are passed in registers, whereas an array whose address is handed to one lives in local memory
+// (an L2 round trip inside the stage-to-stage dependency chain of the integrator).
+struct PlantLive { real v[NLIVE]; };       // live continuous states / their derivatives, compact order (PLANT_XI)
+struct PlantState { double v[NX]; };       // the integrator state rtX
+// ONE out-of-line copy of the right-hand side per table address space (the generated body is inlined here only)
+static __device__ __noinline__ PlantLive plant_rhs_regs(PlantLive x, real u0, real u1, real u2, real u3, const real* tab,
+                                                        const real* pvrow)
+{
+    const real u[4] = {u0, u1, u2, u3};
+    PlantLive d;
+    plant_rhs_common(x.v, u, d.v, tab, pvrow);
+    return d;
+}
+static __device__ __noinline__ PlantLive plant_rhs_regs_smem(PlantLive x, real u0, real u1, real u2, real u3, const real* tab,
+                                                             const real* pvrow)
+{
+    const real u[4] = {u0, u1, u2, u3};
+    PlantLive d;
+    plant_rhs_common_smem(x.v, u, d.v, tab, pvrow);
+    return d;
+}
 
 // live continuous states of the plant (SURVEY.md 2.3): p q r V alpha beta phi theta | h | washout | N1 N1 N2 N2
 // (psi, x_e, y_e never feed back and are integrated only for traces; Parameter_CSTATE(_g) are folded constants).
@@ -278,8 +307,9 @@ static __device__ __noinline__ void plant_step_nav(double* Xnav, const double* X
 }
 
 // Stage loop fully unrolled (h*B folds to constants).  The right-hand side is ONE __noinline__ function (the same code for
-// every plant variant), so the compact state x[14], the stage derivative it writes and the six stage derivatives are in
-// local memory (672 bytes per thread, cached in L1 / L2).  The integrator state and the
+// every plant variant) that takes the stage state and returns the stage derivative by value.  The six stage derivatives
+// (84 values, all live for the last combination) do not fit next to the rest in 255 registers: ptxas keeps part of them
+// in local memory.  The integrator state and the
 // stage combinations are double in every build; `real` (the type of the right-hand side) is double unless PLANT_F32.
 // pv_post / call: time-triggered builds (cg_timed): the parameter row switches to pv_post when the model clock
 // call * 0.01 + c_s * 0.01 of a stage reaches 20 s: every stage from call SERL_TRIGGER_CALLS on, and the LAST stage (c = 1) of
@@ -297,45 +327,55 @@ __device__ __forceinline__ real plant_gust_offset(int call, int s, real V)
     if (!on) return (real)0;
     return (real)(atan(PLANT_DIV((double)SERL_GUST_W, (double)V)) * 1.0);
 }
+// X (the state) and the command arrive by value and the new state is returned: nothing of the hot path has its address
+// taken (see PlantState).  Only the trace path (nav) copies the stage derivatives to an array for plant_step_nav.
 template <bool STAB = false, bool GUST = false>
-static __device__ __noinline__ void plant_step(const real* pv, double* X, const double* U, const real* tab, bool nav = false,
-                                               const real* pv_post = nullptr, int call = 0)
+static __device__ __noinline__ PlantState plant_step(const real* pv, PlantState X, double U0, double U1, double U2, const real* tab,
+                                                     bool nav = false, const real* pv_post = nullptr, int call = 0)
 {
     const bool gust = GUST && (call & PLANT_CALL_GUST) != 0, gust_up = GUST && (call & PLANT_CALL_GUST_UP) != 0;
     if (GUST) call &= ~(PLANT_CALL_GUST | PLANT_CALL_GUST_UP);
     constexpr double h = 0.01;
     constexpr double B[6][6] = ODE5_B_INIT;
     constexpr int LIVE[NLIVE] = ODE5_LIVE_INIT;
-    real x[NLIVE], u[4];
-    u[0] = (real)U[0]; u[1] = (real)U[1]; u[2] = (real)U[2]; u[3] = (real)0;
+    const real u0 = (real)U0, u1 = (real)U1, u2 = (real)U2;
+    real u3 = (real)0;
+    PlantLive x;
 #pragma unroll
-    for (int li = 0; li < NLIVE; ++li) x[li] = (real)X[LIVE[li]];
+    for (int li = 0; li < NLIVE; ++li) x.v[li] = (real)X.v[LIVE[li]];
     double xl[NLIVE];
-    {
-        real f[6][NLIVE];
+    PlantLive f[6];
 #pragma unroll
-        for (int s = 0; s < 6; ++s) {
-            const bool post = pv_post != nullptr && (call >= SERL_TRIGGER_CALLS || (s == 5 && call == SERL_TRIGGER_CALLS - 1));
-            if (GUST) { u[3] = gust ? plant_gust_offset(call, s, x[3]) : (real)0; if (gust_up) u[3] = -u[3]; }
-            if (STAB) plant_rhs_common_smem(x, u, f[s], tab, post ? pv_post : pv);
-            else plant_rhs_common(x, u, f[s], tab, post ? pv_post : pv);
+    for (int s = 0; s < 6; ++s) {
+        const bool post = pv_post != nullptr && (call >= SERL_TRIGGER_CALLS || (s == 5 && call == SERL_TRIGGER_CALLS - 1));
+        if (GUST) { u3 = gust ? plant_gust_offset(call, s, x.v[3]) : (real)0; if (gust_up) u3 = -u3; }
+        f[s] = STAB ? plant_rhs_regs_smem(x, u0, u1, u2, u3, tab, post ? pv_post : pv)
+                    : plant_rhs_regs(x, u0, u1, u2, u3, tab, post ? pv_post : pv);
 #pragma unroll
-            for (int li = 0; li < NLIVE; ++li) {
-                double acc = (double)f[0][li] * (h * B[s][0]);
+        for (int li = 0; li < NLIVE; ++li) {
+            double acc = (double)f[0].v[li] * (h * B[s][0]);
 #pragma unroll
-                for (int j = 1; j <= s; ++j) acc += (double)f[j][li] * (h * B[s][j]);
-                xl[li] = X[LIVE[li]] + acc;
-                x[li] = (real)xl[li];
-            }
-        }
-        if (nav) {
-            double xn[3];
-            plant_step_nav(xn, X, f, u, tab);
-            X[8] = xn[0]; X[10] = xn[1]; X[11] = xn[2];
+            for (int j = 1; j <= s; ++j) acc += (double)f[j].v[li] * (h * B[s][j]);
+            xl[li] = X.v[LIVE[li]] + acc;
+            x.v[li] = (real)xl[li];
         }
     }
+    if (nav) {
+        double X0[NX], xn[3];
+        real fa[6][NLIVE];
+        const real u[4] = {u0, u1, u2, u3};
 #pragma unroll
-    for (int li = 0; li < NLIVE; ++li) X[LIVE[li]] = xl[li];
+        for (int i = 0; i < NX; ++i) X0[i] = X.v[i];
+#pragma unroll
+        for (int s = 0; s < 6; ++s)
+#pragma unroll
+            for (int li = 0; li < NLIVE; ++li) fa[s][li] = f[s].v[li];
+        plant_step_nav(xn, X0, fa, u, tab);
+        X.v[8] = xn[0]; X.v[10] = xn[1]; X.v[11] = xn[2];
+    }
+#pragma unroll
+    for (int li = 0; li < NLIVE; ++li) X.v[LIVE[li]] = xl[li];
+    return X;
 }
 
 // activations: IEEE-only sequences of actor_math.cuh (bit-reproducible on a CPU; see oracle/plant/actor_kernel_order.c)
@@ -403,6 +443,18 @@ struct Env {
     int gust;                // env_mode >> 24: 1 = SERL_MODE_GUST, 3 = with SERL_MODE_GUST_UP
 };
 
+// one plant step of the env (reset's zero-command step and env_step share this single plant_step instance)
+template <bool STAB, bool GUST>
+__device__ __forceinline__ void plant_step_env(Env& e, const double* cmd, bool nav, int call)
+{
+    PlantState s;
+#pragma unroll
+    for (int i = 0; i < NX; ++i) s.v[i] = e.X[i];
+    s = plant_step<STAB, GUST>(e.pv, s, cmd[0], cmd[1], cmd[2], e.tab, nav, e.pv_post, call);
+#pragma unroll
+    for (int i = 0; i < NX; ++i) e.X[i] = s.v[i];
+}
+
 #define DEG2RAD 0.017453292519943295   // numpy deg2rad multiplier (pi/180)
 #define RAD2DEG 57.29577951308232      // numpy rad2deg multiplier (180/pi)
 
@@ -450,8 +502,10 @@ __device__ __forceinline__ void sensor_noise(const RolloutArgs& a, size_t traj, 
 }
 
 // reset(): initialize(), one zero-command step returns the initial state (phlabenv.py:401-428). obs = [0,0,0,p,q,r,alpha]
-template <bool STAB = false>
-static __device__ void env_reset(Env& e, const RolloutArgs& a, int env, float* obs, size_t traj = 0)
+// GUST names the same plant_step instance as env_step<STAB, GUST> (call 0 has no gust stage either way), so a kernel
+// carries one copy of the step code.
+template <bool STAB = false, bool GUST = false>
+static __device__ __forceinline__ void env_reset(Env& e, const RolloutArgs& a, int env, float* obs, size_t traj = 0)
 {
     const double* ic = plant_ic(a.env_mode[env] & 0xff);
 #pragma unroll
@@ -464,13 +518,13 @@ static __device__ void env_reset(Env& e, const RolloutArgs& a, int env, float* o
     obs[3] = (float)x0[0]; obs[4] = (float)x0[1]; obs[5] = (float)x0[2]; obs[6] = (float)x0[4];
     double U[3] = {0.0, 0.0, 0.0}, cmd[3];
     apply_fault(e.fault, U, cmd);
-    plant_step<STAB>(e.pv, e.X, cmd, e.tab, a.trace != nullptr, e.pv_post, 0);      // call 0: no gust stage
+    plant_step_env<STAB, GUST>(e, cmd, a.trace != nullptr, 0);      // call 0: no gust stage
     e.t = 0.0; e.ret = 0.0; e.k = 0; e.done = false;
 }
 
 // one CitationEnv.step (phlabenv.py:430-482) + the bookkeeping of Agent.evaluate (agent.py:85-118)
 template <bool STAB = false, bool GUST = false>
-static __device__ void env_step(Env& e, const RolloutArgs& ar, size_t traj, int actor, bool replay, const float* a, float* obs)
+static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, size_t traj, int actor, bool replay, const float* a, float* obs)
 {
     const double bound = 10.0 * DEG2RAD;                       // phlabenv.py:208
     const double max_theta = 60.0 * DEG2RAD, max_phi = 75.0 * DEG2RAD;
@@ -501,7 +555,7 @@ static __device__ void env_step(Env& e, const RolloutArgs& ar, size_t traj, int 
     double xo[12];
 #pragma unroll
     for (int i = 0; i < 12; ++i) xo[i] = e.X[i];
-    plant_step<STAB, GUST>(e.pv, e.X, cmd, e.tab, ar.trace != nullptr, e.pv_post, (e.k + 1) | (GUST && (e.gust & 1) ? PLANT_CALL_GUST | ((e.gust & 2) ? PLANT_CALL_GUST_UP : 0) : 0));
+    plant_step_env<STAB, GUST>(e, cmd, ar.trace != nullptr, (e.k + 1) | (GUST && (e.gust & 1) ? PLANT_CALL_GUST | ((e.gust & 2) ? PLANT_CALL_GUST_UP : 0) : 0));
     sensor_noise(ar, traj, e.k + 1, xo);
 
     const double t = e.t;

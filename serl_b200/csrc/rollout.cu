@@ -333,10 +333,11 @@ rollout_kernel_persist(RolloutArgs ar)
     }
     // segments in the order: head of the last task (published) -> whole tasks -> tail of the first task (continued)
     long long t_cur = t_first + (k0 > 0 ? 1 : 0);
-    // LOCKSTEP: all warps of the CTA take their steps together (one CTA barrier per step).  The step body is ~180 KB of
-    // straight-line code (actor 100 KB, right-hand side 41 KB x 6 calls, integrator, environment); eight warps drifting
-    // through it independently each stream it through the instruction caches on their own, and instruction fetch was the
-    // top stall (no_instruction 27 % of the warp samples).  In lockstep a fetched line serves every warp of the SM.
+    // LOCKSTEP: all warps of the CTA take their steps together (one CTA barrier per step).  The step body is ~155 KB of
+    // code at h = 72 (sm_90a SASS: actor 57 KB + the out-of-line tanh 0.8 KB, right-hand side 41 KB x 6 calls, ode5 step
+    // 16 KB, environment and segment bookkeeping up to 41 KB); eight warps drifting through it independently each stream it
+    // through the instruction caches on their own, and instruction fetch was the top stall (no_instruction 27 % of the warp
+    // samples on B200).  In lockstep a fetched line serves every warp of the SM.
     Env e;
     e.tab = tab;
     e.done = true; e.k = 0;
@@ -440,7 +441,7 @@ rollout_kernel_persist(RolloutArgs ar)
                         const int kk = __ldcg(ar.ho.k + hx);
                         e.k = kk & 0x3fffffff; e.done = ((kk >> 30) & 1) != 0;
                     } else {
-                        env_reset<TABS>(e, ar, env, obs, traj);
+                        env_reset<TABS, GUST>(e, ar, env, obs, traj);
                     }
                 } else {
                     e.done = true; e.k = 0; e.ret = 0.0; e.t = 0.0; e.fault = 0; e.gust = 0; e.pv = pv_base; e.pv_post = nullptr; e.theta_trim = 0.0;
@@ -487,7 +488,7 @@ rollout_kernel_simple(RolloutArgs ar)
     e.tab = plant_tables_blob;
     float obs[7], a[3];
     env_bind(e, ar, env, &plant_pv[0][0], (size_t)actor * ar.n_envs + env);
-    env_reset(e, ar, env, obs, (size_t)actor * ar.n_envs + env);
+    env_reset<false, true>(e, ar, env, obs, (size_t)actor * ar.n_envs + env);
     const size_t traj = (size_t)actor * ar.n_envs + env;
     const bool replay = ar.replay != nullptr && env == ar.replay_env;
     while (!e.done) {
@@ -556,16 +557,16 @@ __global__ void plant_step_kernel(double* __restrict__ X, const double* __restri
 {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    double x[NX], u[3];
+    PlantState x;
 #pragma unroll
-    for (int k = 0; k < NX; ++k) x[k] = X[(size_t)i * NX + k];
-    u[0] = cmd[3 * i]; u[1] = cmd[3 * i + 1]; u[2] = cmd[3 * i + 2];
+    for (int k = 0; k < NX; ++k) x.v[k] = X[(size_t)i * NX + k];
     const int post = (variant[i] >> 16) & 0xff;
-    plant_step<false, true>(plant_pv[variant[i] & 0xff], x, u, plant_tables_blob, false, post ? plant_pv[post] : nullptr,
-                                   (call ? call[i] : 0) | ((variant[i] & SERL_MODE_GUST) ? PLANT_CALL_GUST : 0) |
-                                       ((variant[i] & SERL_MODE_GUST_UP) ? PLANT_CALL_GUST_UP : 0));
+    x = plant_step<false, true>(plant_pv[variant[i] & 0xff], x, cmd[3 * i], cmd[3 * i + 1], cmd[3 * i + 2], plant_tables_blob, false,
+                                post ? plant_pv[post] : nullptr,
+                                (call ? call[i] : 0) | ((variant[i] & SERL_MODE_GUST) ? PLANT_CALL_GUST : 0) |
+                                    ((variant[i] & SERL_MODE_GUST_UP) ? PLANT_CALL_GUST_UP : 0));
 #pragma unroll
-    for (int k = 0; k < NX; ++k) X[(size_t)i * NX + k] = x[k];
+    for (int k = 0; k < NX; ++k) X[(size_t)i * NX + k] = x.v[k];
 }
 
 __global__ void plant_ic_kernel(double* __restrict__ X, const int* __restrict__ variant, int n)
@@ -950,7 +951,9 @@ static int device_sms()
 
 // CTA shape of the persistent kernel: `apc` genome slots x `wps` warps.  A slot's warps fly wps*32 envs of one actor;
 // the estimate below is (rounds of work per slot) x (time of one step with apc*wps resident warps per SM), the latter a
-// linear fit of measurements at 4 and 8 warps (profiles/): a lone warp steps 1.4x faster than one of eight.
+// least-squares fit (ms per 2001-step horizon) of single-round launches at apc x wps = 1x1 .. 2x4 (config 2: pop 50 x 64
+// envs, and pop 64 x 128 envs; H100 SXM, 400 W power limit, SERL_ROLLOUT_APC / SERL_ROLLOUT_WPS): flat from 1 to 4 warps,
+// a lone warp 1.15x faster than one of eight.
 static void choose_shape(int pop, int n_envs, int apc_max, int sms, int* apc_out, int* wps_out)
 {
     double best = 1e300;
@@ -966,7 +969,7 @@ static void choose_shape(int pop, int n_envs, int apc_max, int sms, int* apc_out
             const long long ns = grid * apc;
             const double rounds = nt <= ns ? 1.0 : (double)nt / (double)ns;
             const double lanes = (double)chunks * wps * 32 / n_envs;        // idle-lane overhead of a ragged last chunk
-            const double est = rounds * (13.2 + 0.825 * apc * wps) * (lanes > 1.0 ? 1.0 + 0.2 * (lanes - 1.0) : 1.0);
+            const double est = rounds * (166.5 + 4.1 * apc * wps) * (lanes > 1.0 ? 1.0 + 0.2 * (lanes - 1.0) : 1.0);
             if (est < best - 1e-9) { best = est; *apc_out = apc; *wps_out = wps; }
         }
     }
