@@ -1,4 +1,4 @@
-/* serl_b200 — C-ABI of the B200-native population-rollout + neuro-evolution engine.
+/* serl_b200 — C-ABI of the H100 (sm_90a) population-rollout + neuro-evolution engine.
  *
  * Drop-in boundary for the per-generation fitness hot path of VladGavra98/SERL (paths relative to the
  * reference tree).  All pointers named d_* are DEVICE pointers owned by the caller; `stream` is a

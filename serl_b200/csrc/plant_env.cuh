@@ -467,8 +467,11 @@ __device__ __forceinline__ void apply_fault(int fault, const double* u, double* 
     else if (fault == SERL_FAULT_SE) { const double b = 2.5 * DEG2RAD; c[0] = fmin(fmax(u[0], -b), b); }   // envs/se :73-79
 }
 
-// bind the env's constants (plant variant row, fault shim, reference signals, trim pitch); no dynamics
-__device__ __forceinline__ void env_bind(Env& e, const RolloutArgs& a, int env, const real* pv_base, size_t traj = 0)
+// bind the env's constants (plant variant row, fault shim, reference signals, trim pitch); no dynamics.
+// GUST: the kernel instantiation flies the gust schedule (serl_rollout_desc.flags & SERL_ROLLOUT_GUST).  One without it
+// carries no trace of the feature, so a gust env bound there is reported (SERL_STATUS_GUST_FLAG) instead of flown as nominal.
+template <bool GUST>
+__device__ __forceinline__ void env_bind(Env& e, const RolloutArgs& a, int env, const real* pv_base, size_t traj)
 {
     const int mode = a.env_mode[env];
     const int variant = mode & 0xff;
@@ -483,6 +486,27 @@ __device__ __forceinline__ void env_bind(Env& e, const RolloutArgs& a, int env, 
     double th0 = plant_ic(variant)[7];
     if (a.sensor_noise) th0 += 4.0 * 1e-3 + 3.2 * 1e-5 * (double)a.sensor_noise[traj * (size_t)(a.horizon + 1) * 7 + 6];
     e.theta_trim = th0 * RAD2DEG;
+    if (!GUST && e.gust && a.status) atomicOr(a.status, SERL_STATUS_GUST_FLAG);
+}
+
+// a lane without an env: done from the start, with a zero state and observation (it still takes part in the actor)
+__device__ __forceinline__ void env_idle(Env& e, const RolloutArgs& a, const real* pv_base, float* obs)
+{
+    e.done = true; e.k = 0; e.ret = 0.0; e.t = 0.0; e.fault = 0; e.gust = 0; e.pv = pv_base; e.pv_post = nullptr; e.theta_trim = 0.0;
+    e.ref_lv = a.ref_levels; e.ref_st = a.ref_starts;
+#pragma unroll
+    for (int i = 0; i < NX; ++i) e.X[i] = 0.0;
+#pragma unroll
+    for (int i = 0; i < 7; ++i) obs[i] = 0.f;
+}
+
+// end of a trajectory: return and executed steps.  A NaN action poisons the state at once, so a non-finite return or
+// state raises SERL_STATUS_NONFINITE.
+__device__ __forceinline__ void traj_store(const Env& e, const RolloutArgs& a, size_t traj)
+{
+    a.returns[traj] = e.ret;
+    a.steps[traj] = e.k;
+    if (a.status && !isfinite(e.ret + e.X[3] + e.X[7] + e.X[9])) atomicOr(a.status, SERL_STATUS_NONFINITE);
 }
 
 // sensor-noise shim (envs/noise/citation.py:72-82, same model in envs/gust): every native step() output gets

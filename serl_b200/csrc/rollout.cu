@@ -370,9 +370,7 @@ rollout_kernel_persist(RolloutArgs ar)
                     __syncwarp();
                     if (lane == 0) atomicExch(ar.ho.flag + slot * wps + wslot, 1);
                 } else if (valid) {
-                    ar.returns[traj] = e.ret;
-                    ar.steps[traj] = e.k;
-                    if (ar.status && !isfinite(e.ret + e.X[3] + e.X[7] + e.X[9])) atomicOr(ar.status, SERL_STATUS_NONFINITE);   // NaN actions poison the state at once
+                    traj_store(e, ar, traj);
                 }
                 in_seg = false;
             }
@@ -429,8 +427,7 @@ rollout_kernel_persist(RolloutArgs ar)
                 const int env = valid ? (ar.env_order ? ar.env_order[eslot] : eslot) : 0;
                 traj = (size_t)actor * ar.n_envs + env;
                 if (valid) {
-                    env_bind(e, ar, env, pv_base, traj);
-                    if (!GUST && e.gust && ar.status) atomicOr(ar.status, SERL_STATUS_GUST_FLAG);
+                    env_bind<GUST>(e, ar, env, pv_base, traj);
                     if (from_h) {
                         const long long hx = (slot - 1) * slot_threads + wslot * 32 + lane;
 #pragma unroll
@@ -444,12 +441,7 @@ rollout_kernel_persist(RolloutArgs ar)
                         env_reset<TABS, GUST>(e, ar, env, obs, traj);
                     }
                 } else {
-                    e.done = true; e.k = 0; e.ret = 0.0; e.t = 0.0; e.fault = 0; e.gust = 0; e.pv = pv_base; e.pv_post = nullptr; e.theta_trim = 0.0;
-                    e.ref_lv = ar.ref_levels; e.ref_st = ar.ref_starts;
-#pragma unroll
-                    for (int i = 0; i < NX; ++i) e.X[i] = 0.0;
-#pragma unroll
-                    for (int i = 0; i < 7; ++i) obs[i] = 0.f;
+                    env_idle(e, ar, pv_base, obs);
                 }
                 replay = valid && ar.replay != nullptr && env == ar.replay_env;
                 in_seg = true;
@@ -487,7 +479,7 @@ rollout_kernel_simple(RolloutArgs ar)
     Env e;
     e.tab = plant_tables_blob;
     float obs[7], a[3];
-    env_bind(e, ar, env, &plant_pv[0][0], (size_t)actor * ar.n_envs + env);
+    env_bind<true>(e, ar, env, &plant_pv[0][0], (size_t)actor * ar.n_envs + env);
     env_reset<false, true>(e, ar, env, obs, (size_t)actor * ar.n_envs + env);
     const size_t traj = (size_t)actor * ar.n_envs + env;
     const bool replay = ar.replay != nullptr && env == ar.replay_env;
@@ -495,9 +487,7 @@ rollout_kernel_simple(RolloutArgs ar)
         actor_forward_simple(w, ar.sh, bufA, bufB, tid, 128, obs, a);
         env_step<false, true>(e, ar, traj, actor, replay, a, obs);       // (the gust schedule costs nothing that matters here)
     }
-    ar.returns[traj] = e.ret;
-    ar.steps[traj] = e.k;
-    if (ar.status && !isfinite(e.ret + e.X[3] + e.X[7] + e.X[9])) atomicOr(ar.status, SERL_STATUS_NONFINITE);   // NaN actions poison the state at once
+    traj_store(e, ar, traj);
 }
 
 // ---- Actor.forward for a batch of observations (same device functions as the rollout) --------------------------
@@ -885,7 +875,6 @@ smoothness_fft_kernel(const float* __restrict__ actions, const int* __restrict__
     }
 }
 
-static cudaError_t scratch_get(cudaStream_t s, size_t bytes, void** out, int which);
 extern "C" int serl_smoothness(const float* d_actions, const int32_t* d_steps, int32_t n_traj, int32_t horizon, double dt,
                                double* d_out, void* stream)
 {
@@ -901,7 +890,7 @@ extern "C" int serl_smoothness(const float* d_actions, const int32_t* d_steps, i
         e = cudaFuncSetAttribute(smoothness_fft_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return serl_fail_cuda(e, "cudaFuncSetAttribute(smoothness_fft)");
         void* tabs = nullptr;
-        e = scratch_get((cudaStream_t)stream, (size_t)(FM + FM / 2 + FM) * sizeof(float2), &tabs, 1);
+        e = serl_scratch(SERL_SCRATCH_K6, (cudaStream_t)stream, (size_t)(FM + FM / 2 + FM) * sizeof(float2), &tabs);
         if (e != cudaSuccess) return serl_fail_cuda(e, "smoothness scratch");
         float2* tw_g = (float2*)tabs;
         float2* hf_g = tw_g + FM / 2;
@@ -931,22 +920,24 @@ extern "C" int64_t serl_actor_num_params(const serl_actor_shape* s)
     return S * H + H + L * (H * H + 3 * H) + H * A + A;
 }
 
-static int g_force_simple = -1;
 static int env_int(const char* name)
 {
     const char* v = getenv(name);
     return v ? atoi(v) : 0;
 }
 
-static int device_sms()
+// SERL_ROLLOUT_IMPL=simple: every launch of the uniform actor takes the one-thread-per-env kernels (cross-check)
+static bool force_simple()
 {
-    static int num_sms = 0;
-    if (num_sms == 0) {
-        int dev = 0;
-        cudaGetDevice(&dev);
-        if (cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || num_sms <= 0) num_sms = 132;
-    }
-    return num_sms;
+    static const bool v = [] { const char* s = getenv("SERL_ROLLOUT_IMPL"); return s && strcmp(s, "simple") == 0; }();
+    return v;
+}
+
+// the uniform actors of the PH-LAB attitude task the kernels of this file implement
+static bool actor_shape_ok(const serl_actor_shape& sh)
+{
+    return sh.state_dim == 7 && sh.action_dim == 3 && sh.hidden >= 2 && sh.hidden <= 256 && sh.num_layers >= 0 &&
+           sh.activation >= 0 && sh.activation <= 2;
 }
 
 // CTA shape of the persistent kernel: `apc` genome slots x `wps` warps.  A slot's warps fly wps*32 envs of one actor;
@@ -975,37 +966,11 @@ static void choose_shape(int pop, int n_envs, int apc_max, int sms, int* apc_out
     }
 }
 
-// Scratch of a launch (genomes in the shared-memory layout + hand-over records): one grow-only buffer per (device,
-// stream), kept for the life of the process.  Launches on one stream are ordered, so they can share it; launches on
-// different streams (the Agent's side-stream episodes next to the population rollout) get their own.  No stream-ordered
-// allocator here: growing its pool maps memory, which waits for kernels in flight on OTHER streams.
-#include <map>
-#include <mutex>
-struct ScratchBuf { void* p; size_t bytes; };
-static std::mutex g_scratch_mu;
-static std::map<std::pair<std::pair<int, int>, cudaStream_t>, ScratchBuf> g_scratch;
-static cudaError_t scratch_get(cudaStream_t s, size_t bytes, void** out, int which)      // which: 0 = K1, 1 = K6 tables
-{
-    int dev = 0;
-    cudaGetDevice(&dev);
-    std::lock_guard<std::mutex> lk(g_scratch_mu);
-    ScratchBuf& b = g_scratch[std::make_pair(std::make_pair(dev, which), s)];
-    if (b.bytes < bytes) {
-        if (b.p) { cudaStreamSynchronize(s); cudaFree(b.p); b.p = nullptr; b.bytes = 0; }
-        const size_t want = bytes + bytes / 4;
-        cudaError_t e = cudaMalloc(&b.p, want);
-        if (e != cudaSuccess) return e;
-        b.bytes = want;
-    }
-    *out = b.p;
-    return cudaSuccess;
-}
-
-template <int H, bool TABS, bool GUST = false>
-static cudaError_t launch_persist(RolloutArgs& ar, int apc_max, cudaStream_t s, void** scratch)
+template <int H, bool TABS, bool GUST>
+static cudaError_t launch_persist(RolloutArgs& ar, int apc_max, cudaStream_t s)
 {
     constexpr int TABN2 = (PT_TOTAL + SERL_PLANT_COUNT * PLANT_NPV + 1) & ~1;
-    const int sms = ar.sm_limit > 0 && ar.sm_limit < device_sms() ? ar.sm_limit : device_sms();
+    const int sms = ar.sm_limit > 0 && ar.sm_limit < serl_device_sms() ? ar.sm_limit : serl_device_sms();
     int apc, wps;
     choose_shape(ar.pop, ar.n_envs, apc_max, sms, &apc, &wps);
     static int f_apc = -1, f_wps = -1;       // experiment knobs
@@ -1022,9 +987,10 @@ static cudaError_t launch_persist(RolloutArgs& ar, int apc_max, cudaStream_t s, 
     const size_t wt_bytes = (size_t)ar.pop * ar.P4 * 4;
     const long long hn = ar.n_tasks > ar.n_slots ? ar.n_slots * wps * 32 : 0;
     const size_t ho_bytes = (size_t)hn * (NX * 8 + 8 + 8 + 7 * 4 + 4) + (size_t)(hn / 32) * 4;
-    cudaError_t e = scratch_get(s, wt_bytes + ho_bytes + 512, scratch, 0);
+    void* scratch = nullptr;
+    cudaError_t e = serl_scratch(SERL_SCRATCH_K1, s, wt_bytes + ho_bytes + 512, &scratch);
     if (e != cudaSuccess) return e;
-    unsigned char* base = (unsigned char*)*scratch;
+    unsigned char* base = (unsigned char*)scratch;
     float* wt = (float*)base;
     ar.wt = wt;
     ar.ho.n = hn;
@@ -1051,38 +1017,19 @@ static cudaError_t launch_persist(RolloutArgs& ar, int apc_max, cudaStream_t s, 
     return cudaGetLastError();
 }
 
-static int rollout_impl(const serl_rollout_desc& d, void* stream)
+// K1 launch: the checks only this kernel needs, then the genome part of the argument block and the kernel for the hidden size
+static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t s)
 {
-    const serl_actor_shape* shape = &d.shape;
-    if (!d.d_weights || !d.d_ref_levels || !d.d_ref_starts || !d.d_env_mode || !d.d_returns || !d.d_steps)
-        return serl_fail(SERL_ERR_ARG, "serl_rollout: null pointer argument");
-    if (d.pop <= 0 || d.n_envs <= 0 || d.horizon <= 0) return serl_fail(SERL_ERR_ARG, "serl_rollout: pop, n_envs, horizon must be > 0");
-    if (d.pop > 65535) return serl_fail(SERL_ERR_ARG, "serl_rollout: pop must be <= 65535 per call");
-    if (shape->state_dim != 7 || shape->action_dim != 3)
-        return serl_fail(SERL_ERR_ARG, "serl_rollout: PH-LAB attitude task needs state_dim=7, action_dim=3");
-    if (shape->hidden < 2 || shape->hidden > 256 || shape->num_layers < 0 || shape->activation < 0 || shape->activation > 2)
-        return serl_fail(SERL_ERR_ARG, "serl_rollout: unsupported actor shape");
-    if (d.d_replay && (d.replay_env < 0 || d.replay_env >= d.n_envs)) return serl_fail(SERL_ERR_ARG, "serl_rollout: replay_env out of range");
-    if (d.horizon >= (1 << 30)) return serl_fail(SERL_ERR_ARG, "serl_rollout: horizon too long");
-    if (g_force_simple < 0) {
-        const char* v = getenv("SERL_ROLLOUT_IMPL");
-        g_force_simple = (v && strcmp(v, "simple") == 0) ? 1 : 0;
-    }
-    cudaStream_t s = (cudaStream_t)stream;
-    RolloutArgs ar;
-    memset(&ar, 0, sizeof(ar));
-    ar.weights = d.d_weights; ar.P = (int)serl_actor_num_params(shape); ar.sh = *shape;
-    ar.ref_levels = d.d_ref_levels; ar.ref_starts = d.d_ref_starts; ar.env_mode = d.d_env_mode; ar.n_envs = d.n_envs; ar.horizon = d.horizon;
-    ar.action_noise = d.d_action_noise; ar.returns = d.d_returns; ar.steps = d.d_steps; ar.trace = d.d_trace; ar.actions = d.d_actions;
-    ar.pop = d.pop;
-    ar.t_max = d.t_max > 0.0 ? d.t_max : 20.0;
-    ar.smooth_w = d.t_max > 0.0 ? d.smooth_width : 3.0;
-    ar.env_order = d.d_env_order; ar.replay = d.d_replay; ar.replay_env = d.replay_env; ar.status = d.d_status; ar.sm_limit = d.sm_limit; ar.sensor_noise = d.d_sensor_noise;
+    if (!actor_shape_ok(d.shape))
+        return serl_fail(SERL_ERR_ARG, "serl_rollout: unsupported actor shape (state_dim = 7, action_dim = 3, 2 <= hidden <= 256)");
+    if (d.pop > 65535) return serl_fail(SERL_ERR_ARG, "serl_rollout: pop must be <= 65535 per call");       // grid.y of the simple kernel
+    if (d.horizon >= (1 << 30)) return serl_fail(SERL_ERR_ARG, "serl_rollout: horizon too long");        // Handoff.k: steps | done << 30
+    const int H = d.shape.hidden;
+    ar.weights = d.d_weights; ar.P = (int)serl_actor_num_params(&d.shape); ar.sh = d.shape;
     ar.P4 = (ar.P + 3) & ~3;
-    const int H = shape->hidden;
     cudaError_t e;
     const size_t tab_bytes = (size_t)((PT_TOTAL + SERL_PLANT_COUNT * PLANT_NPV + 1) & ~1) * sizeof(real);
-    const bool warp_ok = !g_force_simple && (H == 32 || H == 64 || H == 72 || H == 96 || H == 128) && (size_t)ar.P4 * 4 <= 227 * 1024;
+    const bool warp_ok = !force_simple() && (H == 32 || H == 64 || H == 72 || H == 96 || H == 128) && (size_t)ar.P4 * 4 <= 227 * 1024;
     if (warp_ok) {
         // as many genome slots per CTA as shared memory holds next to the plant tables (h <= 72: two; h = 96: one);
         // h = 128 (207 KB genome) reads the tables through L1 instead
@@ -1091,9 +1038,8 @@ static int rollout_impl(const serl_rollout_desc& d, void* stream)
         int apc_max = (int)(((tabs ? budget - tab_bytes : budget)) / ((size_t)ar.P4 * 4));
         if (apc_max > 4) apc_max = 4;
         if (apc_max > 2 && H > 32) apc_max = 2;
-        void* scratch = nullptr;
         const bool gust = (d.flags & SERL_ROLLOUT_GUST) != 0;
-#define K1_LAUNCH(HH, TT) (gust ? launch_persist<HH, TT, true>(ar, apc_max, s, &scratch) : launch_persist<HH, TT, false>(ar, apc_max, s, &scratch))
+#define K1_LAUNCH(HH, TT) (gust ? launch_persist<HH, TT, true>(ar, apc_max, s) : launch_persist<HH, TT, false>(ar, apc_max, s))
         if (H == 32) e = K1_LAUNCH(32, true);
         else if (H == 64) e = K1_LAUNCH(64, true);
         else if (H == 72) e = K1_LAUNCH(72, true);
@@ -1111,34 +1057,54 @@ static int rollout_impl(const serl_rollout_desc& d, void* stream)
         e = cudaGetLastError();
     }
     if (e != cudaSuccess) return serl_fail_cuda(e, "rollout_kernel launch");
-    if (d.d_fitness) {
-        fitness_mean_kernel<<<(d.pop + 127) / 128, 128, 0, s>>>(d.d_returns, d.pop, d.n_envs, d.d_fitness);
-        serl_count_launch();
-        e = cudaGetLastError();
-        if (e != cudaSuccess) return serl_fail_cuda(e, "fitness_mean_kernel launch");
-    }
     return SERL_OK;
 }
 
-int rollout_tc_impl(const serl_rollout_desc& d, const int32_t* widths, int n_widths, void* stream);     // rollout_tc.cu
+int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, cudaStream_t s);     // rollout_tc.cu
 
+// the checks of a launch description that hold for both kernels
+static int check_desc(const serl_rollout_desc& d)
+{
+    if (!d.d_weights || !d.d_ref_levels || !d.d_ref_starts || !d.d_env_mode || !d.d_returns || !d.d_steps)
+        return serl_fail(SERL_ERR_ARG, "serl_rollout: null pointer argument");
+    if (d.pop <= 0 || d.n_envs <= 0 || d.horizon <= 0) return serl_fail(SERL_ERR_ARG, "serl_rollout: pop, n_envs, horizon must be > 0");
+    if (d.shape.activation < 0 || d.shape.activation > 2) return serl_fail(SERL_ERR_ARG, "serl_rollout: unsupported activation");
+    if (d.d_replay && (d.replay_env < 0 || d.replay_env >= d.n_envs)) return serl_fail(SERL_ERR_ARG, "serl_rollout: replay_env out of range");
+    if (d.t_max > 0.0 && !(d.smooth_width > 0.0)) return serl_fail(SERL_ERR_ARG, "serl_rollout: smooth_width must be > 0");
+    if (d.n_widths > 0 && !d.widths) return serl_fail(SERL_ERR_ARG, "serl_rollout: n_widths > 0 but widths is null");
+    return SERL_OK;
+}
+
+// the env / output part of the argument block, the same for both kernels; t_max <= 0 selects the training episode
+static RolloutArgs rollout_args(const serl_rollout_desc& d)
+{
+    RolloutArgs ar;
+    memset(&ar, 0, sizeof(ar));
+    ar.ref_levels = d.d_ref_levels; ar.ref_starts = d.d_ref_starts; ar.env_mode = d.d_env_mode; ar.n_envs = d.n_envs; ar.horizon = d.horizon;
+    ar.action_noise = d.d_action_noise; ar.returns = d.d_returns; ar.steps = d.d_steps; ar.trace = d.d_trace; ar.actions = d.d_actions;
+    ar.pop = d.pop;
+    ar.t_max = d.t_max > 0.0 ? d.t_max : 20.0;
+    ar.smooth_w = d.t_max > 0.0 ? d.smooth_width : 3.0;
+    ar.env_order = d.d_env_order; ar.replay = d.d_replay; ar.replay_env = d.replay_env; ar.status = d.d_status; ar.sm_limit = d.sm_limit;
+    ar.sensor_noise = d.d_sensor_noise;
+    return ar;
+}
+
+// Every population rollout comes through here: the shared checks, the kernel of the actor form (widths: K1-TC, else K1),
+// whose own checks also come before any CUDA call, then the per-actor fitness.
 extern "C" int serl_rollout_run(const serl_rollout_desc* desc, void* stream)
 {
     if (!desc) return serl_fail(SERL_ERR_ARG, "serl_rollout_run: null descriptor");
-    if (desc->t_max > 0.0 && !(desc->smooth_width > 0.0)) return serl_fail(SERL_ERR_ARG, "serl_rollout_run: smooth_width must be > 0");
-    if (desc->n_widths > 0) {
-        if (!desc->widths) return serl_fail(SERL_ERR_ARG, "serl_rollout_run: n_widths > 0 but widths is null");
-        const int rc = rollout_tc_impl(*desc, desc->widths, desc->n_widths, stream);
-        if (rc != SERL_OK) return rc;
-        if (desc->d_fitness) {
-            fitness_mean_kernel<<<(desc->pop + 127) / 128, 128, 0, (cudaStream_t)stream>>>(desc->d_returns, desc->pop, desc->n_envs, desc->d_fitness);
-            serl_count_launch();
-            cudaError_t e = cudaGetLastError();
-            if (e != cudaSuccess) return serl_fail_cuda(e, "fitness_mean_kernel launch");
-        }
-        return SERL_OK;
-    }
-    return rollout_impl(*desc, stream);
+    const serl_rollout_desc& d = *desc;
+    int rc = check_desc(d);
+    if (rc != SERL_OK) return rc;
+    cudaStream_t s = (cudaStream_t)stream;
+    rc = d.n_widths > 0 ? rollout_tc_impl(d, rollout_args(d), s) : rollout_impl(d, rollout_args(d), s);
+    if (rc != SERL_OK || !d.d_fitness) return rc;
+    fitness_mean_kernel<<<(d.pop + 127) / 128, 128, 0, s>>>(d.d_returns, d.pop, d.n_envs, d.d_fitness);
+    serl_count_launch();
+    const cudaError_t e = cudaGetLastError();
+    return e == cudaSuccess ? SERL_OK : serl_fail_cuda(e, "fitness_mean_kernel launch");
 }
 
 static serl_rollout_desc make_desc(const float* d_weights, int32_t pop, const serl_actor_shape* shape,
@@ -1148,7 +1114,7 @@ static serl_rollout_desc make_desc(const float* d_weights, int32_t pop, const se
 {
     serl_rollout_desc d;
     memset(&d, 0, sizeof(d));
-    d.d_weights = d_weights; d.pop = pop; if (shape) d.shape = *shape;
+    d.d_weights = d_weights; d.pop = pop; d.shape = *shape;
     d.d_ref_levels = d_ref_levels; d.d_ref_starts = d_ref_starts; d.d_env_mode = d_env_mode; d.n_envs = n_envs; d.horizon = horizon;
     d.d_action_noise = d_action_noise; d.d_returns = d_returns; d.d_steps = d_steps; d.d_fitness = d_fitness; d.d_trace = d_trace;
     d.d_actions = d_actions;
@@ -1161,8 +1127,9 @@ extern "C" int serl_rollout(const float* d_weights, int32_t pop, const serl_acto
                             double* d_returns, int32_t* d_steps, double* d_fitness, double* d_trace, float* d_actions, void* stream)
 {
     if (!shape) return serl_fail(SERL_ERR_ARG, "serl_rollout: null pointer argument");
-    return rollout_impl(make_desc(d_weights, pop, shape, d_ref_levels, d_ref_starts, d_env_mode, n_envs, horizon, d_action_noise,
-                                  d_returns, d_steps, d_fitness, d_trace, d_actions), stream);
+    const serl_rollout_desc d = make_desc(d_weights, pop, shape, d_ref_levels, d_ref_starts, d_env_mode, n_envs, horizon, d_action_noise,
+                                          d_returns, d_steps, d_fitness, d_trace, d_actions);
+    return serl_rollout_run(&d, stream);
 }
 
 extern "C" int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shape* shape,
@@ -1176,16 +1143,14 @@ extern "C" int serl_rollout_eval(const float* d_weights, int32_t pop, const serl
     serl_rollout_desc d = make_desc(d_weights, pop, shape, d_ref_levels, d_ref_starts, d_env_mode, n_envs, horizon, d_action_noise,
                                     d_returns, d_steps, d_fitness, d_trace, d_actions);
     d.t_max = t_max; d.smooth_width = smooth_width;
-    return rollout_impl(d, stream);
+    return serl_rollout_run(&d, stream);
 }
 
 extern "C" int serl_actor_forward(const float* d_genome, const serl_actor_shape* shape, const float* d_obs, int32_t n,
                                   float* d_actions, void* stream)
 {
     if (!d_genome || !shape || !d_obs || !d_actions || n <= 0) return serl_fail(SERL_ERR_ARG, "serl_actor_forward: bad argument");
-    if (shape->state_dim != 7 || shape->action_dim != 3 || shape->hidden < 2 || shape->hidden > 256 || shape->num_layers < 0 ||
-        shape->activation < 0 || shape->activation > 2)
-        return serl_fail(SERL_ERR_ARG, "serl_actor_forward: unsupported actor shape");
+    if (!actor_shape_ok(*shape)) return serl_fail(SERL_ERR_ARG, "serl_actor_forward: unsupported actor shape");
     cudaStream_t s = (cudaStream_t)stream;
     const int P = (int)serl_actor_num_params(shape), H = shape->hidden;
     const int grid = (n + 127) / 128;
@@ -1193,15 +1158,12 @@ extern "C" int serl_actor_forward(const float* d_genome, const serl_actor_shape*
     const size_t smem = (size_t)((P + 3) & ~3) * 4;
 #define AF_LAUNCH(HH) do { e = cudaFuncSetAttribute(actor_forward_kernel<HH>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
         if (e == cudaSuccess) { actor_forward_kernel<HH><<<grid, 128, smem, s>>>(d_genome, P, *shape, d_obs, n, d_actions); e = cudaGetLastError(); } } while (0)
-    if (g_force_simple < 0) {
-        const char* v = getenv("SERL_ROLLOUT_IMPL");
-        g_force_simple = (v && strcmp(v, "simple") == 0) ? 1 : 0;
-    }
-    if (!g_force_simple && H == 32) AF_LAUNCH(32);
-    else if (!g_force_simple && H == 64) AF_LAUNCH(64);
-    else if (!g_force_simple && H == 72) AF_LAUNCH(72);
-    else if (!g_force_simple && H == 96) AF_LAUNCH(96);
-    else if (!g_force_simple && H == 128) AF_LAUNCH(128);
+    const bool warp = !force_simple();
+    if (warp && H == 32) AF_LAUNCH(32);
+    else if (warp && H == 64) AF_LAUNCH(64);
+    else if (warp && H == 72) AF_LAUNCH(72);
+    else if (warp && H == 96) AF_LAUNCH(96);
+    else if (warp && H == 128) AF_LAUNCH(128);
     else {
         const size_t sm2 = smem + 2ull * H * 128 * 4;
         if (sm2 > 227 * 1024) return serl_fail(SERL_ERR_UNSUPPORTED, "serl_actor_forward: genome + activations exceed shared memory");

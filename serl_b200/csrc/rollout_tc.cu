@@ -370,7 +370,9 @@ __device__ __forceinline__ void tc_load_small(TcCtx& c, const TcArgs& ar, int ac
     group_sync(c.grp);
 }
 
-template <int ACT>
+// GUST as in rollout_kernel_persist: the launch has envs of the gust build, and reset and step share the one plant_step
+// instance of the kernel; without it a gust env raises SERL_STATUS_GUST_FLAG
+template <int ACT, bool GUST>
 __global__ void __launch_bounds__(2 * TC_THREADS, 1)
 rollout_kernel_tc(TcArgs ar)
 {
@@ -383,9 +385,6 @@ rollout_kernel_tc(TcArgs ar)
     const RolloutArgs& r = ar.r;
     const real* tab = reinterpret_cast<const real*>(smem_raw);
     const real* pv_base = tab + PT_TOTAL;
-    int gust_mine = 0;
-    for (int i = threadIdx.x; i < r.n_envs; i += blockDim.x) gust_mine |= r.env_mode[i] & SERL_MODE_GUST;
-    const bool any_gust = __syncthreads_or(gust_mine) != 0;      // does any env of the launch fly the gust build?
     const int tid = c.gtid;
     const int n_stages = ar.w1 / TC_KSLAB;
     // the two groups of a CTA run independent task loops
@@ -400,30 +399,18 @@ rollout_kernel_tc(TcArgs ar)
         e.tab = tab;
         float obs[7], a[3];
         if (valid) {
-            env_bind(e, r, env, pv_base, (size_t)actor * r.n_envs + env);
-            env_reset<true>(e, r, env, obs, (size_t)actor * r.n_envs + env);
+            env_bind<GUST>(e, r, env, pv_base, (size_t)actor * r.n_envs + env);
+            env_reset<true, GUST>(e, r, env, obs, (size_t)actor * r.n_envs + env);
         } else {
-            e.done = true; e.k = 0; e.ret = 0.0; e.t = 0.0; e.fault = 0; e.gust = 0; e.pv = pv_base; e.pv_post = nullptr; e.theta_trim = 0.0;
-            e.ref_lv = r.ref_levels; e.ref_st = r.ref_starts;
-#pragma unroll
-            for (int i = 0; i < NX; ++i) e.X[i] = 0.0;
-#pragma unroll
-            for (int i = 0; i < 7; ++i) obs[i] = 0.f;
+            env_idle(e, r, pv_base, obs);
         }
         const size_t traj = (size_t)actor * r.n_envs + env;
         const bool replay = valid && r.replay != nullptr && env == r.replay_env;
         while (group_any(c.grp, !e.done)) {
             tc_actor_forward<ACT>(c, ar, tiles_actor, obs, a);
-            if (!e.done) {
-                if (any_gust) env_step<true, true>(e, r, traj, actor, replay, a, obs);
-                else env_step<true>(e, r, traj, actor, replay, a, obs);
-            }
+            if (!e.done) env_step<true, GUST>(e, r, traj, actor, replay, a, obs);
         }
-        if (valid) {
-            r.returns[traj] = e.ret;
-            r.steps[traj] = e.k;
-            if (r.status && !isfinite(e.ret + e.X[3] + e.X[7] + e.X[9])) atomicOr(r.status, SERL_STATUS_NONFINITE);
-        }
+        if (valid) traj_store(e, r, traj);
     }
 }
 
@@ -450,26 +437,6 @@ actor_forward_tc_kernel(TcArgs ar)
 }
 
 // ---- host side ------------------------------------------------------------------------------------------------
-#include <map>
-#include <mutex>
-static std::mutex g_tc_mu;
-static std::map<std::pair<int, cudaStream_t>, std::pair<void*, size_t>> g_tc_scratch;
-static cudaError_t tc_scratch_get(cudaStream_t s, size_t bytes, void** out)
-{
-    int dev = 0;
-    cudaGetDevice(&dev);
-    std::lock_guard<std::mutex> lk(g_tc_mu);
-    auto& b = g_tc_scratch[std::make_pair(dev, s)];
-    if (b.second < bytes) {
-        if (b.first) { cudaStreamSynchronize(s); cudaFree(b.first); b.first = nullptr; b.second = 0; }
-        cudaError_t e = cudaMalloc(&b.first, bytes + bytes / 8);
-        if (e != cudaSuccess) return e;
-        b.second = bytes + bytes / 8;
-    }
-    *out = b.first;
-    return cudaSuccess;
-}
-
 extern "C" int64_t serl_actor_num_params_wide(const int32_t* widths, int32_t n_widths)
 {
     if (!widths || n_widths < 1) return -1;
@@ -478,14 +445,8 @@ extern "C" int64_t serl_actor_num_params_wide(const int32_t* widths, int32_t n_w
     return P + 3 * (int64_t)widths[n_widths - 1] + 3;
 }
 
-static int device_sms()
-{
-    int sms = 0, dev = 0;
-    cudaGetDevice(&dev);
-    if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 132;
-    return sms;
-}
-
+// Checks the widths and sizes the kernel's buffers (all before any CUDA call), then brings the genomes into the kernel
+// layout (K0-TC) in the stream's scratch buffer.
 static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t* widths, int n_widths, cudaStream_t s, size_t* smem_out)
 {
     if (n_widths != 2) return serl_fail(SERL_ERR_UNSUPPORTED, "wide actors: the tensor-core path implements two hidden layers [w1, w2]");
@@ -497,12 +458,16 @@ static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t
     ar.w2 = w2; ar.n2pad = (w2 + TC_NCH - 1) / TC_NCH * TC_NCH;
     ar.small_floats = (tc_small_floats(ar.w1, ar.n2pad) + 3) & ~3;
     ar.stage_floats = 2 * TC_CH * ar.n2pad * 4;
+    constexpr int A_STAGE_FLOATS = 2 * TC_CH * TC_M * 4;
+    *smem_out = (size_t)TC_TABN2 * sizeof(real) +
+                (size_t)(2 * ((ar.small_floats + 31) & ~31) + 2 * TC_IO_FLOATS + TC_STAGES * A_STAGE_FLOATS + TC_STAGES * ar.stage_floats) * 4;
+    if (*smem_out > 227 * 1024 - 256) return serl_fail(SERL_ERR_UNSUPPORTED, "wide actors: tables + parameters + rings exceed the shared memory of an SM");
     const int P = (int)serl_actor_num_params_wide(widths, n_widths);
     const int n_stages = ar.w1 / TC_KSLAB;
     const size_t small_bytes = (size_t)pop * ar.small_floats * 4;
     const size_t tile_bytes = (size_t)pop * n_stages * ar.stage_floats * 4;
     void* scratch = nullptr;
-    cudaError_t e = tc_scratch_get(s, ((small_bytes + 255) & ~(size_t)255) + tile_bytes + 256, &scratch);
+    cudaError_t e = serl_scratch(SERL_SCRATCH_TC, s, ((small_bytes + 255) & ~(size_t)255) + tile_bytes + 256, &scratch);
     if (e != cudaSuccess) return serl_fail_cuda(e, "wide actors: scratch allocation");
     float* small = (float*)scratch;
     float* tiles = (float*)((unsigned char*)scratch + ((small_bytes + 255) & ~(size_t)255));
@@ -511,47 +476,40 @@ static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t
     const int grid = (int)((total + 255) / 256 < 8192 ? (total + 255) / 256 : 8192);
     tc_layout_kernel<<<grid, 256, 0, s>>>(d_weights, pop, P, ar.w1, w1, w2, ar.n2pad, ar.small_floats, ar.stage_floats, small, tiles);
     serl_count_launch();
-    constexpr int A_STAGE_FLOATS = 2 * TC_CH * TC_M * 4;
-    *smem_out = (size_t)TC_TABN2 * sizeof(real) +
-                (size_t)(2 * ((ar.small_floats + 31) & ~31) + 2 * TC_IO_FLOATS + TC_STAGES * A_STAGE_FLOATS + TC_STAGES * ar.stage_floats) * 4;
-    if (*smem_out > 227 * 1024 - 256) return serl_fail(SERL_ERR_UNSUPPORTED, "wide actors: tables + parameters + rings exceed the shared memory of an SM");
     return SERL_OK;
 }
 
-int rollout_tc_impl(const serl_rollout_desc& d, const int32_t* widths, int n_widths, void* stream)
+// one CTA = the two groups of TC_THREADS threads
+static cudaError_t tc_launch(void (*kernel)(TcArgs), const TcArgs& ar, unsigned grid, size_t smem, cudaStream_t s)
 {
-    if (!d.d_weights || !d.d_ref_levels || !d.d_ref_starts || !d.d_env_mode || !d.d_returns || !d.d_steps)
-        return serl_fail(SERL_ERR_ARG, "serl_rollout: null pointer argument");
-    if (d.pop <= 0 || d.n_envs <= 0 || d.horizon <= 0) return serl_fail(SERL_ERR_ARG, "serl_rollout: pop, n_envs, horizon must be > 0");
-    if (d.shape.activation < 0 || d.shape.activation > 2) return serl_fail(SERL_ERR_ARG, "serl_rollout: unsupported activation");
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    kernel<<<grid, 2 * TC_THREADS, smem, s>>>(ar);
+    serl_count_launch();
+    return cudaGetLastError();
+}
+
+// K1-TC launch (serl_rollout_run has checked the descriptor and built the env / output arguments `r`)
+int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, cudaStream_t s)
+{
     if (d.d_trace) return serl_fail(SERL_ERR_UNSUPPORTED, "wide actors: per-step traces are not produced by the tensor-core kernel");
-    cudaStream_t s = (cudaStream_t)stream;
     TcArgs ar;
     memset(&ar, 0, sizeof(ar));
-    RolloutArgs& r = ar.r;
-    r.ref_levels = d.d_ref_levels; r.ref_starts = d.d_ref_starts; r.env_mode = d.d_env_mode; r.n_envs = d.n_envs; r.horizon = d.horizon;
-    r.action_noise = d.d_action_noise; r.returns = d.d_returns; r.steps = d.d_steps; r.actions = d.d_actions; r.pop = d.pop;
-    r.t_max = d.t_max > 0.0 ? d.t_max : 20.0;
-    r.smooth_w = d.t_max > 0.0 ? d.smooth_width : 3.0;
-    r.env_order = d.d_env_order; r.replay = d.d_replay; r.replay_env = d.replay_env; r.status = d.d_status; r.sensor_noise = d.d_sensor_noise;
+    ar.r = r;
     size_t smem = 0;
-    int rc = tc_prepare(ar, d.d_weights, d.pop, widths, n_widths, s, &smem);
+    const int rc = tc_prepare(ar, d.d_weights, d.pop, d.widths, d.n_widths, s, &smem);
     if (rc != SERL_OK) return rc;
     ar.n_chunks = (d.n_envs + TC_THREADS - 1) / TC_THREADS;
     ar.n_tasks = (long long)d.pop * ar.n_chunks;
-    int sms = device_sms();
+    int sms = serl_device_sms();
     if (d.sm_limit > 0 && d.sm_limit < sms) sms = d.sm_limit;
     const long long grid = (ar.n_tasks + 1) / 2 < sms ? (ar.n_tasks + 1) / 2 : sms;
-    cudaError_t e;
-#define TC_LAUNCH(A) do { e = cudaFuncSetAttribute(rollout_kernel_tc<A>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        if (e == cudaSuccess) { rollout_kernel_tc<A><<<(unsigned)grid, 2 * TC_THREADS, smem, s>>>(ar); e = cudaGetLastError(); } } while (0)
-    if (d.shape.activation == SERL_ACT_TANH) TC_LAUNCH(SERL_ACT_TANH);
-    else if (d.shape.activation == SERL_ACT_ELU) TC_LAUNCH(SERL_ACT_ELU);
-    else TC_LAUNCH(SERL_ACT_LEAKY_RELU);
-#undef TC_LAUNCH
-    serl_count_launch();
-    if (e != cudaSuccess) return serl_fail_cuda(e, "rollout_kernel_tc launch");
-    return SERL_OK;
+    static void (*const kernels[3][2])(TcArgs) = {          // [SERL_ACT_*][gust]
+        {rollout_kernel_tc<SERL_ACT_TANH, false>, rollout_kernel_tc<SERL_ACT_TANH, true>},
+        {rollout_kernel_tc<SERL_ACT_ELU, false>, rollout_kernel_tc<SERL_ACT_ELU, true>},
+        {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true>}};
+    const cudaError_t e = tc_launch(kernels[d.shape.activation][(d.flags & SERL_ROLLOUT_GUST) != 0], ar, (unsigned)grid, smem, s);
+    return e == cudaSuccess ? SERL_OK : serl_fail_cuda(e, "rollout_kernel_tc launch");
 }
 
 extern "C" int serl_actor_forward_wide(const float* d_genome, const int32_t* widths, int32_t n_widths, int32_t activation,
@@ -567,15 +525,10 @@ extern "C" int serl_actor_forward_wide(const float* d_genome, const int32_t* wid
     if (rc != SERL_OK) return rc;
     ar.obs_in = d_obs; ar.act_out = d_actions; ar.n_obs = n;
     const int blocks = (n + 2 * TC_THREADS - 1) / (2 * TC_THREADS);
-    const int sms = device_sms();
+    const int sms = serl_device_sms();
     const int grid = blocks < sms ? blocks : sms;
-    cudaError_t e;
-#define TC_LAUNCH(A) do { e = cudaFuncSetAttribute(actor_forward_tc_kernel<A>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem); \
-        if (e == cudaSuccess) { actor_forward_tc_kernel<A><<<grid, 2 * TC_THREADS, smem, s>>>(ar); e = cudaGetLastError(); } } while (0)
-    if (activation == SERL_ACT_TANH) TC_LAUNCH(SERL_ACT_TANH);
-    else if (activation == SERL_ACT_ELU) TC_LAUNCH(SERL_ACT_ELU);
-    else TC_LAUNCH(SERL_ACT_LEAKY_RELU);
-#undef TC_LAUNCH
-    serl_count_launch();
+    static void (*const kernels[3])(TcArgs) = {actor_forward_tc_kernel<SERL_ACT_TANH>, actor_forward_tc_kernel<SERL_ACT_ELU>,
+                                               actor_forward_tc_kernel<SERL_ACT_LEAKY_RELU>};      // [SERL_ACT_*]
+    const cudaError_t e = tc_launch(kernels[activation], ar, (unsigned)grid, smem, s);
     return e == cudaSuccess ? SERL_OK : serl_fail_cuda(e, "actor_forward_tc_kernel");
 }

@@ -42,6 +42,32 @@ def test_compute_fails_loudly_without_cuda():
                                    torch.zeros(1, dtype=torch.int32))
 
 
+@pytest.mark.parametrize('widths', [None, [128, 128]])
+def test_rollout_run_rejects_a_bad_descriptor_before_any_cuda_call(widths):
+    """Both kernels (K1 and, with widths, K1-TC) go through the same checks; the device pointers are never dereferenced."""
+    from serl_b200 import build, _native, rollout
+    build.build()
+    L = _native.lib()
+    warr = (ctypes.c_int32 * 2)(*(widths or [0, 0]))
+
+    def run(**kw):
+        d = _native.RolloutDesc()
+        fake = iter(range(0x10000, 0x100000, 0x1000))      # non-null, never read
+        for f in ('d_weights', 'd_ref_levels', 'd_ref_starts', 'd_env_mode', 'd_returns', 'd_steps', 'd_fitness', 'd_replay', 'd_status'):
+            setattr(d, f, next(fake))
+        d.pop, d.shape, d.n_envs, d.horizon, d.replay_env = 4, rollout.actor_shape(72), 8, 100, 0
+        if widths:
+            d.widths, d.n_widths = ctypes.cast(warr, ctypes.c_void_p), 2
+        for k, v in kw.items():
+            setattr(d, k, v)
+        return L.serl_rollout_run(ctypes.byref(d), None), L.serl_last_error().decode()
+
+    rc, msg = run(replay_env=8)
+    assert rc == -1 and 'replay_env' in msg, (rc, msg)
+    assert run(pop=0)[0] == -1
+    assert run(shape=_native.ActorShape(7, 3, 72, 3, 5))[0] == -1          # activation 5
+
+
 def test_ctypes_mirror_of_the_rollout_descriptor_matches_the_header(tmp_path):
     """serl_b200/_native.py RolloutDesc / ActorShape vs include/serl_b200.h: same size and same field offsets (gcc)."""
     import subprocess

@@ -86,3 +86,36 @@ def test_config5_shape_many_ctas_deterministic():
         assert np.isfinite(ret).all() and (r.steps.cpu().numpy() == 40).all()
         for a in range(3, 360):
             assert np.array_equal(ret[a], ret[a % 3]), a
+
+
+def test_gust_schedule_of_the_tensor_core_kernel_matches_k1():
+    """K1-TC takes the gust instantiation from the launch's flag, as K1 does.  A [128, 128] genome has the parameters() layout of
+    K1's hidden = 128, num_layers = 1 actor; with zero output weights both kernels emit the same constant action am_tanh1(bo), and
+    the env / plant code they share must then give the same bits through the 20-23 s pulse."""
+    from serl_b200 import rollout
+    dev = torch.device('cuda:0')
+    g = wide_genomes(1, [128, 128], 'tanh', 3)[0]
+    g[-3 - 3 * 128:-3] = 0.0
+    g[-3:] = [0.02, -0.01, 0.01]
+    w = torch.as_tensor(g[None], device=dev)
+    modes = ['gust', 'test', 'nominal', 'cg-timed', 'gust', 'nominal']
+    lv, st = refsig.make_ref_params(len(modes), seed_base=77, t_max=25)
+    lv, st = torch.as_tensor(lv, device=dev), torch.as_tensor(st, device=dev)
+    md = torch.as_tensor(np.array([rollout.mode_code(m) for m in modes], dtype=np.int32), device=dev)
+    run = lambda shape, widths, gust: rollout.population_rollout(w, shape, lv, st, md, horizon=2501, t_max=25.0, widths=widths, gust=gust)
+    k1 = run(rollout.actor_shape(128, 1, 'tanh'), None, True)
+    tc = run(rollout.actor_shape(72), [128, 128], True)
+    torch.cuda.synchronize()
+    k1.check()
+    tc.check()
+    assert torch.equal(tc.steps, k1.steps), (tc.steps, k1.steps)
+    assert torch.equal(tc.returns, k1.returns), (tc.returns, k1.returns)
+    steps, ret = tc.steps.cpu().numpy()[0], tc.returns.cpu().numpy()[0]
+    gust = np.array([m in ('gust', 'test') for m in modes])
+    assert (steps[gust] > 2301).all(), steps                     # flown through the whole pulse
+    # without the flag the gust envs fly the nominal dynamics, and that is reported
+    nominal = run(rollout.actor_shape(72), [128, 128], False)
+    torch.cuda.synchronize()
+    assert (ret[gust] != nominal.returns.cpu().numpy()[0][gust]).all()      # the pulse was really on
+    with pytest.raises(Exception, match='gust'):
+        nominal.check()
