@@ -11,5 +11,5 @@ r = rollout.population_rollout(w, rollout.actor_shape(72), torch.as_tensor(lv, d
 for i in range(3):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record(); sm = rollout.smoothness(r.actions, r.steps); e1.record(); torch.cuda.synchronize()
-    print('K6 %s: %.2f ms for %d trajectories' % (os.environ.get('SERL_SMOOTHNESS_IMPL', 'fft'), e0.elapsed_time(e1), r.steps.numel()))
+    print('K6: %.2f ms for %d trajectories' % (e0.elapsed_time(e1), r.steps.numel()))
 print('mean smoothness', float(sm.mean()))

@@ -1,5 +1,5 @@
 """`Episode` (the record Agent.evaluate returns, base/core/utils.py:12-36), the host version of the action-smoothness
-metric (:82-120; the device version is csrc/rollout.cu smoothness_kernel) and the wandb-config loader (:123-146)."""
+metric (:82-120; the device version is K6, csrc/smoothness.cu) and the wandb-config loader (:123-146)."""
 from dataclasses import dataclass
 from pathlib import Path
 from typing import List

@@ -113,14 +113,8 @@ extern "C" int serl_ssne_select(const double* d_fitness, int32_t pop, const int3
 {
     if (!d_fitness || !d_index_rank || (n_off > 0 && (!d_draws || !d_offsprings_raw))) return serl_fail(SERL_ERR_ARG, "serl_ssne_select: null pointer");
     if (pop <= 0 || pop > 16384 || n_off < 0) return serl_fail(SERL_ERR_ARG, "serl_ssne_select: 0 < pop <= 16384 required");
-    if (pop * sizeof(int) > 48 * 1024) {        // above the default dynamic shared-memory limit: opt in
-        cudaError_t ea = cudaFuncSetAttribute(ssne_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(pop * sizeof(int)));
-        if (ea != cudaSuccess) return serl_fail_cuda(ea, "cudaFuncSetAttribute(ssne_select)");
-    }
-    ssne_select_kernel<<<1, 1024, pop * sizeof(int), (cudaStream_t)stream>>>(d_fitness, pop, d_draws, n_off, d_index_rank, d_offsprings_raw);
-    serl_count_launch();
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? SERL_OK : serl_fail_cuda(e, "ssne_select_kernel");
+    return serl_launch("ssne_select_kernel", ssne_select_kernel, 1, 1024, pop * sizeof(int), (cudaStream_t)stream, d_fitness, pop, d_draws,
+                       n_off, d_index_rank, d_offsprings_raw);
 }
 
 extern "C" int serl_ssne_clone(float* d_weights, int32_t pop, int32_t P, const int32_t* d_pairs, int32_t n, void* stream)
@@ -128,10 +122,7 @@ extern "C" int serl_ssne_clone(float* d_weights, int32_t pop, int32_t P, const i
     if (n == 0) return SERL_OK;
     if (!d_weights || !d_pairs || pop <= 0 || P <= 0 || n < 0) return serl_fail(SERL_ERR_ARG, "serl_ssne_clone: bad argument");
     dim3 grid((P + 1023) / 1024 > 8 ? 8 : (P + 1023) / 1024, n);
-    ssne_clone_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(d_weights, P, d_pairs, n);
-    serl_count_launch();
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? SERL_OK : serl_fail_cuda(e, "ssne_clone_kernel");
+    return serl_launch("ssne_clone_kernel", ssne_clone_kernel, grid, 256, 0, (cudaStream_t)stream, d_weights, P, d_pairs, n);
 }
 
 extern "C" int serl_ssne_crossover(float* d_weights, int32_t pop, int32_t P, const int32_t* d_pair_desc, int32_t n_pairs,
@@ -139,10 +130,7 @@ extern "C" int serl_ssne_crossover(float* d_weights, int32_t pop, int32_t P, con
 {
     if (n_pairs == 0) return SERL_OK;
     if (!d_weights || !d_pair_desc || !d_ops || pop <= 0 || P <= 0 || n_pairs < 0) return serl_fail(SERL_ERR_ARG, "serl_ssne_crossover: bad argument");
-    ssne_crossover_kernel<<<n_pairs, 256, 0, (cudaStream_t)stream>>>(d_weights, P, d_pair_desc, d_ops);
-    serl_count_launch();
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? SERL_OK : serl_fail_cuda(e, "ssne_crossover_kernel");
+    return serl_launch("ssne_crossover_kernel", ssne_crossover_kernel, n_pairs, 256, 0, (cudaStream_t)stream, d_weights, P, d_pair_desc, d_ops);
 }
 
 extern "C" int serl_ssne_mutate(float* d_weights, int32_t pop, int32_t P, const int32_t* d_seg, int32_t n_seg,
@@ -152,8 +140,6 @@ extern "C" int serl_ssne_mutate(float* d_weights, int32_t pop, int32_t P, const 
     if (n_seg == 0) return SERL_OK;
     if (!d_weights || !d_seg || !d_op_off || !d_op_kind || !d_op_z || pop <= 0 || P <= 0 || n_seg < 0)
         return serl_fail(SERL_ERR_ARG, "serl_ssne_mutate: bad argument");
-    ssne_mutate_kernel<<<(n_seg + 63) / 64, 64, 0, (cudaStream_t)stream>>>(d_weights, P, d_seg, n_seg, d_op_off, d_op_kind, d_op_z, mag32, super32);
-    serl_count_launch();
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? SERL_OK : serl_fail_cuda(e, "ssne_mutate_kernel");
+    return serl_launch("ssne_mutate_kernel", ssne_mutate_kernel, (n_seg + 63) / 64, 64, 0, (cudaStream_t)stream, d_weights, P, d_seg, n_seg,
+                       d_op_off, d_op_kind, d_op_z, mag32, super32);
 }

@@ -430,6 +430,11 @@ struct RolloutArgs {
     Handoff ho;
 };
 
+// plant tables + per-variant parameter rows (reals), and that count rounded up to an even one: the block K1 stages at the
+// start of its dynamic shared memory, in front of the genome slots
+constexpr int PLANT_TABN = PT_TOTAL + SERL_PLANT_COUNT * PLANT_NPV;
+constexpr int PLANT_TABN2 = (PLANT_TABN + 1) & ~1;
+
 struct Env {
     double X[NX];
     const real* tab;         // plant tables (shared or global memory)

@@ -332,8 +332,7 @@ __device__ __forceinline__ void tc_actor_forward(TcCtx& c, const TcArgs& ar, con
     action[0] = act_s[tid * 4]; action[1] = act_s[tid * 4 + 1]; action[2] = act_s[tid * 4 + 2];
 }
 
-constexpr int TC_TABN = PT_TOTAL + SERL_PLANT_COUNT * PLANT_NPV;      // plant tables + per-variant parameter rows
-constexpr int TC_TABN2 = (TC_TABN + 15) & ~15;                          // keeps the float regions 128-byte aligned
+constexpr int TC_TABN2 = (PLANT_TABN + 15) & ~15;                       // keeps the float regions 128-byte aligned
 constexpr int TC_IO_FLOATS = TC_THREADS * 12;                           // per group: observations [128][8], actions [128][4]
 
 __device__ __forceinline__ void tc_setup(TcCtx& c, const TcArgs& ar, unsigned char* smem_raw, uint64_t* bars, uint32_t* shared_state)
@@ -461,7 +460,7 @@ static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t
     constexpr int A_STAGE_FLOATS = 2 * TC_CH * TC_M * 4;
     *smem_out = (size_t)TC_TABN2 * sizeof(real) +
                 (size_t)(2 * ((ar.small_floats + 31) & ~31) + 2 * TC_IO_FLOATS + TC_STAGES * A_STAGE_FLOATS + TC_STAGES * ar.stage_floats) * 4;
-    if (*smem_out > 227 * 1024 - 256) return serl_fail(SERL_ERR_UNSUPPORTED, "wide actors: tables + parameters + rings exceed the shared memory of an SM");
+    if (*smem_out > SERL_SMEM_OPTIN - 256) return serl_fail(SERL_ERR_UNSUPPORTED, "wide actors: tables + parameters + rings exceed the shared memory of an SM");
     const int P = (int)serl_actor_num_params_wide(widths, n_widths);
     const int n_stages = ar.w1 / TC_KSLAB;
     const size_t small_bytes = (size_t)pop * ar.small_floats * 4;
@@ -474,19 +473,8 @@ static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t
     ar.small = small; ar.tiles = tiles;
     const long long total = (long long)pop * ((long long)ar.small_floats + (long long)n_stages * ar.stage_floats);
     const int grid = (int)((total + 255) / 256 < 8192 ? (total + 255) / 256 : 8192);
-    tc_layout_kernel<<<grid, 256, 0, s>>>(d_weights, pop, P, ar.w1, w1, w2, ar.n2pad, ar.small_floats, ar.stage_floats, small, tiles);
-    serl_count_launch();
-    return SERL_OK;
-}
-
-// one CTA = the two groups of TC_THREADS threads
-static cudaError_t tc_launch(void (*kernel)(TcArgs), const TcArgs& ar, unsigned grid, size_t smem, cudaStream_t s)
-{
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    kernel<<<grid, 2 * TC_THREADS, smem, s>>>(ar);
-    serl_count_launch();
-    return cudaGetLastError();
+    return serl_launch("tc_layout_kernel", tc_layout_kernel, grid, 256, 0, s, d_weights, pop, P, ar.w1, w1, w2, ar.n2pad, ar.small_floats,
+                       ar.stage_floats, small, tiles);
 }
 
 // K1-TC launch (serl_rollout_run has checked the descriptor and built the env / output arguments `r`)
@@ -508,8 +496,9 @@ int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, cudaStream
         {rollout_kernel_tc<SERL_ACT_TANH, false>, rollout_kernel_tc<SERL_ACT_TANH, true>},
         {rollout_kernel_tc<SERL_ACT_ELU, false>, rollout_kernel_tc<SERL_ACT_ELU, true>},
         {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true>}};
-    const cudaError_t e = tc_launch(kernels[d.shape.activation][(d.flags & SERL_ROLLOUT_GUST) != 0], ar, (unsigned)grid, smem, s);
-    return e == cudaSuccess ? SERL_OK : serl_fail_cuda(e, "rollout_kernel_tc launch");
+    // one CTA = the two groups of TC_THREADS threads
+    return serl_launch("rollout_kernel_tc launch", kernels[d.shape.activation][(d.flags & SERL_ROLLOUT_GUST) != 0], (unsigned)grid,
+                       2 * TC_THREADS, smem, s, ar);
 }
 
 extern "C" int serl_actor_forward_wide(const float* d_genome, const int32_t* widths, int32_t n_widths, int32_t activation,
@@ -529,6 +518,5 @@ extern "C" int serl_actor_forward_wide(const float* d_genome, const int32_t* wid
     const int grid = blocks < sms ? blocks : sms;
     static void (*const kernels[3])(TcArgs) = {actor_forward_tc_kernel<SERL_ACT_TANH>, actor_forward_tc_kernel<SERL_ACT_ELU>,
                                                actor_forward_tc_kernel<SERL_ACT_LEAKY_RELU>};      // [SERL_ACT_*]
-    const cudaError_t e = tc_launch(kernels[activation], ar, (unsigned)grid, smem, s);
-    return e == cudaSuccess ? SERL_OK : serl_fail_cuda(e, "actor_forward_tc_kernel");
+    return serl_launch("actor_forward_tc_kernel", kernels[activation], (unsigned)grid, 2 * TC_THREADS, smem, s, ar);
 }

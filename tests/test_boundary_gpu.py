@@ -225,6 +225,25 @@ def test_smoothness_kernel_matches_reference_formula():
             assert abs(sm[i, e] - ref) <= 2e-5 * abs(ref) + 1e-9, (i, e, sm[i, e], ref)
 
 
+def test_smoothness_direct_dft_matches_reference_formula():
+    """K6 for histories longer than 2048 steps (the 80 s evaluation episode: 8001), which take the direct DFT instead of
+    the FFT: seeded synthetic actions (offset + slow sine + noise) in an 8001-step buffer, executed lengths on both sides
+    of 2048."""
+    from serl_b200 import rollout
+    from serl_b200.core.utils import calc_smoothness
+    rng = np.random.RandomState(3)
+    horizon, steps = 8001, np.array([8001, 5000, 3000, 1500], dtype=np.int32)
+    t = np.arange(horizon)[None, :, None] * 0.01
+    f = rng.uniform(0.05, 0.5, (len(steps), 1, 3))
+    ph = rng.uniform(0, 2 * np.pi, (len(steps), 1, 3))
+    a = (0.05 + 0.1 * np.sin(2 * np.pi * f * t + ph) + 0.01 * rng.randn(len(steps), horizon, 3)).astype(np.float32)
+    dev = torch.device('cuda:0')
+    sm = rollout.smoothness(torch.as_tensor(a, device=dev), torch.as_tensor(steps, device=dev)).cpu().numpy()
+    for i, n in enumerate(steps):
+        ref = calc_smoothness(a[i, :n].astype(np.float64))
+        assert abs(sm[i] - ref) <= 2e-5 * abs(ref) + 1e-9, (n, sm[i], ref)
+
+
 def test_evaluation_mode_80s_episode_matches_oracle():
     """set_eval_mode (envs/phlabenv.py:295-301): t_max = 80 s -> 8001 steps, reference widths scaled (block 16 s, smooth 13 s)."""
     from serl_b200 import rollout
