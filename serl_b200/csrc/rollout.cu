@@ -13,8 +13,8 @@
 //
 // Two actor implementations:
 //   rollout_kernel_persist<H, TABS, GUST>  persistent grid, one CTA per SM.  The MLP is a register-tiled GEMM inside a warp
-//                           (lane = 1/4 of the output neurons x 4 envs, float2 pairs, activations exchanged with warp
-//                           shuffles, weights broadcast from shared memory; h in {32,64,72,96,128}).  The CTA's warps take
+//                           (lane = 1/4 of the output neurons x 4 envs, float2 pairs, activations exchanged through a
+//                           per-warp shared-memory buffer, weights broadcast from shared memory; h in {32,64,72,96,128}).  The CTA's warps take
 //                           their steps in lockstep (one barrier per step: shared instruction fetch), genomes arrive by bulk
 //                           TMA copies.
 //   rollout_kernel_simple   every thread runs the whole MLP for its env (any h that fits); cross-check / fallback shape.
@@ -89,47 +89,82 @@ __device__ void actor_forward_simple(const float* __restrict__ w, const serl_act
 // smem: plant tables [PT_TOTAL] f64 | per actor of the CTA: transposed weights
 //       Wt0[S][H] b0[H] | L x { Wt[H][H] b[H] gamma[H] beta[H] } | Wo[A][H] bo[A]
 // lane = (g = lane>>2, og = lane&3): output neurons og*TM .. og*TM+TM-1 of the envs 4g .. 4g+3 of this warp.
-// The activation of neuron k for env 4g+c lives in lane (g, og = k/TM), register in[k%TM][c]; the next layer
-// fetches it with one shuffle per (k, c).  Reductions over neurons are xor-butterflies over the two og bits, so
-// the four lanes of a group hold bit-identical means / deviations.
+// The activation of neuron k for env 4g+c lives in lane (g, og = k/TM), register in[k%TM][c].  The next layer reads
+// it from the warp's exchange buffer xb in shared memory, one source quarter at a time: before quarter so the og == so
+// lanes store their in[][] as xb[m][g][c] (one STS.128 per neuron), so that one LDS.128 per source neuron gives a
+// lane the four envs of its group and the loop over source neurons is a rolled loop with a small body (unrolled, the
+// register selection and shuffles of every neuron made the actor too large for the instruction cache next to the
+// plant).  Reductions over neurons are xor-butterflies over the two og bits, so the four lanes of a group hold
+// bit-identical means / deviations.
 // All MLP arithmetic is written on float2 pairs (am_fma2: two independent IEEE-rn fmas); a float2
 // register pair holds two consecutive output neurons (m, m+1) of one env, exactly what one LDS.64 of the transposed
 // weight row delivers, and the activation of the source neuron is broadcast into both halves.
+__host__ __device__ constexpr int actor_xbuf_floats(int H) { return H / 4 * 32; }    // exchange buffer per warp: a quarter x 32 envs
+
+// one source row: its activation for the group's four envs and the lane's h/4 weights
+template <int H>
+struct WarpRow {
+    float4 x;
+    float2 w[H / 8];
+    __device__ __forceinline__ void load(const float* __restrict__ wrow, const float* xg, int k)
+    {
+        x = *reinterpret_cast<const float4*>(xg + k * 32);
+        const float2* wp = reinterpret_cast<const float2*>(wrow + k * H);
+#pragma unroll
+        for (int m2 = 0; m2 < H / 8; ++m2) w[m2] = wp[m2];
+    }
+    __device__ __forceinline__ void fma(float2 (&acc)[H / 8][4]) const
+    {
+#pragma unroll
+        for (int m2 = 0; m2 < H / 8; ++m2) {
+            acc[m2][0] = am_fma2(w[m2], am_splat(x.x), acc[m2][0]);
+            acc[m2][1] = am_fma2(w[m2], am_splat(x.y), acc[m2][1]);
+            acc[m2][2] = am_fma2(w[m2], am_splat(x.z), acc[m2][2]);
+            acc[m2][3] = am_fma2(w[m2], am_splat(x.w), acc[m2][3]);
+        }
+    }
+};
+
+// acc[m2][c] += sum over source rows k < nk (in order from 0) of wrow[k*H + 2*m2 (+1)] * xg[k*32 + c].
+// Two rows per trip, each row's loads issued before the multiply-adds of the row ahead of it: the shared-memory latency
+// is hidden without unrolling the loop.
+template <int H>
+__device__ __forceinline__ void warp_rows(const float* __restrict__ wrow, int nk, const float* xg, float2 (&acc)[H / 8][4])
+{
+    WarpRow<H> ra, rb;
+    ra.load(wrow, xg, 0);
+    int k = 0;
+#pragma unroll 1
+    for (; k + 2 <= nk; k += 2) {
+        rb.load(wrow, xg, k + 1);
+        ra.fma(acc);
+        ra.load(wrow, xg, k + 2 < nk ? k + 2 : k + 1);      // (the last trip re-reads row k + 1: stays in bounds)
+        rb.fma(acc);
+    }
+    if (k < nk) ra.fma(acc);
+}
+
 template <int H>
 __device__ __forceinline__ void warp_layer(const float* __restrict__ Wt, const float2 (&in)[H / 8][4], float2 (&acc)[H / 8][4],
-                                           int og, int lane)
+                                           int og, int g, float* xb)
 {
     constexpr int TM = H / 4, TM2 = H / 8;
 #pragma unroll
     for (int m = 0; m < TM2; ++m)
 #pragma unroll
         for (int c = 0; c < 4; ++c) acc[m][c] = make_float2(0.f, 0.f);
-    const int gbase = lane & ~3;
 #pragma unroll 1
     for (int so = 0; so < 4; ++so) {
-        const float* wrow = Wt + (size_t)(so * TM) * H + og * TM;
-#pragma unroll
-        for (int m = 0; m < TM; ++m) {
-            // activation of source neuron k = so*TM + m for the four envs of this group
-            const float src0 = (m & 1) ? in[m >> 1][0].y : in[m >> 1][0].x;
-            const float src1 = (m & 1) ? in[m >> 1][1].y : in[m >> 1][1].x;
-            const float src2 = (m & 1) ? in[m >> 1][2].y : in[m >> 1][2].x;
-            const float src3 = (m & 1) ? in[m >> 1][3].y : in[m >> 1][3].x;
-            const float a0 = __shfl_sync(0xffffffffu, src0, gbase + so);
-            const float a1 = __shfl_sync(0xffffffffu, src1, gbase + so);
-            const float a2 = __shfl_sync(0xffffffffu, src2, gbase + so);
-            const float a3 = __shfl_sync(0xffffffffu, src3, gbase + so);
-            const float2 b0 = make_float2(a0, a0), b1 = make_float2(a1, a1), b2 = make_float2(a2, a2), b3 = make_float2(a3, a3);
-            const float2* wp = reinterpret_cast<const float2*>(wrow + m * H);
+        __syncwarp();                                  // the previous quarter has been read
+        if (og == so) {
 #pragma unroll
             for (int m2 = 0; m2 < TM2; ++m2) {
-                const float2 w2 = wp[m2];
-                acc[m2][0] = am_fma2(w2, b0, acc[m2][0]);
-                acc[m2][1] = am_fma2(w2, b1, acc[m2][1]);
-                acc[m2][2] = am_fma2(w2, b2, acc[m2][2]);
-                acc[m2][3] = am_fma2(w2, b3, acc[m2][3]);
+                *reinterpret_cast<float4*>(xb + (2 * m2) * 32 + g * 4) = make_float4(in[m2][0].x, in[m2][1].x, in[m2][2].x, in[m2][3].x);
+                *reinterpret_cast<float4*>(xb + (2 * m2 + 1) * 32 + g * 4) = make_float4(in[m2][0].y, in[m2][1].y, in[m2][2].y, in[m2][3].y);
             }
         }
+        __syncwarp();
+        warp_rows<H>(Wt + (size_t)(so * TM) * H + og * TM, TM, xb + g * 4, acc);
     }
 }
 
@@ -140,38 +175,34 @@ __device__ __forceinline__ float group_sum(float v)
     return v;
 }
 
+// observation in, action out: by value (registers) rather than through pointers, which put them in local memory
+struct ActorObs { float v[7]; };
+struct ActorAct { float v[3]; };
+
+// xb: this warp's exchange buffer, actor_xbuf_floats(H) floats in shared memory, 16-byte aligned
 template <int H, int ACT>
-__device__ __noinline__ void actor_forward_warp(const float* __restrict__ w, int L, int lane, const float* obs, float* action)
+__device__ __noinline__ ActorAct actor_forward_warp(const float* __restrict__ w, int L, int lane, float* xb, ActorObs obs)
 {
     constexpr int TM = H / 4, TM2 = H / 8;
     constexpr int S = 7, A = 3;
-    const int og = lane & 3, gbase = lane & ~3;
+    static_assert(TM >= S, "the observation rows fit the exchange buffer");
+    const int og = lane & 3, g = lane >> 2;
     const float* Wt0 = w;
     const float* b0 = Wt0 + S * H;
     const float* hid = b0 + H;
     const float* Wo = hid + (size_t)L * (H * H + 3 * H);
     const float* bo = Wo + A * H;
     float2 in[TM2][4], acc[TM2][4];
-    // input layer: observation of env 4g+c lives in lane gbase+c
+    // input layer: the observation of env lane = 4g+c goes to xb[k][g][c]
 #pragma unroll
     for (int m = 0; m < TM2; ++m)
 #pragma unroll
         for (int c = 0; c < 4; ++c) acc[m][c] = make_float2(0.f, 0.f);
+    __syncwarp();                                      // the previous call has read the buffer
 #pragma unroll
-    for (int k = 0; k < S; ++k) {
-        const float a0 = __shfl_sync(0xffffffffu, obs[k], gbase + 0);
-        const float a1 = __shfl_sync(0xffffffffu, obs[k], gbase + 1);
-        const float a2 = __shfl_sync(0xffffffffu, obs[k], gbase + 2);
-        const float a3 = __shfl_sync(0xffffffffu, obs[k], gbase + 3);
-        const float2 b0v = make_float2(a0, a0), b1v = make_float2(a1, a1), b2v = make_float2(a2, a2), b3v = make_float2(a3, a3);
-        const float2* wp = reinterpret_cast<const float2*>(Wt0 + k * H + og * TM);
-#pragma unroll
-        for (int m2 = 0; m2 < TM2; ++m2) {
-            const float2 w2 = wp[m2];
-            acc[m2][0] = am_fma2(w2, b0v, acc[m2][0]); acc[m2][1] = am_fma2(w2, b1v, acc[m2][1]);
-            acc[m2][2] = am_fma2(w2, b2v, acc[m2][2]); acc[m2][3] = am_fma2(w2, b3v, acc[m2][3]);
-        }
-    }
+    for (int k = 0; k < S; ++k) xb[k * 32 + lane] = obs.v[k];
+    __syncwarp();
+    warp_rows<H>(Wt0 + og * TM, S, xb + g * 4, acc);
 #pragma unroll
     for (int m2 = 0; m2 < TM2; ++m2) {
         const float2 b = *reinterpret_cast<const float2*>(b0 + og * TM + 2 * m2);
@@ -185,7 +216,7 @@ __device__ __noinline__ void actor_forward_warp(const float* __restrict__ w, int
         const float* bb = Wt + H * H;
         const float* gamma = bb + H;
         const float* beta = gamma + H;
-        warp_layer<H>(Wt, in, acc, og, lane);
+        warp_layer<H>(Wt, in, acc, og, g, xb);
         float s[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
         for (int m2 = 0; m2 < TM2; ++m2) {
@@ -224,6 +255,7 @@ __device__ __noinline__ void actor_forward_warp(const float* __restrict__ w, int
         }
     }
     // output layer: partial dot products over this lane's neurons, reduced over the group; lane og keeps env 4g+og
+    ActorAct action;
 #pragma unroll
     for (int j = 0; j < A; ++j) {
         float p[4] = {0.f, 0.f, 0.f, 0.f};
@@ -236,8 +268,25 @@ __device__ __noinline__ void actor_forward_warp(const float* __restrict__ w, int
 #pragma unroll
         for (int c = 0; c < 4; ++c) p[c] = group_sum(p[c]);
         const float mine = og == 0 ? p[0] : (og == 1 ? p[1] : (og == 2 ? p[2] : p[3]));
-        action[j] = am_tanh1(__fadd_rn(mine, bo[j]));
+        action.v[j] = am_tanh1(__fadd_rn(mine, bo[j]));
     }
+    return action;
+}
+
+// one instantiation per activation: the choice is compiled into the 4 x h/4 activation calls of every layer
+template <int H>
+__device__ __forceinline__ void actor_forward(int act, const float* __restrict__ w, int L, int lane, float* xb, const float (&obs)[7],
+                                              float (&a)[3])
+{
+    ActorObs o;
+#pragma unroll
+    for (int k = 0; k < 7; ++k) o.v[k] = obs[k];
+    ActorAct r;
+    if (act == SERL_ACT_TANH) r = actor_forward_warp<H, SERL_ACT_TANH>(w, L, lane, xb, o);
+    else if (act == SERL_ACT_ELU) r = actor_forward_warp<H, SERL_ACT_ELU>(w, L, lane, xb, o);
+    else r = actor_forward_warp<H, SERL_ACT_LEAKY_RELU>(w, L, lane, xb, o);
+#pragma unroll
+    for (int j = 0; j < 3; ++j) a[j] = r.v[j];
 }
 
 
@@ -316,6 +365,7 @@ rollout_kernel_persist(RolloutArgs ar)
     }
     __syncthreads();
     float* w = wbase + (size_t)slot_l * ar.P4;
+    float* xb = wbase + (size_t)ar.apc * ar.P4 + warp * actor_xbuf_floats(H);     // after the genomes of all slots
     const int slot_threads = wps * 32;
     const int actfn = ar.sh.activation;
     const int horizon = ar.horizon;
@@ -338,9 +388,9 @@ rollout_kernel_persist(RolloutArgs ar)
     }
     // segments in the order: head of the last task (published) -> whole tasks -> tail of the first task (continued)
     long long t_cur = t_first + (k0 > 0 ? 1 : 0);
-    // LOCKSTEP: all warps of the CTA take their steps together (one CTA barrier per step).  The step body is ~155 KB of
-    // code at h = 72 (sm_90a SASS: actor 57 KB + the out-of-line tanh 0.8 KB, right-hand side 41 KB x 6 calls, ode5 step
-    // 16 KB, environment and segment bookkeeping up to 41 KB); eight warps drifting through it independently each stream it
+    // LOCKSTEP: all warps of the CTA take their steps together (one CTA barrier per step).  The step body is ~130 KB of
+    // code at h = 72 (sm_90a SASS: actor 32 KB + the out-of-line tanh 0.8 KB, right-hand side 41 KB x 6 calls, ode5 step
+    // 16 KB, environment and segment bookkeeping up to 40 KB); eight warps drifting through it independently each stream it
     // through the instruction caches on their own, and instruction fetch was the top stall (no_instruction 27 % of the warp
     // samples on B200).  In lockstep a fetched line serves every warp of the SM.
     Env e;
@@ -456,10 +506,7 @@ rollout_kernel_persist(RolloutArgs ar)
         if (!__syncthreads_or(in_seg || pending)) break;
         const bool mine = in_seg && !e.done && e.k < ke;
         if (__any_sync(0xffffffffu, mine)) {
-            // one instantiation per activation: the choice is compiled into the 4 x h/4 activation calls of every layer
-            if (actfn == SERL_ACT_TANH) actor_forward_warp<H, SERL_ACT_TANH>(w, L, lane, obs, a);
-            else if (actfn == SERL_ACT_ELU) actor_forward_warp<H, SERL_ACT_ELU>(w, L, lane, obs, a);
-            else actor_forward_warp<H, SERL_ACT_LEAKY_RELU>(w, L, lane, obs, a);
+            actor_forward<H>(actfn, w, L, lane, xb, obs, a);
             if (mine) env_step<TABS, GUST>(e, ar, traj, actor, replay, a, obs);
         }
     }
@@ -504,6 +551,7 @@ actor_forward_kernel(const float* __restrict__ genome, int P, serl_actor_shape s
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float* w = reinterpret_cast<float*>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31;
+    float* xb = w + ((P + 3) & ~3) + (tid >> 5) * actor_xbuf_floats(H);      // after the genome
     for (int i = tid; i < P; i += 128) w[genome_layout_index(i, sh.state_dim, H, sh.num_layers)] = genome[i];
     __syncthreads();
     const int base = (blockIdx.x * 128 + (tid & ~31));
@@ -512,9 +560,7 @@ actor_forward_kernel(const float* __restrict__ genome, int P, serl_actor_shape s
     float obs[7], a[3];
 #pragma unroll
     for (int k = 0; k < 7; ++k) obs[k] = i < n ? obs_in[(size_t)i * 7 + k] : 0.f;
-    if (sh.activation == SERL_ACT_TANH) actor_forward_warp<H, SERL_ACT_TANH>(w, sh.num_layers, lane, obs, a);
-    else if (sh.activation == SERL_ACT_ELU) actor_forward_warp<H, SERL_ACT_ELU>(w, sh.num_layers, lane, obs, a);
-    else actor_forward_warp<H, SERL_ACT_LEAKY_RELU>(w, sh.num_layers, lane, obs, a);
+    actor_forward<H>(sh.activation, w, sh.num_layers, lane, xb, obs, a);
     if (i < n) { act_out[(size_t)i * 3] = a[0]; act_out[(size_t)i * 3 + 1] = a[1]; act_out[(size_t)i * 3 + 2] = a[2]; }
 }
 
@@ -693,7 +739,8 @@ static int launch_persist(RolloutArgs& ar, int apc_max, bool gust, cudaStream_t 
     const int rc = serl_launch("genome_layout_kernel", genome_layout_kernel, lay_grid, 256, 0, s, ar.weights, wt, ar.pop, ar.P, ar.P4,
                                ar.sh.state_dim, H, ar.sh.num_layers);
     if (rc != SERL_OK) return rc;
-    const size_t smem = (TABS ? (size_t)PLANT_TABN2 * sizeof(real) : 0) + (size_t)apc * ar.P4 * 4;
+    const size_t smem = (TABS ? (size_t)PLANT_TABN2 * sizeof(real) : 0) + (size_t)apc * ar.P4 * 4 +
+                        (size_t)apc * wps * actor_xbuf_floats(H) * 4;
     void (*const kernel)(RolloutArgs) = gust ? rollout_kernel_persist<H, TABS, true> : rollout_kernel_persist<H, TABS, false>;
     return serl_launch("rollout_kernel launch", kernel, (unsigned)grid, apc * wps * 32, smem, s, ar);
 }
@@ -730,11 +777,13 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
         return serl_launch("rollout_kernel launch", rollout_kernel_simple, dim3((d.n_envs + 127) / 128, d.pop), 128, smem, s, ar);
     }
     // as many genome slots per CTA as shared memory holds next to the plant tables (h <= 72: two; h = 96: one);
-    // h = 128 (207 KB genome) reads the tables through L1 instead
+    // h = 128 (207 KB genome) reads the tables through L1 instead.  A slot is its genome and the actor exchange buffers
+    // of up to 4 warps.
     const size_t tab_bytes = (size_t)PLANT_TABN2 * sizeof(real);
     const size_t budget = SERL_SMEM_OPTIN - 256;       // static shared memory + alignment of the dynamic part
-    const bool tabs = tab_bytes + (size_t)ar.P4 * 4 <= budget;
-    int apc_max = (int)(((tabs ? budget - tab_bytes : budget)) / ((size_t)ar.P4 * 4));
+    const size_t slot_bytes = (size_t)ar.P4 * 4 + 4ull * actor_xbuf_floats(H) * 4;      // h = 128: 218 KB
+    const bool tabs = tab_bytes + slot_bytes <= budget;
+    int apc_max = (int)(((tabs ? budget - tab_bytes : budget)) / slot_bytes);
     if (apc_max > 4) apc_max = 4;
     if (apc_max > 2 && H > 32) apc_max = 2;
     const bool gust = (d.flags & SERL_ROLLOUT_GUST) != 0;
@@ -843,9 +892,9 @@ extern "C" int serl_actor_forward(const float* d_genome, const serl_actor_shape*
     const int grid = (n + 127) / 128;
     const size_t smem = (size_t)((P + 3) & ~3) * 4;
     int rc = SERL_OK;
-    const auto warp_launch = [&](auto h) {
-        rc = serl_launch("actor_forward_kernel", actor_forward_kernel<decltype(h)::value>, grid, 128, smem, s, d_genome, P, *shape, d_obs, n,
-                         d_actions);
+    const auto warp_launch = [&](auto h) {      // genome + the exchange buffers of 4 warps
+        rc = serl_launch("actor_forward_kernel", actor_forward_kernel<decltype(h)::value>, grid, 128, smem + 4ull * actor_xbuf_floats(H) * 4,
+                         s, d_genome, P, *shape, d_obs, n, d_actions);
     };
     if (!force_simple() && warp_hidden(H, warp_launch)) return rc;
     const size_t sm2 = smem + 2ull * H * 128 * 4;
