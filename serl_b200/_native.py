@@ -1,11 +1,25 @@
-"""ctypes binding of the C-ABI library (include/serl_b200.h).  The product path has no CPU fallback:
-importing succeeds without a GPU (so host logic is testable), but the library must exist and every
-compute call fails loudly when CUDA is unavailable."""
+"""ctypes binding of the C-ABI library (include/serl_b200.h): the only module that binds it.  The product path has no CPU
+fallback: importing succeeds without a GPU (so host logic is testable), but the library must exist and every compute call
+fails loudly when CUDA is unavailable.  tests/test_capi.py holds the signatures and constants below to the header."""
 import ctypes
 import os
 
+import numpy as np
+import torch
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('SERL_B200_LIB') or os.path.join(HERE, 'libserl_b200.so')   # SERL_B200_LIB: e.g. the --exact validation build
+
+ACTIVATIONS = {'tanh': 0, 'elu': 1, 'relu': 2}        # SERL_ACT_* ('relu' is the reference's LeakyReLU(0.01))
+PLANT_VARIANTS = ['h2000_v90', 'ice', 'cg', 'cg_for', 'h2000_v150', 'h10000_v90', 'cg_timed', 'cg_timed_post']   # SERL_PLANT_*
+FAULTS = ['none', 'be', 'jr', 'sa', 'se']             # SERL_FAULT_*
+TRACE_COLS = 22
+REPLAY_COLS = 20
+MODE_GUST = 1 << 24
+MODE_GUST_UP = 1 << 25
+ROLLOUT_GUST = 1
+STATUS_NONFINITE = 1
+STATUS_GUST_FLAG = 2
 
 
 class ActorShape(ctypes.Structure):
@@ -27,11 +41,32 @@ class RolloutDesc(ctypes.Structure):
                 ('flags', ctypes.c_int32)]
 
 
-REPLAY_COLS = 20
-STATUS_NONFINITE = 1
-STATUS_GUST_FLAG = 2
-ROLLOUT_GUST = 1
-ACTIVATIONS = {'tanh': 0, 'elu': 1, 'relu': 2}
+_vp, _i32, _i64, _f64, _int, _shape = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_double, ctypes.c_int, ctypes.POINTER(ActorShape)
+_rollout_args = [_vp, _i32, _shape, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]
+# entry point -> (restype, argtypes), in the header's order; every entry point returning a serl_status takes the stream last
+SIGNATURES = {
+    'serl_actor_num_params': (_i64, [_shape]),
+    'serl_rollout': (_int, _rollout_args + [_vp]),
+    'serl_rollout_eval': (_int, _rollout_args + [_f64, _f64, _vp]),
+    'serl_rollout_run': (_int, [ctypes.POINTER(RolloutDesc), _vp]),
+    'serl_actor_forward': (_int, [_vp, _shape, _vp, _i32, _vp, _vp]),
+    'serl_actor_num_params_wide': (_i64, [_vp, _i32]),
+    'serl_actor_forward_wide': (_int, [_vp, _vp, _i32, _i32, _vp, _i32, _vp, _vp]),
+    'serl_smoothness': (_int, [_vp, _vp, _i32, _i32, _f64, _vp, _vp]),
+    'serl_plant_init': (_int, [_vp, _vp, _i32, _vp]),
+    'serl_plant_step': (_int, [_vp, _vp, _vp, _i32, _vp]),
+    'serl_plant_step_timed': (_int, [_vp, _vp, _vp, _vp, _i32, _vp]),
+    'serl_ssne_select': (_int, [_vp, _i32, _vp, _i32, _vp, _vp, _vp]),
+    'serl_ssne_clone': (_int, [_vp, _i32, _i32, _vp, _i32, _vp]),
+    'serl_ssne_crossover': (_int, [_vp, _i32, _i32, _vp, _i32, _vp, _vp]),
+    'serl_ssne_mutate': (_int, [_vp, _i32, _i32, _vp, _i32, _vp, _vp, _vp, ctypes.c_float, ctypes.c_float, _vp]),
+    'serl_plan_create': (_vp, [_vp, _vp, _vp, _vp, _i32, _vp, _i32, _vp, _i32, _vp, _i32, _vp, _i32, _f64]),
+    'serl_plan_sizes': (None, [_vp, _vp]),
+    'serl_plan_copy': (None, [_vp] * 7),
+    'serl_plan_destroy': (None, [_vp]),
+    'serl_launch_count': (_i64, []),
+    'serl_last_error': (ctypes.c_char_p, []),
+}
 _lib = None
 
 
@@ -46,27 +81,9 @@ def lib():
             raise NativeError('serl_b200: %s is missing — build it with `python -m serl_b200.build` '
                               '(there is no CPU fallback)' % LIB_PATH)
         L = ctypes.CDLL(LIB_PATH)
-        vp, i32, i64 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64
-        L.serl_actor_num_params.restype = i64
-        L.serl_actor_num_params.argtypes = [ctypes.POINTER(ActorShape)]
-        L.serl_rollout.restype = ctypes.c_int
-        L.serl_rollout.argtypes = [vp, i32, ctypes.POINTER(ActorShape), vp, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp]
-        L.serl_rollout_eval.restype = ctypes.c_int
-        L.serl_rollout_eval.argtypes = L.serl_rollout.argtypes[:-1] + [ctypes.c_double, ctypes.c_double, vp]
-        L.serl_rollout_run.restype = ctypes.c_int
-        L.serl_rollout_run.argtypes = [ctypes.POINTER(RolloutDesc), vp]
-        L.serl_actor_forward.restype = ctypes.c_int
-        L.serl_actor_forward.argtypes = [vp, ctypes.POINTER(ActorShape), vp, i32, vp, vp]
-        L.serl_actor_num_params_wide.restype = i64
-        L.serl_actor_num_params_wide.argtypes = [vp, i32]
-        L.serl_actor_forward_wide.restype = ctypes.c_int
-        L.serl_actor_forward_wide.argtypes = [vp, vp, i32, i32, vp, i32, vp, vp]
-        L.serl_plant_step_timed.restype = ctypes.c_int
-        L.serl_plant_step_timed.argtypes = [vp, vp, vp, vp, i32, vp]
-        L.serl_smoothness.restype = ctypes.c_int
-        L.serl_smoothness.argtypes = [vp, vp, i32, i32, ctypes.c_double, vp, vp]
-        L.serl_launch_count.restype = i64
-        L.serl_last_error.restype = ctypes.c_char_p
+        for name, (restype, argtypes) in SIGNATURES.items():
+            f = getattr(L, name)
+            f.restype, f.argtypes = restype, argtypes
         _lib = L
     return _lib
 
@@ -74,3 +91,11 @@ def lib():
 def check(rc, what):
     if rc != 0:
         raise NativeError('%s failed (%d): %s' % (what, rc, lib().serl_last_error().decode()))
+
+
+def call(name, *args, device=None):
+    """lib().<name>(*args, stream) for a serl_status entry point: tensors and arrays go as pointers (`args` keeps them alive through
+    the call), the stream is the current one of `device` (default: the first tensor's device); a failure raises NativeError."""
+    device = device or next((a.device for a in args if isinstance(a, torch.Tensor)), None)
+    ptrs = [a.data_ptr() if isinstance(a, torch.Tensor) else a.ctypes if isinstance(a, np.ndarray) else a for a in args]
+    check(getattr(lib(), name)(*ptrs, torch.cuda.current_stream(device).cuda_stream), name)

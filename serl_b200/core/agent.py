@@ -103,9 +103,7 @@ class Agent:
     def _eval_kw(self):
         env = self.env
         kw = {} if env.t_max == 20 else {'t_max': float(env.t_max), 'smooth_width': refsig.widths(env.t_max)[1]}
-        if env.mode_code & rollout.MODE_GUST:
-            kw['gust'] = True
-        return kw
+        return dict(kw, gust=rollout.mode_gust(env.mode_code))
 
     def _fly(self, agent, n, is_action_noise=False, store_transition=False, trace=False, stream=None, copy_genome=False, draws=None) -> _Flight:
         """launch n episodes of one actor (fresh reference signals each, or the given `draws`) without waiting for them."""
@@ -150,7 +148,7 @@ class Agent:
         rows = rows[:n]
         self.replay_buffer.add_rows(rows)
         agent.buffer.add_rows(rows)
-        crit = rows[rows[:, 19] > 0.5]
+        crit = rows[rows[:, rollout.REPLAY_COST] > 0.5]
         if crit.shape[0]:
             agent.critical_buffer.add_rows(crit)
         self.num_frames += n
@@ -180,7 +178,7 @@ class Agent:
                 f.r.replay.record_stream(torch.cuda.current_stream(self.device))     # read below by kernels of this stream
             self._store_rows(agent, f.r.replay[0], int(steps[0]))
         env = self.env
-        theta_trim = np.rad2deg(self._initial_state(env)[7])
+        theta_trim = np.rad2deg(rollout.initial_state(rollout.mode_variant(env.mode_code))[7])
         from ..envs.phlabenv import _RefSignal
         sw = refsig.widths(env.t_max)[1]
         eps = []
@@ -191,9 +189,9 @@ class Agent:
             state_lst, actions, rewards = [], None, None
             if f.r.trace is not None and (want_history or f.n == 1):
                 tr = hist[e]
-                rewards = [float(x) for x in tr[:, 15]]
-                actions = tr[:, 12:15].copy()
-                state_lst = [] if store_transition else [tr[k, 0:12].copy() for k in range(n)]
+                rewards = [float(x) for x in tr[:, rollout.TRACE_R]]
+                actions = tr[:, rollout.TRACE_U].copy()
+                state_lst = [] if store_transition else [tr[k, rollout.TRACE_X].copy() for k in range(n)]
             else:
                 actions = hist[e] if want_history else np.zeros((0, 3))
                 rewards = _ReturnOnly(float(returns[e]))
@@ -205,20 +203,6 @@ class Agent:
         """Play one episode (agent.py:63-138) on the GPU."""
         f = self._fly(agent, 1, is_action_noise=is_action_noise, store_transition=store_transition, trace=True)
         return self._collect(agent, f, store_transition=store_transition, want_history=True)[0]
-
-    _ic_cache: Dict[int, np.ndarray] = {}
-
-    def _initial_state(self, env):
-        v = env.mode_code & 0xff
-        if v not in Agent._ic_cache:
-            import ctypes
-            from .. import _native
-            X = torch.empty((1, 19), dtype=torch.float64, device=self.device)
-            var = torch.tensor([v], dtype=torch.int32, device=self.device)
-            _native.check(_native.lib().serl_plant_init(ctypes.c_void_p(X.data_ptr()), ctypes.c_void_p(var.data_ptr()), 1,
-                                                       ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), 'serl_plant_init')
-            Agent._ic_cache[v] = X.cpu().numpy()[0, :12].copy()
-        return Agent._ic_cache[v]
 
     def rl_to_evo(self, rl_agent, evo_net):
         for target_param, param in zip(evo_net.actor.parameters(), rl_agent.actor.parameters()):
@@ -321,7 +305,7 @@ class Agent:
             self.replay_buffer.add_rows(rows_all[sel])
             actors = torch.arange(pop, device=self.device)
             self.pop.buffers.append(actors, rows_all, sel)
-            self.pop.critical_buffers.append(actors, rows_all, sel & (rows_all[..., 19] > 0.5))
+            self.pop.critical_buffers.append(actors, rows_all, sel & (rows_all[..., rollout.REPLAY_COST] > 0.5))
         rec_host = rec_all.cpu().numpy()
         if r is not None:
             r.check()

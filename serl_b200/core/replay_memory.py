@@ -9,6 +9,8 @@ from collections import namedtuple
 import numpy as np
 import torch
 
+from ..rollout import TRANSITION_COLS
+
 Transition = namedtuple('Transition', ('state', 'action', 'next_state', 'reward', 'done'))
 
 
@@ -74,7 +76,7 @@ class ReplayMemory:
         return tuple(torch.from_numpy(self._store[f][pick]).to(self.device) for f in Transition._fields)
 
 
-REPLAY_DIMS = (7, 3, 7, 1, 1)        # obs, action, next_obs, reward, done = columns 0..18 of a K1 replay row
+REPLAY_DIMS = (7, 3, 7, 1, 1)        # obs, action, next_obs, reward, done = the first TRANSITION_COLS columns of a K1 replay row
 
 
 def _split(rows):
@@ -90,7 +92,6 @@ class DeviceReplayMemory:
     SERL_REPLAY_COLS: obs 7 | action 3 | next_obs 7 | reward | done | cost); sampling uses a device generator, so the
     stdlib `random` stream the SSNE planner consumes does not depend on the buffer (every rank holds identical buffers and
     identical generators -> identical batches)."""
-    COLS = 19
 
     def __init__(self, capacity, device, seed=0):
         self.capacity, self.device = int(capacity), torch.device(device)
@@ -107,17 +108,17 @@ class DeviceReplayMemory:
 
     def _alloc(self):
         if self.data is None:
-            self.data = torch.zeros((self.capacity, self.COLS), dtype=torch.float32, device=self.device)
+            self.data = torch.zeros((self.capacity, TRANSITION_COLS), dtype=torch.float32, device=self.device)
             self.gen = torch.Generator(device=self.device)
             self.gen.manual_seed(self._seed)
 
     def add_rows(self, rows):
-        """append n transitions [n, >=19] (device tensor, chronological order) with ring semantics."""
+        """append n transitions [n, >=TRANSITION_COLS] (device tensor, chronological order) with ring semantics."""
         n = int(rows.shape[0])
         if n == 0:
             return
         self._alloc()
-        rows = rows[:, :self.COLS].to(self.device, torch.float32)
+        rows = rows[:, :TRANSITION_COLS].to(self.device, torch.float32)
         if n > self.capacity:
             skip = n - self.capacity
             rows = rows[skip:]
@@ -145,7 +146,7 @@ class DeviceReplayMemory:
     def _chronological_rows(self):
         n = len(self)
         if n == 0:
-            return torch.zeros((0, self.COLS), dtype=torch.float32, device=self.device)
+            return torch.zeros((0, TRANSITION_COLS), dtype=torch.float32, device=self.device)
         if self._count <= self.capacity:
             return self.data[:n]
         return torch.cat((self.data[self.position:], self.data[:self.position]))
@@ -172,7 +173,7 @@ class DeviceReplayMemory:
 
 class PopulationBuffers:
     """The per-actor replay buffers of the whole population (GeneticAgent.buffer / .critical_buffer,
-    base/core/genetic_agent.py:14-16) as ONE device tensor [pop, capacity, 19] with per-actor ring positions, filled
+    base/core/genetic_agent.py:14-16) as ONE device tensor [pop, capacity, TRANSITION_COLS] with per-actor ring positions, filled
     for all actors of a generation by one vectorised scatter."""
 
     def __init__(self, pop, capacity, device):
@@ -184,12 +185,12 @@ class PopulationBuffers:
 
     def _alloc(self):
         if self.data is None:
-            self.data = torch.zeros((self.pop, self.capacity, 19), dtype=torch.float32, device=self.device)
+            self.data = torch.zeros((self.pop, self.capacity, TRANSITION_COLS), dtype=torch.float32, device=self.device)
             self.gen = torch.Generator(device=self.device)
             self.gen.manual_seed(1)
 
     def append(self, actors, rows, select):
-        """rows [n, horizon, >=19]; select [n, horizon] bool (time order): the selected rows of rows[i] go to actor actors[i]."""
+        """rows [n, horizon, >=TRANSITION_COLS]; select [n, horizon] bool (time order): the selected rows of rows[i] go to actor actors[i]."""
         self._alloc()
         n, h = select.shape
         cnt = select.sum(1)
@@ -197,7 +198,7 @@ class PopulationBuffers:
         keep = select & (rank >= (cnt - self.capacity)[:, None])
         a_idx = actors.to(torch.int64)[:, None].expand(n, h)
         slot = (self.pos[actors][:, None] + rank) % self.capacity
-        self.data[a_idx[keep], slot[keep]] = rows[..., :19][keep].to(torch.float32)
+        self.data[a_idx[keep], slot[keep]] = rows[..., :TRANSITION_COLS][keep].to(torch.float32)
         self.pos[actors] = (self.pos[actors] + cnt) % self.capacity
         self.count[actors] += cnt
 
@@ -210,7 +211,7 @@ class PopulationBuffers:
     def rows_of(self, i):
         n = int(min(int(self.count[i]), self.capacity))
         if n == 0 or self.data is None:
-            return torch.zeros((0, 19), dtype=torch.float32, device=self.device)
+            return torch.zeros((0, TRANSITION_COLS), dtype=torch.float32, device=self.device)
         if int(self.count[i]) <= self.capacity:
             return self.data[i, :n]
         p = int(self.pos[i])
@@ -241,7 +242,7 @@ class ActorBuffer:
             return
         o = self.owner
         o._alloc()
-        rows = rows[-o.capacity:, :19].to(o.device, torch.float32)
+        rows = rows[-o.capacity:, :TRANSITION_COLS].to(o.device, torch.float32)
         m = int(rows.shape[0])
         slot = (o.pos[self.index] + (n - m) + torch.arange(m, device=o.device)) % o.capacity
         o.data[self.index, slot] = rows

@@ -8,8 +8,6 @@ Agent.train hands the env's mode and freshly drawn reference-signal parameters t
 Reference signals: `signals.RandomizedCosineStepSequence` (third-party, absent) is replaced by serl_b200/refsig.py's
 generator, drawing from the global np.random stream at reset() like the reference's init_ref (:303-345).
 """
-import ctypes
-
 import numpy as np
 import torch
 
@@ -152,11 +150,6 @@ class CitationEnv:
                     _RefSignal(self.levels[1], self.starts[1], 0.0, sw), lambda t: 0.0]
 
     # ---- native plant on the device ----
-    def _plant(self, fn, *args):
-        L = _native.lib()
-        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        _native.check(getattr(L, fn)(*args, stream), fn)
-
     def _native_step(self, u):
         cmd = np.pad(u, (0, self.n_actions_full - self.n_actions), 'constant', constant_values=(0.))
         if self.fault == 'be':
@@ -174,14 +167,12 @@ class CitationEnv:
             x[5] += 1.8 * 10**(-3) + 2.7 * 10**(-4) * np.random.randn(1)[0]
             x[6:8] += 4.0 * 10**(-3) + 3.2 * 10**(-5) * np.random.randn(2)
         dcmd = torch.as_tensor(cmd[:3].reshape(1, 3), device=self._X.device)
-        if self.mode_code >> 16:          # time-triggered build: the plant needs its clock (native calls made so far)
+        timed = rollout.timed_plant_code(self.mode_code)
+        if timed is not None:          # time-triggered build: the plant needs its clock (native calls made so far)
             call = torch.tensor([self._calls], dtype=torch.int32, device=self._X.device)
-            var = torch.tensor([self.mode_code & ~0xff00], dtype=torch.int32, device=self._X.device)     # without the fault field
-            self._plant('serl_plant_step_timed', ctypes.c_void_p(self._X.data_ptr()), ctypes.c_void_p(dcmd.data_ptr()),
-                        ctypes.c_void_p(var.data_ptr()), ctypes.c_void_p(call.data_ptr()), 1)
+            rollout.plant_step(self._X, dcmd, torch.tensor([timed], dtype=torch.int32, device=self._X.device), call)
         else:
-            self._plant('serl_plant_step', ctypes.c_void_p(self._X.data_ptr()), ctypes.c_void_p(dcmd.data_ptr()),
-                        ctypes.c_void_p(self._variant.data_ptr()), 1)
+            rollout.plant_step(self._X, dcmd, self._variant)
         self._calls += 1
         return x
 
@@ -190,9 +181,8 @@ class CitationEnv:
             raise _native.NativeError('CitationEnv needs a CUDA device (no CPU fallback)')
         self.t = 0.
         dev = torch.device('cuda', torch.cuda.current_device())
-        self._variant = torch.tensor([self.mode_code & 0xff], dtype=torch.int32, device=dev)
-        self._X = torch.empty((1, 19), dtype=torch.float64, device=dev)
-        self._plant('serl_plant_init', ctypes.c_void_p(self._X.data_ptr()), ctypes.c_void_p(self._variant.data_ptr()), 1)
+        self._variant = torch.tensor([rollout.mode_variant(self.mode_code)], dtype=torch.int32, device=dev)
+        self._X = rollout.plant_init(self._variant)
         self.last_u = np.zeros(self.n_actions)
         self._calls = 0
         self.x = self._native_step(self.last_u)

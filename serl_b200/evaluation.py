@@ -44,29 +44,22 @@ def validate_agent(genome, shape, env, user_refs_lst, num_trails=1, device=None)
         noise = torch.as_tensor(sensor_noise_draws(n, horizon).reshape(1, n, horizon + 1, 7), device=dev)
     r = rollout.population_rollout(g, shape, torch.as_tensor(levels, device=dev), torch.as_tensor(starts, device=dev), md,
                                    horizon=horizon, trace=True, t_max=float(env.t_max), smooth_width=smooth_w, sensor_noise=noise,
-                                   gust=bool(env.mode_code & rollout.MODE_GUST))
+                                   gust=rollout.mode_gust(env.mode_code))
     torch.cuda.synchronize()
     r.check()
     steps = r.steps[0].cpu().numpy()
     trace = r.trace[0].cpu().numpy()
-    v = env.mode_code & 0xff
-    import ctypes
-    from . import _native
-    X = torch.empty((1, 19), dtype=torch.float64, device=dev)
-    var = torch.tensor([v], dtype=torch.int32, device=dev)
-    _native.check(_native.lib().serl_plant_init(ctypes.c_void_p(X.data_ptr()), ctypes.c_void_p(var.data_ptr()), 1,
-                                               ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)), 'serl_plant_init')
-    x_ic = X.cpu().numpy()[0, :12]
+    x_ic = rollout.initial_state(rollout.mode_variant(env.mode_code))
     nmaes, sms, data = [], [], None
     for i in range(n):
         k = int(steps[i])
         tr = trace[i, :k]
-        x_after = tr[:, 0:12]                                   # env.x after each step() = state before that plant step
-        ref_values = tr[:, 19:22] + x_after[:, [7, 6, 5]]       # ref(t_k) [rad] = error_k + controlled state
+        x_after = tr[:, rollout.TRACE_X]                        # env.x after each step() = state before that plant step
+        ref_values = tr[:, rollout.TRACE_ERR] + x_after[:, [7, 6, 5]]      # ref(t_k) [rad] = error_k + controlled state
         x_before = np.vstack((x_ic[None], x_after[:-1]))        # env.x when the loop body starts (evaluate.py:73)
-        u_before = np.vstack((np.zeros((1, 3)), tr[:-1, 12:15]))
+        u_before = np.vstack((np.zeros((1, 3)), tr[:-1, rollout.TRACE_U]))
         errors = ref_values - x_before[:, [7, 6, 5]]
         nmaes.append(calc_nMAE(errors))
         sms.append(calc_smoothness(u_before, plot_spectra=False))
-        data = np.concatenate((ref_values, u_before, x_before, tr[:, 15:16]), axis=1)
+        data = np.concatenate((ref_values, u_before, x_before, tr[:, rollout.TRACE_R, None]), axis=1)
     return data, Stats(float(np.average(nmaes)), float(np.std(nmaes)), float(np.average(sms)), float(np.std(sms)))

@@ -8,7 +8,6 @@ base/train.py:88-91 selects, crosses and mutates exactly the individuals the ref
 Documented deviations (SURVEY.md F3): index draws use an exclusive upper bound (the reference's inclusive
 `random.randint(0, n)` indexes one past the end); ranking ties resolve to the larger index first.
 """
-import ctypes
 import math
 import random
 
@@ -152,21 +151,19 @@ def _plan_tail_native(plan, table, mut_order, mutation_prob):
     tab = np.asarray(table, dtype=np.int32).reshape(-1, 3).copy()
     i32 = lambda a: np.ascontiguousarray(np.asarray(a, dtype=np.int32))
     uns, ne, offs, mo = i32(plan.unselects), i32(plan.new_elitists), i32(plan.offsprings), i32(mut_order)
-    vp = lambda a: a.ctypes.data_as(ctypes.c_void_p)
-    L.serl_plan_create.restype = ctypes.c_void_p
-    h = L.serl_plan_create(vp(py_state), vp(py_gauss), vp(np_state), vp(tab), tab.shape[0], vp(uns), uns.shape[0],
-                           vp(ne), ne.shape[0], vp(offs), offs.shape[0], vp(mo), mo.shape[0], ctypes.c_double(mutation_prob))
+    # ndarray.ctypes keeps its array alive while ctypes converts it to the pointer argument
+    h = L.serl_plan_create(py_state.ctypes, py_gauss.ctypes, np_state.ctypes, tab.ctypes, tab.shape[0], uns.ctypes, uns.shape[0],
+                           ne.ctypes, ne.shape[0], offs.ctypes, offs.shape[0], mo.ctypes, mo.shape[0], mutation_prob)
     if not h:
         raise IndexError('SSNE.epoch: empty choice pool (no new elitists / offsprings) with crossover pairs pending, as '
                          'random.choice([]) in base/core/mod_neuro_evo.py:519-520')
-    h = ctypes.c_void_p(h)
     sizes = np.zeros(5, dtype=np.int64)
-    L.serl_plan_sizes(h, vp(sizes))
+    L.serl_plan_sizes(h, sizes.ctypes)
     n_pairs, n_ops, n_seg, n_mut = (int(x) for x in sizes[:4])
     pairs = np.zeros((n_pairs, 6), np.int32); ops = np.zeros((max(n_ops, 1), 3), np.int32)
     seg = np.zeros((n_seg, 3), np.int32); m_off = np.zeros(n_mut, np.int32); m_kind = np.zeros(n_mut, np.int32)
     m_z = np.zeros(n_mut, np.float32)
-    L.serl_plan_copy(h, vp(pairs), vp(ops), vp(seg), vp(m_off), vp(m_kind), vp(m_z))
+    L.serl_plan_copy(h, *(a.ctypes for a in (pairs, ops, seg, m_off, m_kind, m_z)))
     L.serl_plan_destroy(h)
     random.setstate((ver, tuple(int(x) for x in py_state), (py_gauss[1] if py_gauss[0] else None)))
     np.random.set_state((name, np_state[:624], int(np_state[624]), has_gauss, cached))
@@ -182,13 +179,8 @@ def _dev(a, device):
     return torch.from_numpy(np.ascontiguousarray(a)).to(device, non_blocking=False)
 
 
-def _p(t):
-    return ctypes.c_void_p(t.data_ptr())
-
-
 def select_device(fitness, num_elitists):
     """K2 on the device: tournament draws are made on the host first (np.random.randint(pop, size=3) per slot, :46)."""
-    L = _native.lib()
     dev = fitness.device
     pop = fitness.shape[0]
     n_off = pop - num_elitists
@@ -196,8 +188,7 @@ def select_device(fitness, num_elitists):
     d_draws = _dev(draws, dev)
     rank = torch.empty(pop, dtype=torch.int32, device=dev)
     offs = torch.empty(max(n_off, 1), dtype=torch.int32, device=dev)
-    stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    _native.check(L.serl_ssne_select(_p(fitness), pop, _p(d_draws), n_off, _p(rank), _p(offs), stream), 'serl_ssne_select')
+    _native.call('serl_ssne_select', fitness, pop, d_draws, n_off, rank, offs)
     both = torch.cat([rank, offs[:n_off]]).cpu().numpy()
     return both[:pop], both[pop:]
 
@@ -205,27 +196,23 @@ def select_device(fitness, num_elitists):
 def apply_plan(weights, plan, mutation_mag, phase='all'):
     """phase 'all', or 'pre' (elitism clones + crossover) / 'mut' (point mutations) when something runs in between
     (distillation crossover writes the unselected genomes before they are mutated)."""
-    L = _native.lib()
     dev = weights.device
     pop, P = weights.shape
-    stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
     keep = []
     for w in (plan.clone_waves if phase in ('all', 'pre') else []):
         t = _dev(w, dev); keep.append(t)
-        _native.check(L.serl_ssne_clone(_p(weights), pop, P, _p(t), w.shape[0], stream), 'serl_ssne_clone')
+        _native.call('serl_ssne_clone', weights, pop, P, t, w.shape[0])
     d_ops = None
     for desc, ops in (plan.cross_waves if phase in ('all', 'pre') else []):
         if d_ops is None:
             d_ops = _dev(ops if ops.size else np.zeros((1, 3), np.int32), dev); keep.append(d_ops)
         t = _dev(desc, dev); keep.append(t)
-        _native.check(L.serl_ssne_crossover(_p(weights), pop, P, _p(t), desc.shape[0], _p(d_ops), stream), 'serl_ssne_crossover')
+        _native.call('serl_ssne_crossover', weights, pop, P, t, desc.shape[0], d_ops)
     if plan.mut_seg.shape[0] and phase in ('all', 'mut'):
         seg, off, kind, z = (_dev(a, dev) for a in (plan.mut_seg, plan.mut_off, plan.mut_kind, plan.mut_z))
         keep += [seg, off, kind, z]
-        mag32 = ctypes.c_float(float(np.float32(mutation_mag)))
-        sup32 = ctypes.c_float(float(np.float32(10 * mutation_mag)))
-        _native.check(L.serl_ssne_mutate(_p(weights), pop, P, _p(seg), plan.mut_seg.shape[0], _p(off), _p(kind), _p(z),
-                                         mag32, sup32, stream), 'serl_ssne_mutate')
+        _native.call('serl_ssne_mutate', weights, pop, P, seg, plan.mut_seg.shape[0], off, kind, z,
+                     float(np.float32(mutation_mag)), float(np.float32(10 * mutation_mag)))
     torch.cuda.current_stream(dev).synchronize()      # op buffers must outlive the kernels
 
 

@@ -3,17 +3,21 @@
 Mirrors the population-evaluation loop of base/core/agent.py:229-245: every actor of the population is flown
 through every environment; fitness[a] = mean over envs of the episodic return.
 """
-import ctypes
+import functools
 
+import numpy as np
 import torch
 
 from . import _native
+from ._native import FAULTS, MODE_GUST, MODE_GUST_UP, PLANT_VARIANTS, REPLAY_COLS, TRACE_COLS
 
 HORIZON = 2001          # envs/phlabenv.py:82,181,392: t_max = 20 s, dt = 0.01, done checked before t += dt
-PLANT_VARIANTS = ['h2000_v90', 'ice', 'cg', 'cg_for', 'h2000_v150', 'h10000_v90', 'cg_timed', 'cg_timed_post']
+# trace record columns (SERL_TRACE_COLS): state before the step, commanded deflection, reward, action fed to the env, error
+TRACE_X, TRACE_U, TRACE_R, TRACE_A, TRACE_ERR = slice(0, 12), slice(12, 15), 15, slice(16, 19), slice(19, 22)
+# replay row (SERL_REPLAY_COLS): the transition obs 7 | action 3 | next_obs 7 | reward | done, then the cost flag
+TRANSITION_COLS = REPLAY_COST = 19
 # time-triggered builds: parameter row the plant switches to when its clock reaches 20 s (envs/phlabenv.py:159-163)
 POST_VARIANT = {'cg_timed': 'cg_timed_post'}
-FAULTS = ['none', 'be', 'jr', 'sa', 'se']
 # env mode string (envs/phlabenv.py:99-172) -> (plant variant, command fault)
 MODES = {
     'nominal': ('h2000_v90', 'none'), 'be': ('h2000_v90', 'be'), 'jr': ('h2000_v90', 'jr'),
@@ -23,8 +27,6 @@ MODES = {
     'gust': ('h2000_v90', 'none'),      # nominal dynamics + MODE_GUST (include/serl_b200.h); the env adds the sensor-noise shim
     'test': ('h2000_v90', 'none'),      # envs/test: the same pulse with the opposite sign (MODE_GUST | MODE_GUST_UP), no shim
 }
-MODE_GUST = 1 << 24
-MODE_GUST_UP = 1 << 25
 
 
 def mode_code(mode):
@@ -33,27 +35,35 @@ def mode_code(mode):
     return PLANT_VARIANTS.index(v) | (FAULTS.index(f) << 8) | (post << 16) | (MODE_GUST if mode in ('gust', 'test') else 0) | (MODE_GUST_UP if mode == 'test' else 0)
 
 
+def mode_variant(code):
+    return code & 0xff
+
+
+def mode_gust(code):
+    return bool(code & MODE_GUST)
+
+
+def timed_plant_code(code):
+    """the env_mode without its fault field (serl_plant_step_timed), or None if the plant needs no clock (no post variant, gust)"""
+    return code & ~0xff00 if code >> 16 else None
+
+
 def actor_shape(hidden, num_layers=3, activation='tanh', state_dim=7, action_dim=3):
     return _native.ActorShape(state_dim, action_dim, hidden, num_layers, _native.ACTIVATIONS[activation.lower()])
 
 
 def num_params(shape):
-    return int(_native.lib().serl_actor_num_params(ctypes.byref(shape)))
-
-
-def _ptr(t):
-    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+    return int(_native.lib().serl_actor_num_params(shape))
 
 
 class RolloutResult:
     __slots__ = ('returns', 'steps', 'fitness', 'trace', 'actions', 'smoothness', 'replay', 'status')
 
-    # views into the trace record (include/serl_b200.h: SERL_TRACE_COLS)
-    trace_x = property(lambda s: s.trace[..., 0:12])
-    trace_u = property(lambda s: s.trace[..., 12:15])
-    trace_r = property(lambda s: s.trace[..., 15])
-    trace_a = property(lambda s: s.trace[..., 16:19])
-    trace_err = property(lambda s: s.trace[..., 19:22])
+    trace_x = property(lambda s: s.trace[..., TRACE_X])
+    trace_u = property(lambda s: s.trace[..., TRACE_U])
+    trace_r = property(lambda s: s.trace[..., TRACE_R])
+    trace_a = property(lambda s: s.trace[..., TRACE_A])
+    trace_err = property(lambda s: s.trace[..., TRACE_ERR])
 
     def check(self):
         """raise if the kernel flagged a non-finite trajectory (synchronises the device)."""
@@ -62,10 +72,6 @@ class RolloutResult:
             raise _native.NativeError("serl_rollout: an env has mode 'gust' but the launch was not made with gust=True")
         if st & _native.STATUS_NONFINITE:
             raise _native.NativeError('serl_rollout: a trajectory produced a non-finite state / return (status flag)')
-
-
-TRACE_COLS = 22
-REPLAY_COLS = _native.REPLAY_COLS
 
 
 def variant_sorted_order(env_mode):
@@ -85,7 +91,6 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     activation."""
     if not weights.is_cuda:
         raise _native.NativeError('population_rollout needs CUDA tensors (no CPU fallback)')
-    L = _native.lib()
     pop, P = weights.shape
     assert weights.dtype == torch.float32 and weights.is_contiguous()
     assert P == (num_params_wide(widths) if widths else num_params(shape)), (P, widths)
@@ -112,8 +117,7 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
             r.trace = torch.full((pop, n_envs, horizon, TRACE_COLS), float('nan'), dtype=torch.float64, device=dev)
     elif r.status is not None:
         r.status.zero_()
-    stream = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-    p = lambda t: t.data_ptr() if t is not None else None
+    p = lambda t: t.data_ptr() if t is not None else None       # device memory owned by the caller or by r
     d = _native.RolloutDesc()
     d.d_weights, d.pop, d.shape = p(weights), pop, shape
     d.d_ref_levels, d.d_ref_starts, d.d_env_mode, d.n_envs, d.horizon = p(ref_levels), p(ref_starts), p(env_mode), n_envs, horizon
@@ -133,15 +137,14 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
         d.d_sensor_noise = p(sensor_noise)
     d.flags = _native.ROLLOUT_GUST if gust else 0       # some env flies the gust build (mode_code(...) & MODE_GUST)
     if widths:
-        warr = (ctypes.c_int32 * len(widths))(*[int(x) for x in widths])
-        d.widths, d.n_widths = ctypes.cast(warr, ctypes.c_void_p), len(widths)
-    _native.check(L.serl_rollout_run(ctypes.byref(d), stream), 'serl_rollout_run')
+        warr = np.asarray(widths, dtype=np.int32)       # host array, alive until the call returns
+        d.widths, d.n_widths = warr.ctypes.data, len(widths)
+    _native.call('serl_rollout_run', d, device=dev)
     return r
 
 
 def num_params_wide(widths):
-    arr = (ctypes.c_int32 * len(widths))(*[int(x) for x in widths])
-    return int(_native.lib().serl_actor_num_params_wide(arr, len(widths)))
+    return int(_native.lib().serl_actor_num_params_wide(np.asarray(widths, dtype=np.int32).ctypes, len(widths)))
 
 
 def actor_forward_wide(genome, widths, activation, obs):
@@ -151,10 +154,8 @@ def actor_forward_wide(genome, widths, activation, obs):
     assert genome.dtype == torch.float32 and genome.is_contiguous() and genome.numel() == num_params_wide(widths)
     assert obs.dtype == torch.float32 and obs.is_contiguous() and obs.shape[1] == 7
     out = torch.empty((obs.shape[0], 3), dtype=torch.float32, device=genome.device)
-    arr = (ctypes.c_int32 * len(widths))(*[int(x) for x in widths])
-    stream = ctypes.c_void_p(torch.cuda.current_stream(genome.device).cuda_stream)
-    _native.check(_native.lib().serl_actor_forward_wide(_ptr(genome), arr, len(widths), _native.ACTIVATIONS[activation.lower()], _ptr(obs),
-                                                        obs.shape[0], _ptr(out), stream), 'serl_actor_forward_wide')
+    act = _native.ACTIVATIONS[activation.lower()]
+    _native.call('serl_actor_forward_wide', genome, np.asarray(widths, dtype=np.int32), len(widths), act, obs, obs.shape[0], out)
     return out
 
 
@@ -166,21 +167,40 @@ def actor_forward(genome, shape, obs):
     assert genome.dtype == torch.float32 and genome.is_contiguous() and genome.numel() == num_params(shape)
     assert obs.dtype == torch.float32 and obs.is_contiguous() and obs.shape[1] == shape.state_dim
     out = torch.empty((obs.shape[0], shape.action_dim), dtype=torch.float32, device=genome.device)
-    stream = ctypes.c_void_p(torch.cuda.current_stream(genome.device).cuda_stream)
-    _native.check(_native.lib().serl_actor_forward(_ptr(genome), ctypes.byref(shape), _ptr(obs), obs.shape[0], _ptr(out), stream),
-                  'serl_actor_forward')
+    _native.call('serl_actor_forward', genome, shape, obs, obs.shape[0], out)
     return out
 
 
 def smoothness(actions, steps, dt=0.01):
     """K6: per-trajectory action smoothness (core/utils.py calc_smoothness) of `actions` [..., horizon, 3] fp32 (cuda) over the
     first `steps` [...] executed steps. Returns f64 tensor shaped like `steps`."""
-    L = _native.lib()
     horizon = actions.shape[-2]
     n = steps.numel()
     assert actions.is_cuda and actions.dtype == torch.float32 and actions.is_contiguous() and actions.numel() == n * horizon * 3
     st = steps.contiguous().to(torch.int32)
     out = torch.empty(st.shape, dtype=torch.float64, device=actions.device)
-    stream = ctypes.c_void_p(torch.cuda.current_stream(actions.device).cuda_stream)
-    _native.check(L.serl_smoothness(_ptr(actions), _ptr(st), n, horizon, dt, _ptr(out), stream), 'serl_smoothness')
+    _native.call('serl_smoothness', actions, st, n, horizon, dt, out)
     return out
+
+
+def plant_init(variant):
+    """serl_plant_init: the initial conditions [n, 19] f64 of the plant variants `variant` [n] int32 (cuda)."""
+    X = torch.empty((variant.shape[0], 19), dtype=torch.float64, device=variant.device)
+    _native.call('serl_plant_init', X, variant, X.shape[0])
+    return X
+
+
+def plant_step(X, cmd, variant, call=None):
+    """one 0.01 s step of the plants X [n, 19] f64 under cmd [n, 3] f64; variant [n] int32, or timed_plant_code values with call [n]"""
+    if call is None:
+        _native.call('serl_plant_step', X, cmd, variant, X.shape[0])
+    else:
+        _native.call('serl_plant_step_timed', X, cmd, variant, call, X.shape[0])
+
+
+@functools.cache        # only the first call per variant waits for the current stream (DESIGN §6: Agent._collect)
+def initial_state(variant):
+    """the 12 flight states (read-only host f64) plant variant `variant` starts from"""
+    x = plant_init(torch.tensor([variant], dtype=torch.int32, device='cuda'))[0, :12].cpu().numpy()
+    x.flags.writeable = False
+    return x

@@ -1,5 +1,4 @@
 """The reference-facing surface on the GPU: batched plant C-ABI, CitationEnv per-step API, Agent.evaluate / train."""
-import ctypes
 import os
 import random
 import types
@@ -29,14 +28,11 @@ def make_args(pop=6, hidden=16, **kw):
 
 @pytest.mark.parametrize('variant', ['h2000_v90', 'ice', 'cg'])
 def test_plant_step_kernel_matches_oracle(variant):
-    from serl_b200 import _native, rollout
-    L = _native.lib()
+    from serl_b200 import rollout
     dev = torch.device('cuda:0')
     n = 5
     v = torch.full((n,), rollout.PLANT_VARIANTS.index(variant), dtype=torch.int32, device=dev)
-    X = torch.empty((n, 19), dtype=torch.float64, device=dev)
-    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    _native.check(L.serl_plant_init(ctypes.c_void_p(X.data_ptr()), ctypes.c_void_p(v.data_ptr()), n, st), 'init')
+    X = rollout.plant_init(v)
     pl = OP.PortPlant(variant)
     assert np.array_equal(X.cpu().numpy()[0], pl.initial_state())
     rng = np.random.RandomState(0)
@@ -45,7 +41,7 @@ def test_plant_step_kernel_matches_oracle(variant):
     for k in range(200):
         cmd = 0.08 * rng.uniform(-1, 1, (n, 3))
         d = torch.as_tensor(cmd, device=dev)
-        _native.check(L.serl_plant_step(ctypes.c_void_p(X.data_ptr()), ctypes.c_void_p(d.data_ptr()), ctypes.c_void_p(v.data_ptr()), n, st), 'step')
+        rollout.plant_step(X, d, v)
         for i in range(n):
             _, Xo[i] = pl.step(Xo[i], np.concatenate([cmd[i], np.zeros(7)]))
     got = X.cpu().numpy()
@@ -60,13 +56,11 @@ def test_timed_plant_step_api_flies_the_gust_pulse_like_the_binary(build):
     """serl_plant_step_timed with SERL_MODE_GUST (the per-step path of CitationEnv in 'gust' mode): one-step predictions from
     the binary's own states through both edges of the pulse (native calls 1996..2003, 2296..2303) and in its middle.  The
     binary's states before and after each of those calls are stored in tests/golden/refbin_kat.npz."""
-    from serl_b200 import _native, rollout
-    L = _native.lib()
+    from serl_b200 import rollout
     dev = torch.device('cuda:0')
-    st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
     kat = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'refbin_kat.npz'))
     X0, X1 = kat['timed_%s_X0' % build], kat['timed_%s_X1' % build]          # envs/test: the same pulse with the opposite sign
-    var = torch.tensor([rollout.mode_code(build) & ~0xff00], dtype=torch.int32, device=dev)
+    var = torch.tensor([rollout.timed_plant_code(rollout.mode_code(build))], dtype=torch.int32, device=dev)
     live = [0, 1, 2, 3, 4, 5, 6, 7, 9, 12, 15, 16, 17, 18]
     worst, changed = 0.0, 0
     ks = [k for k in range(2306) if 1996 <= k <= 2003 or 2296 <= k <= 2303 or k == 2150]
@@ -76,12 +70,10 @@ def test_timed_plant_step_api_flies_the_gust_pulse_like_the_binary(build):
         Xd = torch.as_tensor(X0[w][None].copy(), device=dev)
         d = torch.as_tensor(cmd[None].copy(), device=dev)
         call = torch.tensor([k], dtype=torch.int32, device=dev)
-        _native.check(L.serl_plant_step_timed(ctypes.c_void_p(Xd.data_ptr()), ctypes.c_void_p(d.data_ptr()), ctypes.c_void_p(var.data_ptr()),
-                                              ctypes.c_void_p(call.data_ptr()), 1, st), 'serl_plant_step_timed')
+        rollout.plant_step(Xd, d, var, call)
         call0 = torch.tensor([0], dtype=torch.int32, device=dev)
         Xn = torch.as_tensor(X0[w][None].copy(), device=dev)
-        _native.check(L.serl_plant_step_timed(ctypes.c_void_p(Xn.data_ptr()), ctypes.c_void_p(d.data_ptr()), ctypes.c_void_p(var.data_ptr()),
-                                              ctypes.c_void_p(call0.data_ptr()), 1, st), 'serl_plant_step_timed')
+        rollout.plant_step(Xn, d, var, call0)
         X = X1[w]
         got = Xd.cpu().numpy()[0]
         worst = max(worst, np.abs(got[live] - X[live]).max())
