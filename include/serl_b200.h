@@ -215,4 +215,7 @@ const char* serl_last_error(void);
 #ifdef __cplusplus
 }
 #endif
+
+/* K7, the fused TD3 learner (serl_td3_train, serl_td3_state_floats) */
+#include "serl_td3.h"
 #endif

@@ -1,6 +1,7 @@
 """ctypes binding of the C-ABI library (include/serl_b200.h): the only module that binds it.  The product path has no CPU
 fallback: importing succeeds without a GPU (so host logic is testable), but the library must exist and every compute call
-fails loudly when CUDA is unavailable.  tests/test_capi.py holds the signatures and constants below to the header."""
+fails loudly when CUDA is unavailable.  tests/test_capi.py holds the signatures and constants below to the header,
+tests/test_td3_oracle.py those of include/serl_td3.h (TD3_SIGNATURES, TD3Desc, TD3_*)."""
 import ctypes
 import os
 
@@ -20,6 +21,11 @@ MODE_GUST_UP = 1 << 25
 ROLLOUT_GUST = 1
 STATUS_NONFINITE = 1
 STATUS_GUST_FLAG = 2
+# include/serl_td3.h (K7, the fused TD3 learner)
+TD3_CRITIC_HIDDEN = 64
+TD3_MAX_BATCH = 128
+TD3_CHAMPION_TARGET = 1
+TD3_STATUS_INDEX = 4
 
 
 class ActorShape(ctypes.Structure):
@@ -39,6 +45,21 @@ class RolloutDesc(ctypes.Structure):
                 ('d_status', ctypes.c_void_p), ('sm_limit', ctypes.c_int32),
                 ('widths', ctypes.c_void_p), ('n_widths', ctypes.c_int32), ('d_sensor_noise', ctypes.c_void_p),
                 ('flags', ctypes.c_int32)]
+
+
+class TD3Desc(ctypes.Structure):
+    """serl_td3_desc (include/serl_td3.h)"""
+    _fields_ = [('shape', ActorShape), ('d_state', ctypes.c_void_p),
+                ('d_replay', ctypes.c_void_p), ('replay_cols', ctypes.c_int32), ('n_valid', ctypes.c_int32),
+                ('batch', ctypes.c_int32), ('n_steps', ctypes.c_int32),
+                ('first_iteration', ctypes.c_int64), ('critic_adam_steps', ctypes.c_int64), ('actor_adam_steps', ctypes.c_int64),
+                ('gamma', ctypes.c_double), ('tau', ctypes.c_double), ('lr', ctypes.c_double), ('noise_sd', ctypes.c_double),
+                ('noise_clip', ctypes.c_double), ('policy_update_freq', ctypes.c_int32),
+                ('caps_lambda_t', ctypes.c_double), ('caps_lambda_s', ctypes.c_double), ('caps_eps_sd', ctypes.c_double),
+                ('max_grad_norm', ctypes.c_double), ('flags', ctypes.c_int32), ('seed', ctypes.c_uint64),
+                ('cluster_size', ctypes.c_int32), ('d_indices', ctypes.c_void_p), ('d_losses', ctypes.c_void_p),
+                ('d_rec_indices', ctypes.c_void_p), ('d_rec_noise', ctypes.c_void_p), ('d_rec_caps', ctypes.c_void_p),
+                ('d_status', ctypes.c_void_p)]
 
 
 _vp, _i32, _i64, _f64, _int, _shape = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_double, ctypes.c_int, ctypes.POINTER(ActorShape)
@@ -67,6 +88,11 @@ SIGNATURES = {
     'serl_launch_count': (_i64, []),
     'serl_last_error': (ctypes.c_char_p, []),
 }
+# the entry points of include/serl_td3.h (included by serl_b200.h), bound the same way
+TD3_SIGNATURES = {
+    'serl_td3_state_floats': (_i64, [_shape]),
+    'serl_td3_train': (_int, [ctypes.POINTER(TD3Desc), _vp]),
+}
 _lib = None
 
 
@@ -81,7 +107,7 @@ def lib():
             raise NativeError('serl_b200: %s is missing — build it with `python -m serl_b200.build` '
                               '(there is no CPU fallback)' % LIB_PATH)
         L = ctypes.CDLL(LIB_PATH)
-        for name, (restype, argtypes) in SIGNATURES.items():
+        for name, (restype, argtypes) in {**SIGNATURES, **TD3_SIGNATURES}.items():
             f = getattr(L, name)
             f.restype, f.argtypes = restype, argtypes
         _lib = L

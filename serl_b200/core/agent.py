@@ -54,7 +54,11 @@ class Agent:
             raise NativeError('serl_b200.Agent needs a CUDA device: the rollout / evolution engine has no CPU fallback')
         self.device = torch.device('cuda', torch.cuda.current_device())
         self.pop = PopulationList(args, self.device) if args.pop_size else []
-        self.rl_agent = td3.TD3(args)
+        if getattr(args, 'fused_td3', False):
+            from ..td3_fused import FusedTD3
+            self.rl_agent = FusedTD3(args)
+        else:
+            self.rl_agent = td3.TD3(args)
         self.replay_buffer = replay_memory.DeviceReplayMemory(args.buffer_size, self.device, seed=int(getattr(args, 'seed', 7)))
         self.noise_process = mod_utils.GaussianNoise(args.action_dim, sd=args.noise_sd)
         if len(self.pop):
@@ -222,6 +226,8 @@ class Agent:
             self.rl_agent.actor.train()
             if self.args.use_champion_target and self.champion_actor is not None:
                 self.evo_to_rl(self.rl_agent.actor_target, self.champion_actor)
+            if getattr(self.args, 'fused_td3', False):
+                return self._train_rl_fused(int(rl_transitions * self.args.frac_frames_train))
             for _ in range(int(rl_transitions * self.args.frac_frames_train)):
                 self.rl_iteration += 1
                 batch = self.replay_buffer.sample(self.args.batch_size)
@@ -231,6 +237,16 @@ class Agent:
                 if TD is not None:
                     TD_loss.append(TD)
         return {'PG_obj': np.mean(pgs_obj) if pgs_obj else float('nan'), 'TD_loss': np.median(TD_loss) if TD_loss else float('nan')}
+
+    def _train_rl_fused(self, n):
+        """train_rl's loop as K7 launches; the statistics come from ONE device->host copy of the losses"""
+        if n <= 0:
+            return {'PG_obj': float('nan'), 'TD_loss': float('nan')}
+        first = self.rl_iteration + 1
+        losses = self.rl_agent.train_steps(self.replay_buffer, n, first, self.args.use_champion_target).cpu().numpy()
+        self.rl_iteration += n
+        pg = losses[(np.arange(first, first + n) % self.args.policy_update_freq) == 0, 1]
+        return {'PG_obj': np.mean(-pg) if pg.size else float('nan'), 'TD_loss': np.median(losses[:, 0])}
 
     @staticmethod
     def _validation_stats(eps):

@@ -16,7 +16,7 @@ constexpr size_t SERL_SMEM_OPTIN = 227 * 1024;
 int serl_device_sms();
 
 // what a scratch buffer holds; launches of different purposes never share one
-enum { SERL_SCRATCH_K1 = 0, SERL_SCRATCH_K6 = 1, SERL_SCRATCH_TC = 2 };
+enum { SERL_SCRATCH_K1 = 0, SERL_SCRATCH_K6 = 1, SERL_SCRATCH_TC = 2, SERL_SCRATCH_TD3 = 3 };
 // a device buffer of at least `bytes` for launches of `purpose` on stream `s` of the current device
 cudaError_t serl_scratch(int purpose, cudaStream_t s, size_t bytes, void** out);
 

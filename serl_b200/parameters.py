@@ -46,6 +46,8 @@ class Parameters:
         self.use_caps = g('use_caps', True)
         self.policy_update_freq = 3
         self.noise_clip = 0.5
+        # the RL half's gradient steps in one K7 launch per generation (serl_b200/td3_fused.py) instead of the torch loop
+        self.fused_td3 = bool(g('fused_td3', False))
         # neuro-evolution — parameters.py:76-116
         self.pop_size = g('pop_size', 10)
         self.use_champion_target = g('champion_target', False)

@@ -1,0 +1,135 @@
+"""The TD3 learner on the device: K7 (csrc/td3.cu) takes a generation's gradient steps in one launch.
+
+`FusedTD3` has TD3's interface (core/td3.py: actor / actor_target / critic / critic_target / buffer / critical_buffer,
+update_parameters) and computes the same update up to fp32 summation order.  Every parameter of the four modules is a view
+into one flat device buffer, the kernel's learner state (include/serl_td3.h), so state_dict(), rl_to_evo / evo_to_rl copies,
+save_agent and the critic handed to SSNE read and write the live weights.  The torch Adam optimisers are not used: the Adam
+moments live in the same buffer and the step counts in `critic_steps` / `actor_steps`."""
+import ctypes
+
+import numpy as np
+import torch
+
+from . import _native
+from .core import td3
+from .core.replay_memory import TRANSITION_COLS
+from .rollout import actor_shape
+
+# steps per launch: keeps every launch well under a second at the largest population
+LAUNCH_STEPS = 8192
+
+
+class TD3Launch:
+    """what one or more K7 launches returned: losses [n, 2] (td, pg; pg NaN on critic-only steps), the recorded draws
+    (indices [n, B] int32, noise [n, B, 3], caps [n, B, 7]) when asked for, and the status word."""
+    __slots__ = ('losses', 'indices', 'noise', 'caps', 'status')
+
+    def check(self):
+        st = int(self.status.item())
+        if st & _native.STATUS_NONFINITE:
+            raise _native.NativeError('serl_td3_train: a loss became NaN or infinite')
+        if st & _native.TD3_STATUS_INDEX:
+            raise _native.NativeError('serl_td3_train: a given row index was outside the replay rows')
+
+
+def state_floats(shape):
+    n = int(_native.lib().serl_td3_state_floats(ctypes.byref(shape)))
+    if n < 0:
+        raise _native.NativeError('serl_td3_state_floats: ' + _native.lib().serl_last_error().decode())
+    return n
+
+
+class FusedTD3(td3.TD3):
+    def __init__(self, args, cluster_size=0, seed=None):
+        super().__init__(args)
+        if torch.device(args.device).type != 'cuda':
+            raise _native.NativeError('FusedTD3 needs a CUDA device (no CPU fallback)')
+        self.actor_optim = self.critic_optim = None            # Adam runs inside the kernel
+        self.shape = actor_shape(args.hidden_size, args.num_layers, args.activation_actor, args.state_dim, args.action_dim)
+        self.cluster_size = int(cluster_size)
+        self.seed = int(getattr(args, 'seed', 7) if seed is None else seed)
+        self.critic_steps = self.actor_steps = 0
+        dev = next(self.actor.parameters()).device
+        self.state = torch.zeros(state_floats(self.shape), dtype=torch.float32, device=dev)
+        pa, pc = (sum(q.numel() for q in m.parameters()) for m in (self.actor, self.critic))
+        assert 4 * pa + 4 * pc == self.state.numel()
+        # actor θ | actor target | actor m | actor v | critic θ | critic target | critic m | critic v
+        for mod, off, k in ((self.actor, 0, pa), (self.actor_target, pa, pa), (self.critic, 4 * pa, pc), (self.critic_target, 4 * pa + pc, pc)):
+            _bind(mod, self.state[off:off + k])
+        self.status = torch.zeros(1, dtype=torch.int32, device=dev)
+
+    def run(self, rows, n_valid, n, first_iteration, champion_target=False, indices=None, record=False, cluster_size=None):
+        """n consecutive gradient steps on global iterations first_iteration.. (launches of at most LAUNCH_STEPS) on the replay
+        rows [>= n_valid, >= 19] fp32 (device, row-contiguous).  indices [n, B] int32 replaces the sampler's draw."""
+        a = self.args
+        B = int(a.batch_size)
+        dev = self.state.device
+        assert rows.is_cuda and rows.dtype == torch.float32 and rows.dim() == 2 and rows.shape[1] >= TRANSITION_COLS
+        assert rows.stride(1) == 1 and rows.shape[0] >= n_valid
+        r = TD3Launch()
+        r.losses = torch.empty((n, 2), dtype=torch.float32, device=dev)
+        r.indices = torch.empty((n, B), dtype=torch.int32, device=dev) if record else None
+        r.noise = torch.empty((n, B, 3), dtype=torch.float32, device=dev) if record else None
+        r.caps = torch.empty((n, B, 7), dtype=torch.float32, device=dev) if record else None
+        r.status = self.status
+        self.status.zero_()
+        if indices is not None:
+            assert indices.shape == (n, B) and indices.dtype == torch.int32 and indices.is_cuda and indices.is_contiguous()
+        caps = self.caps_dict or {'lambda_t': 0.0, 'lambda_s': 0.0, 'eps_sd': 0.0}
+        p = lambda t, k0: t[k0:].data_ptr() if t is not None else None
+        k0 = 0
+        while k0 < n:
+            m = min(LAUNCH_STEPS, n - k0)
+            d = _native.TD3Desc()
+            d.shape, d.d_state = self.shape, self.state.data_ptr()
+            d.d_replay, d.replay_cols, d.n_valid = rows.data_ptr(), rows.stride(0), int(n_valid)
+            d.batch, d.n_steps = B, m
+            d.first_iteration, d.critic_adam_steps, d.actor_adam_steps = int(first_iteration) + k0, self.critic_steps, self.actor_steps
+            d.gamma, d.tau, d.lr, d.noise_sd, d.noise_clip = a.gamma, a.tau, a.lr, a.noise_sd, a.noise_clip
+            d.policy_update_freq = int(a.policy_update_freq)
+            d.caps_lambda_t, d.caps_lambda_s, d.caps_eps_sd = caps['lambda_t'], caps['lambda_s'], caps['eps_sd']
+            d.max_grad_norm = float(td3.MAX_GRAD_NORM)
+            d.flags = _native.TD3_CHAMPION_TARGET if champion_target else 0
+            d.seed, d.cluster_size = self.seed, int(self.cluster_size if cluster_size is None else cluster_size)
+            d.d_indices = p(indices, k0)
+            d.d_losses = p(r.losses, k0)
+            d.d_rec_indices, d.d_rec_noise, d.d_rec_caps = p(r.indices, k0), p(r.noise, k0), p(r.caps, k0)
+            d.d_status = self.status.data_ptr()
+            _native.call('serl_td3_train', d, device=dev)
+            its = np.arange(int(first_iteration) + k0, int(first_iteration) + k0 + m)
+            self.critic_steps += m
+            self.actor_steps += int((its % int(a.policy_update_freq) == 0).sum())
+            k0 += m
+        if n:
+            # the kernel wrote the weights behind autograd's back: bump the parameters' version counters, so that anything
+            # keyed on them (Agent's prefetched generation front) sees the change
+            for mod in (self.actor, self.actor_target, self.critic, self.critic_target):
+                for q in mod.parameters():
+                    torch.autograd.graph.increment_version(q)
+        return r
+
+    def train_steps(self, replay, n, first_iteration, champion_target=False):
+        """n gradient steps sampling from `replay` (DeviceReplayMemory, or a [rows, >= 19] device tensor); returns the device
+        losses [n, 2] (td, pg; pg NaN on critic-only steps)."""
+        rows, n_valid = (replay.data, len(replay)) if hasattr(replay, 'data') else (replay, replay.shape[0])
+        return self.run(rows, n_valid, int(n), first_iteration, champion_target).losses
+
+    def update_parameters(self, batch, iteration, champion_policy=False):
+        """one step on the given batch (state, action, next_state, reward, done), as TD3.update_parameters"""
+        dev = self.state.device
+        rows = torch.cat([b.to(dev, torch.float32).reshape(b.shape[0], -1) for b in batch], 1).contiguous()
+        B = rows.shape[0]
+        assert B == int(self.args.batch_size)
+        idx = torch.arange(B, dtype=torch.int32, device=dev).reshape(1, B)
+        out = self.run(rows, B, 1, iteration, champion_policy, indices=idx).losses[0].cpu().numpy()
+        return (out[1] if iteration % self.args.policy_update_freq == 0 else None), out[0]
+
+
+def _bind(module, flat):
+    off = 0
+    for q in module.parameters():
+        k = q.numel()
+        flat[off:off + k].copy_(q.data.reshape(-1))
+        q.data = flat[off:off + k].view(q.shape)
+        off += k
+    assert off == flat.numel()
