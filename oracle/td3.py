@@ -3,7 +3,10 @@
 `update_parameters(agent, rows, iteration, noise, caps_u, champion_policy)` performs the same torch operations in the same
 order as TD3.update_parameters on a TD3 instance `agent` (its modules and its torch Adam optimisers), with the clipped
 target-policy noise and the CAPS uniforms given instead of drawn: fed the draws TD3 itself would have made, it reproduces
-it bit for bit (tests/test_td3_oracle.py); fed the draws K7 recorded, it is the reference the kernel is held to."""
+it bit for bit (tests/test_td3_oracle.py); fed the draws K7 recorded, it is the reference the kernel is held to.
+`as_float64(agent)` is its float64 copy, the sharper reference of tests/test_td3_reference_gpu.py."""
+import copy
+
 import torch
 from torch import nn
 from torch.nn import functional as F
@@ -22,9 +25,27 @@ def split(rows):
     return tuple(out)
 
 
-def update_parameters(agent, rows, iteration, noise, caps_u=None, champion_policy=False):
+def as_float64(agent):
+    """a deep copy of the TD3 `agent` in float64: the four modules in .double(), both Adam optimisers rebuilt on the double
+    parameters and given a copy of the original state (load_state_dict casts exp_avg / exp_avg_sq to the parameter dtype
+    and keeps `step`; the copy keeps the two optimisers from sharing their CPU `step` tensors, which Adam increments in
+    place).  Fed the same draws (in float64), it is the high-precision reference of the fp32 update."""
+    d = copy.deepcopy(agent)
+    for m in (d.actor, d.actor_target, d.critic, d.critic_target):
+        m.double()
+    for name, mod in (('actor_optim', d.actor), ('critic_optim', d.critic)):
+        src = getattr(agent, name)
+        opt = type(src)(mod.parameters(), **src.defaults)
+        opt.load_state_dict(copy.deepcopy(src.state_dict()))
+        setattr(d, name, opt)
+    return d
+
+
+def update_parameters(agent, rows, iteration, noise, caps_u=None, champion_policy=False, norms=None):
     """rows [B, >= 19] transitions; noise [B, A] clipped target-policy noise; caps_u [B, S] U[0,1) draws (actor steps with
-    CAPS).  Returns (pg or None, td) as 0-d tensors."""
+    CAPS).  Returns (pg or None, td) as 0-d tensors.  A list `norms` receives the pre-clip gradient norms that
+    clip_grad_norm_ returned: the critic's, then on actor iterations the actor's."""
+    norms = [] if norms is None else norms
     state, action, next_state, reward, done = split(rows)
     with torch.no_grad():
         next_action = torch.clamp(noise + agent.actor_target(next_state), -1, 1)
@@ -34,7 +55,7 @@ def update_parameters(agent, rows, iteration, noise, caps_u=None, champion_polic
     td = F.mse_loss(cq1, target_q) + F.mse_loss(cq2, target_q)
     agent.critic_optim.zero_grad()
     td.backward()
-    nn.utils.clip_grad_norm_(agent.critic.parameters(), MAX_GRAD_NORM)
+    norms.append(float(nn.utils.clip_grad_norm_(agent.critic.parameters(), MAX_GRAD_NORM)))
     agent.critic_optim.step()
     pgl = None
     if iteration % agent.args.policy_update_freq == 0:
@@ -45,7 +66,7 @@ def update_parameters(agent, rows, iteration, noise, caps_u=None, champion_polic
             bar = agent.actor(state + caps_u * agent.caps_dict['eps_sd'])
             loss = loss + agent.caps_dict['lambda_t'] * F.mse_loss(action, nxt) + agent.caps_dict['lambda_s'] * F.mse_loss(action, bar)
         loss.backward()
-        nn.utils.clip_grad_norm_(agent.actor.parameters(), MAX_GRAD_NORM)
+        norms.append(float(nn.utils.clip_grad_norm_(agent.actor.parameters(), MAX_GRAD_NORM)))
         agent.actor_optim.step()
         if not champion_policy:
             soft_update(agent.actor_target, agent.actor, agent.tau)
