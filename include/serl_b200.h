@@ -108,10 +108,12 @@ int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shap
  *   d_status     optional int32 word the kernel ORs error bits into (SERL_STATUS_*); the caller zeroes it and reads it
  *                after synchronising
  *   widths       HOST pointer to n_widths hidden-layer widths, or NULL.  n_widths == 0: the reference's uniform actor described
- *                by `shape` (K1, warp-GEMV on CUDA cores).  n_widths == 2: the two-hidden-layer generalisation
- *                Linear(7,w1) act Linear(w1,w2) LayerNorm act Linear(w2,3) tanh (BASELINE config 5: [400,300], [128,128]);
+ *                by `shape` (K1, warp-GEMV on CUDA cores).  2 <= n_widths <= 9: the width-list generalisation
+ *                Linear(7,w0) act {Linear(w_{i-1},w_i) LayerNorm act} for i = 1..n-1, Linear(w_{n-1},3) tanh (BASELINE config 5:
+ *                [400,300], [128,128]; the reference's Actor at num_layers = L is [h] * (L + 1), see serl_actor_tc_widths);
+ *                8 <= w0 <= 1024, 8 <= w_i <= 320, SERL_ERR_UNSUPPORTED when the list's buffers exceed an SM's shared memory;
  *                genome = parameters() order, serl_actor_num_params_wide floats per actor; only shape.activation is read
- *                from `shape`; layer 2 runs on the tensor cores (wgmma, 3xTF32) with TMA-streamed weight slabs
+ *                from `shape`; layers 1..n-1 run on the tensor cores (wgmma, 3xTF32) with TMA-streamed weight slabs
  *   d_sensor_noise optional [pop, n_envs, horizon + 1, 7] fp32 standard-normal draws: the sensor-noise shim of
  *                envs/noise/citation.py:72-82 (mode 'noise'; also the outputs of envs/gust) applied to every native step
  *                output — row 0 for reset()'s step, row k + 1 for env step k; order p,q,r, alpha, beta, phi, theta
@@ -218,4 +220,6 @@ const char* serl_last_error(void);
 
 /* K7, the fused TD3 learner (serl_td3_train, serl_td3_state_floats) */
 #include "serl_td3.h"
+/* the kernel of a uniform actor: K1, or K1-TC with the widths [h] * (L + 1) (serl_actor_tc_widths) */
+#include "serl_route.h"
 #endif

@@ -1,7 +1,8 @@
 """ctypes binding of the C-ABI library (include/serl_b200.h): the only module that binds it.  The product path has no CPU
 fallback: importing succeeds without a GPU (so host logic is testable), but the library must exist and every compute call
 fails loudly when CUDA is unavailable.  tests/test_capi.py holds the signatures and constants below to the header,
-tests/test_td3_oracle.py those of include/serl_td3.h (TD3_SIGNATURES, TD3Desc, TD3_*)."""
+tests/test_td3_oracle.py those of include/serl_td3.h (TD3_SIGNATURES, TD3Desc, TD3_*), tests/test_deep_actor.py those of
+include/serl_route.h (ROUTE_SIGNATURES)."""
 import ctypes
 import os
 
@@ -93,6 +94,10 @@ TD3_SIGNATURES = {
     'serl_td3_state_floats': (_i64, [_shape]),
     'serl_td3_train': (_int, [ctypes.POINTER(TD3Desc), _vp]),
 }
+# include/serl_route.h: the kernel of a uniform actor (host only, no stream)
+ROUTE_SIGNATURES = {
+    'serl_actor_tc_widths': (_i32, [_shape, _vp, _i32]),
+}
 _lib = None
 
 
@@ -107,7 +112,7 @@ def lib():
             raise NativeError('serl_b200: %s is missing — build it with `python -m serl_b200.build` '
                               '(there is no CPU fallback)' % LIB_PATH)
         L = ctypes.CDLL(LIB_PATH)
-        for name, (restype, argtypes) in {**SIGNATURES, **TD3_SIGNATURES}.items():
+        for name, (restype, argtypes) in {**SIGNATURES, **TD3_SIGNATURES, **ROUTE_SIGNATURES}.items():
             f = getattr(L, name)
             f.restype, f.argtypes = restype, argtypes
         _lib = L

@@ -761,6 +761,34 @@ static bool warp_hidden(int H, F&& f)
 }
 static bool warp_hidden(int H) { return warp_hidden(H, [](auto) {}); }
 
+// K1's kernel for a valid shape: the warp actor when the hidden size is instantiated and the genome fits one slot, else the
+// one-thread-per-env kernel, which needs the genome and two activation buffers of 128 envs in shared memory
+static bool k1_warp(const serl_actor_shape& sh)
+{
+    const size_t P4 = ((size_t)serl_actor_num_params(&sh) + 3) & ~(size_t)3;
+    return !force_simple() && warp_hidden(sh.hidden) && P4 * 4 <= SERL_SMEM_OPTIN;
+}
+static bool k1_fits(const serl_actor_shape& sh)
+{
+    const size_t P4 = ((size_t)serl_actor_num_params(&sh) + 3) & ~(size_t)3;
+    return k1_warp(sh) || P4 * 4 + 2ull * sh.hidden * 128 * 4 <= SERL_SMEM_OPTIN;
+}
+
+// Which kernel flies a uniform actor: 0 when K1 does (or reports why it cannot: a shape outside the task, L = 0), else
+// the L + 1 widths [h] * (L + 1) of the same genome for K1-TC
+extern "C" int32_t serl_actor_tc_widths(const serl_actor_shape* shape, int32_t* widths_out, int32_t cap)
+{
+    if (!shape) return serl_fail(SERL_ERR_ARG, "serl_actor_tc_widths: null shape");
+    const serl_actor_shape& sh = *shape;
+    const bool task = sh.state_dim == 7 && sh.action_dim == 3 && sh.hidden >= 2 && sh.num_layers >= 1 && sh.activation >= 0 &&
+                      sh.activation <= 2;
+    if (!task || (actor_shape_ok(sh) && k1_fits(sh))) return 0;
+    const int n = sh.num_layers + 1;
+    if (!widths_out || cap < n) return serl_fail(SERL_ERR_ARG, "serl_actor_tc_widths: widths_out holds fewer than num_layers + 1 widths");
+    for (int i = 0; i < n; ++i) widths_out[i] = sh.hidden;
+    return n;
+}
+
 // K1 launch: the checks only this kernel needs, then the genome part of the argument block and the kernel for the hidden size
 static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t s)
 {
@@ -771,9 +799,9 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
     const int H = d.shape.hidden;
     ar.weights = d.d_weights; ar.P = (int)serl_actor_num_params(&d.shape); ar.sh = d.shape;
     ar.P4 = (ar.P + 3) & ~3;
-    if (force_simple() || !warp_hidden(H) || (size_t)ar.P4 * 4 > SERL_SMEM_OPTIN) {
+    if (!k1_warp(d.shape)) {
+        if (!k1_fits(d.shape)) return serl_fail(SERL_ERR_UNSUPPORTED, "serl_rollout: genome + activations exceed 227 KB of shared memory");
         const size_t smem = (size_t)ar.P4 * 4 + 2ull * H * 128 * 4;
-        if (smem > SERL_SMEM_OPTIN) return serl_fail(SERL_ERR_UNSUPPORTED, "serl_rollout: genome + activations exceed 227 KB of shared memory");
         return serl_launch("rollout_kernel launch", rollout_kernel_simple, dim3((d.n_envs + 127) / 128, d.pop), 128, smem, s, ar);
     }
     // as many genome slots per CTA as shared memory holds next to the plant tables (h <= 72: two; h = 96: one);

@@ -87,10 +87,13 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     env_order: optional int32 [n_envs] permutation (see variant_sorted_order); replay_env: record the transitions of that env
     of every actor into result.replay [pop, horizon, REPLAY_COLS]; status: carry the device status word (result.check());
     sm_limit: SMs this launch may occupy (0 = all); fitness=False skips the per-actor mean kernel.
-    widths=[w1, w2]: wide two-hidden-layer actors on the tensor-core kernel (csrc/rollout_tc.cu); `shape` then only supplies the
-    activation."""
+    widths=[w0, w1, ..., w_{n-1}] (2 to 9 widths): width-list actors on the tensor-core kernel K1-TC (csrc/rollout_tc.cu); `shape`
+    then only supplies the activation.  widths=None flies the uniform actor `shape` on K1, or on K1-TC with [h] * (L + 1) when its
+    genome does not fit K1's kernels (tc_widths)."""
     if not weights.is_cuda:
         raise _native.NativeError('population_rollout needs CUDA tensors (no CPU fallback)')
+    if widths is None:
+        widths = tc_widths(shape)
     pop, P = weights.shape
     assert weights.dtype == torch.float32 and weights.is_contiguous()
     assert P == (num_params_wide(widths) if widths else num_params(shape)), (P, widths)
@@ -143,12 +146,22 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     return r
 
 
+def tc_widths(shape):
+    """None when K1 flies the uniform actor `shape` (or reports why it cannot), else the width list [h] * (L + 1) of the same
+    genome for K1-TC (serl_actor_tc_widths: K1's fit rule lives in csrc/rollout.cu)"""
+    out = np.zeros(max(shape.num_layers + 1, 1), dtype=np.int32)
+    n = _native.lib().serl_actor_tc_widths(shape, out.ctypes, out.size)
+    _native.check(min(n, 0), 'serl_actor_tc_widths')
+    return out[:n].tolist() if n else None
+
+
 def num_params_wide(widths):
     return int(_native.lib().serl_actor_num_params_wide(np.asarray(widths, dtype=np.int32).ctypes, len(widths)))
 
 
 def actor_forward_wide(genome, widths, activation, obs):
-    """forward pass of a wide [w1, w2] actor for a batch of observations through the tensor-core device code (wgmma 3xTF32)."""
+    """forward pass of a width-list actor [w0, ..., w_{n-1}] (2 to 9 widths) for a batch of observations through the tensor-core
+    device code (wgmma 3xTF32)."""
     if not genome.is_cuda:
         raise _native.NativeError('actor_forward_wide needs CUDA tensors (no CPU fallback)')
     assert genome.dtype == torch.float32 and genome.is_contiguous() and genome.numel() == num_params_wide(widths)
