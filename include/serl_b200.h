@@ -122,9 +122,13 @@ int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shap
  *   flags        SERL_ROLLOUT_GUST: some env of the launch flies the gust build (SERL_MODE_GUST) — selects the kernel
  *                instantiation with the gust schedule (the training instantiation carries no trace of it; a gust env in a launch
  *                without the flag sets SERL_STATUS_GUST_FLAG)
+ *                SERL_ROLLOUT_STAGGER: K1 launches with two genome slots per CTA run slot 1 half a step behind slot 0
+ *                instead of taking both slots' steps together.  Same result bits; slower on an H100 (DESIGN §5), kept to
+ *                compare the two schedules in one process
  * t_max <= 0 selects the training defaults (20 s, smooth width 3 s). */
 #define SERL_REPLAY_COLS 20
 #define SERL_ROLLOUT_GUST 1
+#define SERL_ROLLOUT_STAGGER 2
 enum { SERL_STATUS_NONFINITE = 1,     /* a trajectory's state / return became NaN or infinite */
        SERL_STATUS_GUST_FLAG = 2 };   /* an env has SERL_MODE_GUST but the launch was not made with SERL_ROLLOUT_GUST */
 typedef struct {

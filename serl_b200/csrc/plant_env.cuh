@@ -424,6 +424,7 @@ struct RolloutArgs {
     const float* wt;                // [pop][P4] genomes in the shared-memory layout (transposed matrices), 16-byte aligned rows
     int P4;                         // row stride of wt / smem slot size in floats (multiple of 4)
     int apc, wps;                   // genome slots per CTA, warps per slot
+    int stagger;                    // apc == 2: slot 1 runs half a step behind slot 0 (rollout_kernel_persist)
     int n_chunks;                   // env chunks of wps*32 lanes per actor
     long long n_tasks;              // pop * n_chunks
     long long n_slots;              // gridDim.x * apc

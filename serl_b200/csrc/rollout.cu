@@ -206,8 +206,12 @@ __device__ __noinline__ ActorAct actor_forward_warp(const float* __restrict__ w,
 #pragma unroll
     for (int m2 = 0; m2 < TM2; ++m2) {
         const float2 b = *reinterpret_cast<const float2*>(b0 + og * TM + 2 * m2);
+        AmF2x4 v;
 #pragma unroll
-        for (int c = 0; c < 4; ++c) in[m2][c] = am_act2<ACT>(am_fma2(acc[m2][c], am_splat(1.0f), b));
+        for (int c = 0; c < 4; ++c) v.v[c] = am_fma2(acc[m2][c], am_splat(1.0f), b);
+        v = am_act2x4<ACT>(v);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) in[m2][c] = v.v[c];
     }
     // hidden layers: Linear -> LayerNorm (unbiased std, eps on std; mod_utils.py:47-50) -> activation
 #pragma unroll 1
@@ -249,13 +253,17 @@ __device__ __noinline__ ActorAct actor_forward_warp(const float* __restrict__ w,
         for (int m2 = 0; m2 < TM2; ++m2) {
             const float2 g = *reinterpret_cast<const float2*>(gamma + og * TM + 2 * m2);
             const float2 be = *reinterpret_cast<const float2*>(beta + og * TM + 2 * m2);
+            AmF2x4 v;
 #pragma unroll
-            for (int c = 0; c < 4; ++c)
-                in[m2][c] = am_act2<ACT>(am_fma2(am_fma2(g, acc[m2][c], am_splat(-0.0f)), am_splat(den[c]), be));
+            for (int c = 0; c < 4; ++c) v.v[c] = am_fma2(am_fma2(g, acc[m2][c], am_splat(-0.0f)), am_splat(den[c]), be);
+            v = am_act2x4<ACT>(v);
+#pragma unroll
+            for (int c = 0; c < 4; ++c) in[m2][c] = v.v[c];
         }
     }
-    // output layer: partial dot products over this lane's neurons, reduced over the group; lane og keeps env 4g+og
-    ActorAct action;
+    // output layer: partial dot products over this lane's neurons, reduced over the group; lane og keeps env 4g+og.
+    // The three tanh go through two pair calls.
+    float y[A];
 #pragma unroll
     for (int j = 0; j < A; ++j) {
         float p[4] = {0.f, 0.f, 0.f, 0.f};
@@ -268,8 +276,12 @@ __device__ __noinline__ ActorAct actor_forward_warp(const float* __restrict__ w,
 #pragma unroll
         for (int c = 0; c < 4; ++c) p[c] = group_sum(p[c]);
         const float mine = og == 0 ? p[0] : (og == 1 ? p[1] : (og == 2 ? p[2] : p[3]));
-        action.v[j] = am_tanh1(__fadd_rn(mine, bo[j]));
+        y[j] = __fadd_rn(mine, bo[j]);
     }
+    static_assert(A == 3, "two tanh pairs");
+    const float2 t01 = am_tanh2(make_float2(y[0], y[1])), t2 = am_tanh2(make_float2(y[2], y[2]));
+    ActorAct action;
+    action.v[0] = t01.x; action.v[1] = t01.y; action.v[2] = t2.x;
     return action;
 }
 
@@ -388,11 +400,16 @@ rollout_kernel_persist(RolloutArgs ar)
     }
     // segments in the order: head of the last task (published) -> whole tasks -> tail of the first task (continued)
     long long t_cur = t_first + (k0 > 0 ? 1 : 0);
-    // LOCKSTEP: all warps of the CTA take their steps together (one CTA barrier per step).  The step body is ~130 KB of
-    // code at h = 72 (sm_90a SASS: actor 32 KB + the out-of-line tanh 0.8 KB, right-hand side 41 KB x 6 calls, ode5 step
-    // 16 KB, environment and segment bookkeeping up to 40 KB); eight warps drifting through it independently each stream it
-    // through the instruction caches on their own, and instruction fetch was the top stall (no_instruction 27 % of the warp
-    // samples on B200).  In lockstep a fetched line serves every warp of the SM.
+    // LOCKSTEP: all warps of the CTA meet at one CTA barrier per loop trip.  The step body is ~130 KB of code at h = 72
+    // (sm_90a SASS: actor 31 KB, right-hand side 41 KB x 6 calls, ode5 step 16 KB, environment and segment bookkeeping up
+    // to 40 KB); eight warps drifting through it independently each stream it through the instruction caches on their own,
+    // and instruction fetch was the top stall (no_instruction 27 % of the warp samples on B200).  Met at a barrier, a
+    // fetched line serves every warp of the SM that runs the same phase.
+    // STAGGER (ar.stagger, two slots): a trip is half a step.  Slot 0 runs its actor while slot 1 runs its environment
+    // step, then they swap, so that each SM sub-partition (one warp of each slot) has one warp on the fp32 pipe and one on
+    // the fp64 pipe instead of both on the same one.  A slot's step boundary (segment close / open, hand-over) comes
+    // before its actor half; the action stays in registers until the environment half.  Opt-in: on an H100 it is slower
+    // than lockstep (the plant is latency bound and slows down next to a warp in the actor; DESIGN §5).
     Env e;
     e.tab = tab;
     e.done = true; e.k = 0;
@@ -400,10 +417,14 @@ rollout_kernel_persist(RolloutArgs ar)
     bool in_seg = false, pending = false, to_h = false, valid = false, replay = false;
     int ke = 0, actor = 0;
     size_t traj = 0;
+    const bool stagger = ar.stagger != 0;
+    bool actor_half = !(stagger && slot_l == 1);       // slot-uniform; slot 1 starts with an empty environment half
     for (;;) {
         // is this slot's segment still flying?  (slot-uniform: OR over the slot's warps at its named barrier)
         bool slot_alive = false;
-        if (in_seg) {
+        if (!actor_half) {
+            slot_alive = true;                         // mid-step: the boundary comes with the next actor half
+        } else if (in_seg) {
             int any;
             asm volatile("{ .reg .pred p, q; setp.ne.s32 p, %1, 0; barrier.cta.red.or.pred q, %2, %3, p; selp.s32 %0, 1, 0, q; }"
                          : "=r"(any) : "r"((int)(!e.done && e.k < ke)), "r"(1 + slot_l), "r"(slot_threads) : "memory");
@@ -502,13 +523,13 @@ rollout_kernel_persist(RolloutArgs ar)
                 in_seg = true;
             }
         }
-        // the CTA's warps meet here once per step; the launch ends when no slot has a segment left
-        if (!__syncthreads_or(in_seg || pending)) break;
+        // the CTA's warps meet here once per trip; the launch ends when no slot has a segment left (stage < 3: slot 1's
+        // first, empty half of a staggered launch)
+        if (!__syncthreads_or(in_seg || pending || stage < 3)) break;
         const bool mine = in_seg && !e.done && e.k < ke;
-        if (__any_sync(0xffffffffu, mine)) {
-            actor_forward<H>(actfn, w, L, lane, xb, obs, a);
-            if (mine) env_step<TABS, GUST>(e, ar, traj, actor, replay, a, obs);
-        }
+        if (actor_half && __any_sync(0xffffffffu, mine)) actor_forward<H>(actfn, w, L, lane, xb, obs, a);
+        if ((!stagger || !actor_half) && mine) env_step<TABS, GUST>(e, ar, traj, actor, replay, a, obs);
+        actor_half ^= stagger;
     }
 }
 
@@ -697,7 +718,7 @@ static void choose_shape(int pop, int n_envs, int apc_max, int sms, int* apc_out
 }
 
 template <int H, bool TABS>
-static int launch_persist(RolloutArgs& ar, int apc_max, bool gust, cudaStream_t s)
+static int launch_persist(RolloutArgs& ar, int apc_max, bool gust, bool stagger, cudaStream_t s)
 {
     const int sms = ar.sm_limit > 0 && ar.sm_limit < serl_device_sms() ? ar.sm_limit : serl_device_sms();
     int apc, wps;
@@ -708,6 +729,7 @@ static int launch_persist(RolloutArgs& ar, int apc_max, bool gust, cudaStream_t 
     if (f_wps == 1 || f_wps == 2 || f_wps == 4) wps = f_wps;
     while (apc * wps * 32 > MAX_CTA_THREADS) --apc;
     ar.apc = apc; ar.wps = wps;
+    ar.stagger = apc == 2 && stagger;
     ar.n_chunks = (ar.n_envs + wps * 32 - 1) / (wps * 32);
     ar.n_tasks = (long long)ar.pop * ar.n_chunks;
     const long long grid = ar.n_tasks / apc < sms ? (ar.n_tasks + apc - 1) / apc : sms;
@@ -814,14 +836,14 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
     int apc_max = (int)(((tabs ? budget - tab_bytes : budget)) / slot_bytes);
     if (apc_max > 4) apc_max = 4;
     if (apc_max > 2 && H > 32) apc_max = 2;
-    const bool gust = (d.flags & SERL_ROLLOUT_GUST) != 0;
+    const bool gust = (d.flags & SERL_ROLLOUT_GUST) != 0, stagger = (d.flags & SERL_ROLLOUT_STAGGER) != 0;
     int rc = SERL_OK;
     warp_hidden(H, [&](auto h) {
         constexpr int HH = decltype(h)::value;
         if constexpr (HH == 128)          // the one size instantiated with the tables in global memory too
-            rc = tabs ? launch_persist<HH, true>(ar, apc_max, gust, s) : launch_persist<HH, false>(ar, apc_max, gust, s);
+            rc = tabs ? launch_persist<HH, true>(ar, apc_max, gust, stagger, s) : launch_persist<HH, false>(ar, apc_max, gust, stagger, s);
         else
-            rc = launch_persist<HH, true>(ar, apc_max, gust, s);
+            rc = launch_persist<HH, true>(ar, apc_max, gust, stagger, s);
     });
     return rc;
 }

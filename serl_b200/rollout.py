@@ -82,11 +82,13 @@ def variant_sorted_order(env_mode):
 
 def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon=HORIZON, trace=False, out=None, action_noise=None,
                        actions=False, t_max=None, smooth_width=None, env_order=None, replay_env=None, status=True, sm_limit=0,
-                       fitness=True, widths=None, sensor_noise=None, gust=False):
+                       fitness=True, widths=None, sensor_noise=None, gust=False, stagger=False):
     """weights [pop,P] fp32 cuda; ref_levels/ref_starts [n_envs,2,6] f64 cuda; env_mode [n_envs] int32 cuda.
     env_order: optional int32 [n_envs] permutation (see variant_sorted_order); replay_env: record the transitions of that env
     of every actor into result.replay [pop, horizon, REPLAY_COLS]; status: carry the device status word (result.check());
     sm_limit: SMs this launch may occupy (0 = all); fitness=False skips the per-actor mean kernel.
+    stagger=True: K1's two genome slots of a CTA run half a step apart instead of taking their steps together (same results,
+    slower on an H100; to time the two schedules against each other).
     widths=[w0, w1, ..., w_{n-1}] (2 to 9 widths): width-list actors on the tensor-core kernel K1-TC (csrc/rollout_tc.cu); `shape`
     then only supplies the activation.  widths=None flies the uniform actor `shape` on K1, or on K1-TC with [h] * (L + 1) when its
     genome does not fit K1's kernels (tc_widths)."""
@@ -138,7 +140,7 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     if sensor_noise is not None:      # envs/noise/citation.py:72-82: standard-normal draws [pop, n_envs, horizon + 1, 7]
         assert sensor_noise.shape == (pop, n_envs, horizon + 1, 7) and sensor_noise.dtype == torch.float32 and sensor_noise.is_contiguous()
         d.d_sensor_noise = p(sensor_noise)
-    d.flags = _native.ROLLOUT_GUST if gust else 0       # some env flies the gust build (mode_code(...) & MODE_GUST)
+    d.flags = (_native.ROLLOUT_GUST if gust else 0) | (_native.ROLLOUT_STAGGER if stagger else 0)   # gust: mode_code(...) & MODE_GUST
     if widths:
         warr = np.asarray(widths, dtype=np.int32)       # host array, alive until the call returns
         d.widths, d.n_widths = warr.ctypes.data, len(widths)
