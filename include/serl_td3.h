@@ -16,10 +16,16 @@ extern "C" {
 
 #define SERL_TD3_CRITIC_HIDDEN 64      /* the 64-64 two-head critic of core/td3.py (Critic) */
 #define SERL_TD3_MAX_BATCH 128
+#define SERL_TD3_MAX_HIDDEN 320        /* the widest actor; above 128 the hidden blocks run as tiled phases */
+#define SERL_TD3_MAX_WIDE_LAYERS 8     /* num_layers limit of the actors wider than 128 */
 #define SERL_TD3_CHAMPION_TARGET 1     /* flags: use_champion_target — the actor target is not soft-updated */
 #define SERL_TD3_STATUS_INDEX 4        /* d_status bit: a d_indices entry was outside [0, n_valid) (row 0 was used) */
 
-/* Learner state: ONE flat fp32 buffer of serl_td3_state_floats(shape) floats,
+/* Supported actors (serl_actor_shape): state_dim 7, action_dim 3, activation 0..2, and either hidden 32, 64, 72, 96 or 128
+ * with any num_layers >= 1, or 129 <= hidden <= SERL_TD3_MAX_HIDDEN with 1 <= num_layers <= SERL_TD3_MAX_WIDE_LAYERS.
+ * Any other shape fails with SERL_ERR_ARG before any CUDA call.
+ *
+ * Learner state: ONE flat fp32 buffer of serl_td3_state_floats(shape) floats,
  *   actor θ | actor target | actor Adam m | actor Adam v | critic θ | critic target | critic Adam m | critic Adam v,
  * each block in nn.Module.parameters() order: the actor's genome layout (serl_actor_num_params floats), and for the critic
  * q1 then q2, each Linear(10,64) LayerNorm(64) Linear(64,64) LayerNorm(64) Linear(64,1) = W, b, gamma, beta, W, b, gamma,

@@ -26,6 +26,8 @@ STATUS_GUST_FLAG = 2
 # include/serl_td3.h (K7, the fused TD3 learner)
 TD3_CRITIC_HIDDEN = 64
 TD3_MAX_BATCH = 128
+TD3_MAX_HIDDEN = 320
+TD3_MAX_WIDE_LAYERS = 8
 TD3_CHAMPION_TARGET = 1
 TD3_STATUS_INDEX = 4
 

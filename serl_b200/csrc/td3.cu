@@ -11,7 +11,8 @@
 // weight gradients over the batch in row order, the gradient norm as fixed 64-element partials summed in order — and the
 // random draws are keyed by (seed, global iteration, row).  The result is therefore the same bits for every cluster size
 // and however the steps are split across launches.  Plain fp32 on CUDA cores: at batch <= 128 the work per step is
-// 10-30 MFLOP, and the step is bound by the ~50 dependent phases, not by arithmetic.
+// 10-30 MFLOP (up to ~0.4 GFLOP for the widest actors), and the step is bound by the ~50 dependent phases, not by
+// arithmetic.  Actors wider than 128 run their h x h blocks as tiled phases (td3_kernel<CS, true>, fwd_wide / bwd_wide).
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -207,8 +208,8 @@ __device__ void fwd_ln(const Net& n, int k, int nh, int rows)
     }
 }
 
-// LayerNorm backward of block k, one warp per row: dU (at the LN output) -> dZ (at the linear output)
-template <int CS>
+// LayerNorm backward of block k, one warp per row: dU (at the LN output) -> dZ (at the linear output); out <= 32 * NJ
+template <int CS, int NJ = 4>
 __device__ void bwd_ln(const Net& n, int k, int nh, int rows)
 {
     const Blk b = n.blk(k);
@@ -222,21 +223,47 @@ __device__ void bwd_ln(const Net& n, int k, int nh, int rows)
         float s = 0.f;
         for (int o = lane; o < out; o += 32) s += ld(du + o) * ld(g + o) * (ld(z + o) - mean);
         const float kq = warp_sum(s) / (rs * rs) / ((float)(out - 1) * sd);     // d std / d c_o = c_o / ((n-1) std)
-        float gc[4];                                                            // out <= 128
+        float gc[NJ];
         float t = 0.f;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
+        for (int j = 0; j < NJ; ++j) {
             const int o = lane + 32 * j;
             gc[j] = 0.f;
             if (o < out) { gc[j] = ld(du + o) * ld(g + o) / rs - kq * (ld(z + o) - mean); t += gc[j]; }
         }
         const float m = warp_sum(t) / (float)out;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
+        for (int j = 0; j < NJ; ++j) {
             const int o = lane + 32 * j;
             if (o < out) n.dZ(k)[rr * out + o] = gc[j] - m;
         }
     }
+}
+
+// Gradient of block k's bias (v < out), LayerNorm gamma (out <= v < 2 out) or beta (v >= 2 out) for head hd, summed over
+// the rows in row order: the sums of bwd_lin's last 3 out elements, for bwd_wide (bwd_lin keeps its own copy inline, which
+// keeps the narrow kernel's code as it was)
+__device__ __forceinline__ float vec_grad(const Net& n, const Blk& b, int k, int hd, int rows, int v)
+{
+    const int out = b.out;
+    float s = 0.f;
+    if (v < out) {
+        const float* dzh = n.dZ(k) + (size_t)hd * rows * out;
+        for (int r = 0; r < rows; ++r) s += ld(dzh + r * out + v);
+    } else {
+        const int o = v - out;
+        const float* du = n.dU(k) + (size_t)hd * rows * out;
+        if (o < out) {             // gamma: sum of dU * (z - mean) / (std + eps)
+            const float* z = n.Z(k) + (size_t)hd * rows * out;
+            for (int r = 0; r < rows; ++r) {
+                const int rr = hd * rows + r;
+                s = fmaf(ld(du + r * out + o) / (ld(n.sd(k) + rr) + LN_EPS), ld(z + r * out + o) - ld(n.mu(k) + rr), s);
+            }
+        } else {                   // beta
+            for (int r = 0; r < rows; ++r) s += ld(du + r * out + o - out);
+        }
+    }
+    return s;
 }
 
 // Block k backward: its parameter gradients (summed over rows in row order) and, if dx, dU of block k-1 =
@@ -287,6 +314,134 @@ __device__ void bwd_lin(const Net& n, int k, int nh, int rows, const float* X, i
             n.dU(k - 1)[rr * in + i] = s * act_d(n.blk(k - 1).act, ld(n.A(k - 1) + rr * in + i));
         }
     }
+}
+
+// ---- the wide actor (128 < h <= SERL_TD3_MAX_HIDDEN): its h x h blocks 1..L as tiled phases ----------------------------
+// A tile is TM x TN outputs of C[m][n] = sum_k A(m, k) B(n, k) on one CTA: thread (ty, tx) = (tid / 16, tid % 16) holds
+// the outputs m0 + ty + 16 i, n0 + tx + 16 j in registers, and the operands pass through shared memory in K-slabs of KS,
+// the next slab loaded into registers while the current one is multiplied.  Every output is still one thread's fmaf
+// chain from k = 0 upward, the order of fwd_lin / bwd_lin (slab padding adds fmaf(0, 0, acc) = acc), and the tile shapes
+// do not depend on CS: the bits depend on neither the cluster size nor the launch split.  A phase deals its tiles
+// round-robin over the cluster's CTAs.  AK (BK): A (B) is contiguous in k in memory, else in m (n) — the loading order
+// that keeps a warp's global loads coalesced and its shared-memory stores free of bank conflicts.
+constexpr int KS = 32;
+constexpr int FWD_TM = 32, FWD_TN = 64;        // forward: rows x output neurons
+constexpr int WG_TM = 64, WG_TN = 64;          // weight gradient: output x input neurons, summed over the rows
+constexpr int DG_TM = 32, DG_TN = 64;          // input gradient: rows x input neurons, summed over the output neurons
+__host__ __device__ constexpr int tile_floats(int tm, int tn) { return KS * (tm + 1) + KS * (tn + 1); }
+__host__ __device__ constexpr int cmax(int x, int y) { return x > y ? x : y; }
+constexpr size_t WIDE_SMEM = sizeof(float) * cmax(tile_floats(FWD_TM, FWD_TN), cmax(tile_floats(WG_TM, WG_TN), tile_floats(DG_TM, DG_TN)));
+// the tiles' shared memory: static, and allocated only in the kernels that reach this function (an extern __shared__
+// array would pad the static shared memory of every kernel of the translation unit to 16 bytes)
+__device__ __forceinline__ float* tile_smem()
+{
+    __shared__ float buf[WIDE_SMEM / sizeof(float)];
+    return buf;
+}
+
+template <int TM, int TN, bool AK, bool BK, class LA, class LB, class Epi>
+__device__ __forceinline__ void tile(float* sm, int m0, int n0, int M, int N, int K, LA la, LB lb, Epi epi)
+{
+    constexpr int MI = TM / 16, NJ = TN / 16, QA = TM * KS / NT, QB = TN * KS / NT;
+    static_assert(TM % 16 == 0 && TN % 16 == 0 && QA * NT == TM * KS && QB * NT == TN * KS, "tile shape");
+    float* As = sm;                    // [KS][TM + 1]
+    float* Bs = sm + KS * (TM + 1);    // [KS][TN + 1]
+    const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
+    float acc[MI][NJ], ra[QA], rb[QB];
+#pragma unroll
+    for (int i = 0; i < MI; ++i)
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) acc[i][j] = 0.f;
+    const auto fetch = [&](int k0) {
+#pragma unroll
+        for (int q = 0; q < QA; ++q) {
+            const int e = threadIdx.x + q * NT, m = AK ? e / KS : e % TM, k = AK ? e % KS : e / TM;
+            ra[q] = m0 + m < M && k0 + k < K ? la(m0 + m, k0 + k) : 0.f;
+        }
+#pragma unroll
+        for (int q = 0; q < QB; ++q) {
+            const int e = threadIdx.x + q * NT, n = BK ? e / KS : e % TN, k = BK ? e % KS : e / TN;
+            rb[q] = n0 + n < N && k0 + k < K ? lb(n0 + n, k0 + k) : 0.f;
+        }
+    };
+    fetch(0);
+    for (int k0 = 0; k0 < K; k0 += KS) {
+        __syncthreads();               // the previous slab (or tile) has been read
+#pragma unroll
+        for (int q = 0; q < QA; ++q) {
+            const int e = threadIdx.x + q * NT, m = AK ? e / KS : e % TM, k = AK ? e % KS : e / TM;
+            As[k * (TM + 1) + m] = ra[q];
+        }
+#pragma unroll
+        for (int q = 0; q < QB; ++q) {
+            const int e = threadIdx.x + q * NT, n = BK ? e / KS : e % TN, k = BK ? e % KS : e / TN;
+            Bs[k * (TN + 1) + n] = rb[q];
+        }
+        __syncthreads();
+        if (k0 + KS < K) fetch(k0 + KS);
+#pragma unroll
+        for (int k = 0; k < KS; ++k) {
+            float av[MI], bv[NJ];
+#pragma unroll
+            for (int i = 0; i < MI; ++i) av[i] = As[k * (TM + 1) + ty + 16 * i];
+#pragma unroll
+            for (int j = 0; j < NJ; ++j) bv[j] = Bs[k * (TN + 1) + tx + 16 * j];
+#pragma unroll
+            for (int i = 0; i < MI; ++i)
+#pragma unroll
+                for (int j = 0; j < NJ; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
+        }
+    }
+#pragma unroll
+    for (int i = 0; i < MI; ++i)
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+            const int m = m0 + ty + 16 * i, n = n0 + tx + 16 * j;
+            if (m < M && n < N) epi(m, n, acc[i][j]);
+        }
+}
+
+// forward of the wide actor's block k (1..L, h x h, LayerNorm): Z[r][o] = sum_i A_{k-1}[r][i] W[o][i] + b[o]
+template <int CS>
+__device__ void fwd_wide(const Net& n, int k, int rows, float* sm)
+{
+    const Blk b = n.blk(k);
+    const int in = b.in, out = b.out;
+    const float *x = n.A(k - 1), *w = n.P + b.off, *bias = w + out * in;
+    float* z = n.Z(k);
+    const int tn = (out + FWD_TN - 1) / FWD_TN, nt = (rows + FWD_TM - 1) / FWD_TM * tn;
+    for (int t = blockIdx.x; t < nt; t += CS)
+        tile<FWD_TM, FWD_TN, true, true>(sm, t / tn * FWD_TM, t % tn * FWD_TN, rows, out, in,
+            [&](int r, int i) { return ld(x + r * in + i); },
+            [&](int o, int i) { return ld(w + o * in + i); },
+            [&](int r, int o, float acc) { z[r * out + o] = acc + ld(bias + o); });
+}
+
+// backward of the wide actor's block k (1..L): the weight gradient G[o][i] = sum_r dZ[r][o] A_{k-1}[r][i] and the input
+// gradient dU_{k-1}[r][i] = (sum_o dZ[r][o] W[o][i]) * act'(A_{k-1}[r][i]) as tiles, then the bias, gamma and beta
+// gradients one per thread (vec_grad, as bwd_lin)
+template <int CS>
+__device__ void bwd_wide(const Net& n, int k, int rows, float* sm)
+{
+    const Blk b = n.blk(k);
+    const int in = b.in, out = b.out, pact = n.blk(k - 1).act;
+    const float *dz = n.dZ(k), *x = n.A(k - 1), *w = n.P + b.off;
+    float *g = n.G + b.off, *du = n.dU(k - 1);
+    const int wn = (in + WG_TN - 1) / WG_TN, nw = (out + WG_TM - 1) / WG_TM * wn;
+    const int dn = (in + DG_TN - 1) / DG_TN, nd = (rows + DG_TM - 1) / DG_TM * dn;
+    for (int t = blockIdx.x; t < nw + nd; t += CS) {
+        if (t < nw)
+            tile<WG_TM, WG_TN, false, false>(sm, t / wn * WG_TM, t % wn * WG_TN, out, in, rows,
+                [&](int o, int r) { return ld(dz + r * out + o); },
+                [&](int i, int r) { return ld(x + r * in + i); },
+                [&](int o, int i, float s) { g[o * in + i] = s; });
+        else
+            tile<DG_TM, DG_TN, true, false>(sm, (t - nw) / dn * DG_TM, (t - nw) % dn * DG_TN, rows, in, out,
+                [&](int r, int o) { return ld(dz + r * out + o); },
+                [&](int i, int o) { return ld(w + o * in + i); },
+                [&](int r, int i, float s) { du[r * in + i] = s * act_d(pact, ld(x + r * in + i)); });
+    }
+    for (int v = gt<CS>(); v < 3 * out; v += GN(CS)) g[out * in + v] = vec_grad(n, b, k, 0, rows, v);
 }
 
 // sum of squares of CHUNK-element slices of the gradient g[0, count)
@@ -396,11 +551,14 @@ __device__ void draw_batch(const Args& a, int k, long long it, int* pick, int* t
     }
 }
 
-template <int CS>
+// WIDE: the actor's hidden blocks take the tiled phases (fwd_wide / bwd_wide, WIDE_SMEM bytes of shared memory)
+template <int CS, bool WIDE>
 __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_kernel(const Args a)
 {
     __shared__ int pick[SERL_TD3_MAX_BATCH], tdraw[SERL_TD3_MAX_BATCH];
     __shared__ float s_coef;
+    float* const wide_sm = WIDE ? tile_smem() : nullptr;
+    constexpr int NJ = WIDE ? (SERL_TD3_MAX_HIDDEN + 31) / 32 : 4;     // bwd_ln of the actor: h <= 32 * NJ
     const int B = a.B, Pa = a.Pa;
     const Lay l = layout(B, a.h, a.L, Pa);
     float* ws = a.ws;
@@ -426,7 +584,8 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_kernel(c
         csync<CS>();
         // ---- target: a' = clamp(actor_target(s') + noise, +-1); y = r + gamma * min(q1', q2') * (1 - done)
         for (int kb = 0; kb <= la; ++kb) {
-            fwd_lin<CS>(actor_t, kb, 1, B, Xt, CI, [&](int, int r, int o, float v) {
+            if (WIDE && kb >= 1 && kb <= a.L) fwd_wide<CS>(actor_t, kb, B, wide_sm);
+            else fwd_lin<CS>(actor_t, kb, 1, B, Xt, CI, [&](int, int r, int o, float v) {
                 float* p = Xt + r * CI + SD + o;
                 *p = fminf(fmaxf(ld(p) + tanhf(v), -1.f), 1.f);
             });
@@ -482,7 +641,8 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_kernel(c
         // ---- actor: -mean(Q1(s, pi(s))) + CAPS terms through the updated critic
         if (actor_step) {
             for (int kb = 0; kb <= la; ++kb) {
-                fwd_lin<CS>(actor, kb, 1, ra, Xa, SD, [&](int, int r, int o, float v) {
+                if (WIDE && kb >= 1 && kb <= a.L) fwd_wide<CS>(actor, kb, ra, wide_sm);
+                else fwd_lin<CS>(actor, kb, 1, ra, Xa, SD, [&](int, int r, int o, float v) {
                     const float y = tanhf(v);
                     actor.A(la)[r * AD + o] = y;
                     if (r < B) Xp[r * CI + SD + o] = y;
@@ -533,8 +693,10 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_kernel(c
             csync<CS>();
             bwd_lin<CS>(actor, la, 1, ra, Xa, SD, true, true); csync<CS>();
             for (int kb = a.L; kb >= 1; --kb) {
-                bwd_ln<CS>(actor, kb, 1, ra); csync<CS>();
-                bwd_lin<CS>(actor, kb, 1, ra, Xa, SD, true, true); csync<CS>();
+                bwd_ln<CS, NJ>(actor, kb, 1, ra); csync<CS>();
+                if (WIDE) bwd_wide<CS>(actor, kb, ra, wide_sm);
+                else bwd_lin<CS>(actor, kb, 1, ra, Xa, SD, true, true);
+                csync<CS>();
             }
             bwd_lin<CS>(actor, 0, 1, ra, Xa, SD, true, false);
             if (gt<CS>() == 0) {
@@ -569,11 +731,21 @@ int64_t actor_floats(const serl_actor_shape& s)
     return (int64_t)s.state_dim * h + h + (int64_t)s.num_layers * (h * h + 3 * h) + h * s.action_dim + s.action_dim;
 }
 
+// the narrow widths at any depth, and the wide ones (the tiled instantiation) up to SERL_TD3_MAX_WIDE_LAYERS blocks
 bool shape_ok(const serl_actor_shape* s)
 {
     const int h = s ? s->hidden : 0;
-    return s && s->state_dim == SD && s->action_dim == AD && (h == 32 || h == 64 || h == 72 || h == 96 || h == 128) &&
+    const bool narrow = h == 32 || h == 64 || h == 72 || h == 96 || h == 128;
+    const bool wide = h > 128 && h <= SERL_TD3_MAX_HIDDEN && s->num_layers <= SERL_TD3_MAX_WIDE_LAYERS;
+    return s && s->state_dim == SD && s->action_dim == AD && (narrow || wide) &&
            s->num_layers >= 1 && s->activation >= SERL_ACT_TANH && s->activation <= SERL_ACT_LEAKY_RELU;
+}
+
+template <int CS>
+int launch(const Args& a, cudaStream_t s)
+{
+    if (a.h > 128) return serl_launch("td3_kernel (wide)", td3_kernel<CS, true>, dim3(CS), dim3(NT), 0, s, a);
+    return serl_launch("td3_kernel", td3_kernel<CS, false>, dim3(CS), dim3(NT), 0, s, a);
 }
 
 }  // namespace
@@ -588,8 +760,8 @@ extern "C" int serl_td3_train(const serl_td3_desc* d, void* stream)
 {
     if (!d) return serl_fail(SERL_ERR_ARG, "serl_td3_train: null descriptor");
     if (!shape_ok(&d->shape))
-        return serl_fail(SERL_ERR_ARG, "serl_td3_train: unsupported actor shape (state 7, action 3, hidden 32/64/72/96/128, "
-                                       "num_layers >= 1, activation 0..2)");
+        return serl_fail(SERL_ERR_ARG, "serl_td3_train: unsupported actor shape (state 7, action 3, hidden 32/64/72/96/128 with "
+                                       "num_layers >= 1 or hidden 129..320 with num_layers 1..8, activation 0..2)");
     if (d->batch < 1 || d->batch > SERL_TD3_MAX_BATCH) return serl_fail(SERL_ERR_ARG, "serl_td3_train: batch must be 1..128");
     if (d->n_steps < 0 || d->n_valid < d->batch || d->replay_cols < COLS)
         return serl_fail(SERL_ERR_ARG, "serl_td3_train: bad n_steps / n_valid (>= batch) / replay_cols (>= 19)");
@@ -618,9 +790,9 @@ extern "C" int serl_td3_train(const serl_td3_desc* d, void* stream)
     if (e != cudaSuccess) return serl_fail_cuda(e, "td3 scratch");
     a.ws = (float*)ws;
     switch (cs) {
-    case 1: return serl_launch("td3_kernel<1>", td3_kernel<1>, dim3(1), dim3(NT), 0, s, a);
-    case 2: return serl_launch("td3_kernel<2>", td3_kernel<2>, dim3(2), dim3(NT), 0, s, a);
-    case 4: return serl_launch("td3_kernel<4>", td3_kernel<4>, dim3(4), dim3(NT), 0, s, a);
-    default: return serl_launch("td3_kernel<8>", td3_kernel<8>, dim3(8), dim3(NT), 0, s, a);
+    case 1: return launch<1>(a, s);
+    case 2: return launch<2>(a, s);
+    case 4: return launch<4>(a, s);
+    default: return launch<8>(a, s);
     }
 }
