@@ -222,7 +222,7 @@ const char* serl_last_error(void);
 }
 #endif
 
-/* K7, the fused TD3 learner (serl_td3_train, serl_td3_state_floats) */
+/* K7, the fused TD3 learner (serl_td3_train, serl_td3_state_floats; serl_td3_train_group through serl_td3_group.h) */
 #include "serl_td3.h"
 /* the kernel of a uniform actor: K1, or K1-TC with the widths [h] * (L + 1) (serl_actor_tc_widths) */
 #include "serl_route.h"

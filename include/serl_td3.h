@@ -75,4 +75,7 @@ int serl_td3_train(const serl_td3_desc* desc, void* stream);
 #ifdef __cplusplus
 }
 #endif
+
+/* several learners in one launch (serl_td3_train_group) */
+#include "serl_td3_group.h"
 #endif

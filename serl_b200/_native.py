@@ -2,7 +2,8 @@
 fallback: importing succeeds without a GPU (so host logic is testable), but the library must exist and every compute call
 fails loudly when CUDA is unavailable.  tests/test_capi.py holds the signatures and constants below to the header,
 tests/test_td3_oracle.py those of include/serl_td3.h (TD3_SIGNATURES, TD3Desc, TD3_*), tests/test_deep_actor.py those of
-include/serl_route.h (ROUTE_SIGNATURES)."""
+include/serl_route.h (ROUTE_SIGNATURES), tests/test_td3_group.py those of include/serl_td3_group.h (TD3_GROUP_SIGNATURES,
+TD3_MAX_GROUP)."""
 import ctypes
 import os
 
@@ -30,6 +31,8 @@ TD3_MAX_HIDDEN = 320
 TD3_MAX_WIDE_LAYERS = 8
 TD3_CHAMPION_TARGET = 1
 TD3_STATUS_INDEX = 4
+# include/serl_td3_group.h (K7 for a group of learners in one launch)
+TD3_MAX_GROUP = 64
 
 
 class ActorShape(ctypes.Structure):
@@ -97,6 +100,10 @@ TD3_SIGNATURES = {
     'serl_td3_state_floats': (_i64, [_shape]),
     'serl_td3_train': (_int, [ctypes.POINTER(TD3Desc), _vp]),
 }
+# include/serl_td3_group.h: n descriptors trained in one launch
+TD3_GROUP_SIGNATURES = {
+    'serl_td3_train_group': (_int, [ctypes.POINTER(TD3Desc), _i32, _vp]),
+}
 # include/serl_route.h: the kernel of a uniform actor (host only, no stream)
 ROUTE_SIGNATURES = {
     'serl_actor_tc_widths': (_i32, [_shape, _vp, _i32]),
@@ -115,7 +122,7 @@ def lib():
             raise NativeError('serl_b200: %s is missing — build it with `python -m serl_b200.build` '
                               '(there is no CPU fallback)' % LIB_PATH)
         L = ctypes.CDLL(LIB_PATH)
-        for name, (restype, argtypes) in {**SIGNATURES, **TD3_SIGNATURES, **ROUTE_SIGNATURES}.items():
+        for name, (restype, argtypes) in {**SIGNATURES, **TD3_SIGNATURES, **TD3_GROUP_SIGNATURES, **ROUTE_SIGNATURES}.items():
             f = getattr(L, name)
             f.restype, f.argtypes = restype, argtypes
         _lib = L

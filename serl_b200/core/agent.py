@@ -22,6 +22,7 @@ ranking) instead of an independent draw per episode; every trajectory starts fro
 its batches with a device generator instead of stdlib `random` (so the SSNE planner's stream does not depend on buffer sizes).
 """
 import os
+import time
 from typing import Dict
 
 import numpy as np
@@ -37,6 +38,12 @@ from ..population import PopulationList
 class _Flight:
     """an asynchronous launch of n episodes of ONE actor (result tensors stay on the device until collected)."""
     __slots__ = ('r', 'levels', 'starts', 'n', 'noise_state', 'stream', 'event', 'keep')
+
+
+class _Generation:
+    """what train_head hands train_tail: the population's statistics and the validation flights in the air"""
+    __slots__ = ('best_train_fitness', 'worst_train_fitness', 'population_avg', 'sm', 'sm_sd', 'elite_index', 'ep_len_avg',
+                 'ep_len_sd', 'pop_fitness', 'f_rlval', 'f_champ')
 
 
 class _Front:
@@ -87,6 +94,8 @@ class Agent:
         self._spec_streams = [torch.cuda.Stream(self.device, priority=-1) for _ in range(self.speculative_validations)]
         self.spec_hits = self.spec_tries = 0
         self.timing = {}
+        self._t_prev = 0.0
+        self._gen = None
 
     # ------------------------------------------------------------------------------------------------ episodes
     def _genome_of(self, agent):
@@ -220,12 +229,19 @@ class Agent:
         for target_param, param in zip(rl_net.parameters(), evo_net.parameters()):
             target_param.data.copy_(param.data)
 
+    def _rl_prologue(self) -> bool:
+        """train_rl's preamble: False while the buffer holds at most learn_start transitions; else the actor is put in
+        training mode and, with use_champion_target, the champion's weights become the actor target"""
+        if len(self.replay_buffer) <= self.args.learn_start:
+            return False
+        self.rl_agent.actor.train()
+        if self.args.use_champion_target and self.champion_actor is not None:
+            self.evo_to_rl(self.rl_agent.actor_target, self.champion_actor)
+        return True
+
     def train_rl(self, rl_transitions: int) -> Dict[str, float]:
         pgs_obj, TD_loss = [], []
-        if len(self.replay_buffer) > self.args.learn_start:
-            self.rl_agent.actor.train()
-            if self.args.use_champion_target and self.champion_actor is not None:
-                self.evo_to_rl(self.rl_agent.actor_target, self.champion_actor)
+        if self._rl_prologue():
             if getattr(self.args, 'fused_td3', False):
                 return self._train_rl_fused(int(rl_transitions * self.args.frac_frames_train))
             for _ in range(int(rl_transitions * self.args.frac_frames_train)):
@@ -238,15 +254,26 @@ class Agent:
                     TD_loss.append(TD)
         return {'PG_obj': np.mean(pgs_obj) if pgs_obj else float('nan'), 'TD_loss': np.median(TD_loss) if TD_loss else float('nan')}
 
-    def _train_rl_fused(self, n):
-        """train_rl's loop as K7 launches; the statistics come from ONE device->host copy of the losses"""
-        if n <= 0:
+    def plan_rl_fused(self, rl_transitions: int):
+        """the fused train_rl up to its K7 launch: None when the buffer is below learn_start, else the number of gradient
+        steps n (0 or more) on global iterations rl_iteration + 1.. (the champion target is already in place)"""
+        return int(rl_transitions * self.args.frac_frames_train) if self._rl_prologue() else None
+
+    def finish_rl_fused(self, n, losses) -> Dict[str, float]:
+        """the fused train_rl after its K7 launch: the statistics of the host losses [n, 2] and the iteration count"""
+        if n is None or n <= 0:
             return {'PG_obj': float('nan'), 'TD_loss': float('nan')}
         first = self.rl_iteration + 1
-        losses = self.rl_agent.train_steps(self.replay_buffer, n, first, self.args.use_champion_target).cpu().numpy()
         self.rl_iteration += n
         pg = losses[(np.arange(first, first + n) % self.args.policy_update_freq) == 0, 1]
         return {'PG_obj': np.mean(-pg) if pg.size else float('nan'), 'TD_loss': np.median(losses[:, 0])}
+
+    def _train_rl_fused(self, n):
+        """train_rl's loop as K7 launches; the statistics come from ONE device->host copy of the losses"""
+        if n <= 0:
+            return self.finish_rl_fused(n, None)
+        losses = self.rl_agent.train_steps(self.replay_buffer, n, self.rl_iteration + 1, self.args.use_champion_target).cpu().numpy()
+        return self.finish_rl_fused(n, losses)
 
     @staticmethod
     def _validation_stats(eps):
@@ -366,47 +393,58 @@ class Agent:
         return fr
 
     def train(self):
+        """one generation (agent.py:211-315): its head (population, epoch, exploration episode), the RL half, its tail"""
+        self.train_head()
+        return self.train_tail(self.train_rl(self.gen_frames))
+
+    def _lap(self, name):
+        now = time.perf_counter()
+        self.timing[name] = self.timing.get(name, 0.0) + 1e3 * (now - self._t_prev)
+        self._t_prev = now
+
+    def train_head(self):
+        """a generation up to its RL half: the front's rollouts, the population's statistics and SSNE epoch, the champion's
+        validation launch and the collected exploration episode.  The RL half (train_rl(self.gen_frames)) and train_tail
+        follow; train() runs the three in order."""
         self.iterations += 1
         self.gen_frames = 0
-        best_train_fitness = worst_train_fitness = population_avg = test_score = sm = 1.
-        test_sd = sm_sd = elite_index = pop_novelty = -1.
-        ep_len_avg = ep_len_sd = 0.
-        pop_fitness = None
+        g = self._gen = _Generation()
+        g.best_train_fitness = g.worst_train_fitness = g.population_avg = 1.
+        g.sm = 1.
+        g.sm_sd = g.elite_index = -1.
+        g.ep_len_avg = g.ep_len_sd = 0.
+        g.pop_fitness = None
         args = self.args
-        import time as _time
-        tm = self.timing = {}
-        t_prev = [_time.perf_counter()]
-
-        def lap(name):
-            now = _time.perf_counter()
-            tm[name] = tm.get(name, 0.0) + 1e3 * (now - t_prev[0])
-            t_prev[0] = now
+        self.timing = {}
+        self._t_prev = time.perf_counter()
+        lap, tm = self._lap, self.timing
         fr, self._prefetched = self._prefetched, None
         if fr is not None and fr.signature != self._signature():
             fr = None                  # the population / RL actor / environment changed since it was launched: fly again
         tm['front_prefetched'] = float(fr is not None)
         if fr is None:
             fr = self._launch_front()
-        f_explore, f_rlval, spec, val_draws = fr.f_explore, fr.f_rlval, fr.spec, fr.val_draws
+        f_explore, g.f_rlval, spec, val_draws = fr.f_explore, fr.f_rlval, fr.spec, fr.val_draws
         lap('launch_front')
-        f_champ = None
+        g.f_champ = None
         if len(self.pop):
             pop_fitness, dev_fitness, rec = self._finish_population(fr.pop)
+            g.pop_fitness = pop_fitness
             lap('evaluate_population')
             n_envs = int(getattr(args, 'num_envs', args.num_evals))
             n_ep = len(self.pop) * n_envs
             dt = self.env.dt
             mean_steps = rec[:, 1].sum() / n_ep
-            ep_len_avg = mean_steps * dt
-            ep_len_sd = float(np.sqrt(max(rec[:, 2].sum() / n_ep - mean_steps ** 2, 0.0))) * dt
+            g.ep_len_avg = mean_steps * dt
+            g.ep_len_sd = float(np.sqrt(max(rec[:, 2].sum() / n_ep - mean_steps ** 2, 0.0))) * dt
             if rec[:, 6].any():                  # K6: per-episode action smoothness on the device (agent.py:242-243)
-                sm = rec[:, 4].sum() / n_ep
-                sm_sd = float(np.sqrt(max(rec[:, 5].sum() / n_ep - sm ** 2, 0.0)))
+                g.sm = rec[:, 4].sum() / n_ep
+                g.sm_sd = float(np.sqrt(max(rec[:, 5].sum() / n_ep - g.sm ** 2, 0.0)))
             else:
-                sm, sm_sd = float('nan'), float('nan')
-            best_train_fitness = np.max(pop_fitness)
-            worst_train_fitness = np.min(pop_fitness)
-            population_avg = np.average(pop_fitness)
+                g.sm, g.sm_sd = float('nan'), float('nan')
+            g.best_train_fitness = np.max(pop_fitness)
+            g.worst_train_fitness = np.min(pop_fitness)
+            g.population_avg = np.average(pop_fitness)
             self.champion = self.pop[int(np.argmax(pop_fitness))]
             self.champion_actor = self.champion.actor
             # validate_agent(champion) (:255-258) on the side stream, from a COPY of its genome: the epoch below may mutate
@@ -415,18 +453,27 @@ class Agent:
             if spec:
                 self.spec_tries += 1
                 self.spec_hits += ci in spec
-            f_champ = spec.get(ci)
-            if f_champ is None:
-                f_champ = self._fly(self.champion, self.validation_tests, trace=bool(args.should_log), stream=self._champ, copy_genome=True,
-                                    draws=val_draws)
+            g.f_champ = spec.get(ci)
+            if g.f_champ is None:
+                g.f_champ = self._fly(self.champion, self.validation_tests, trace=bool(args.should_log), stream=self._champ,
+                                      copy_genome=True, draws=val_draws)
             lap('stats')
-            elite_index = self.evolver.epoch(self.pop, dev_fitness)
+            g.elite_index = self.evolver.epoch(self.pop, dev_fitness)
             lap('epoch')
         # RL half (agent.py:267-281)
         self._collect(self.rl_agent, f_explore, store_transition=True)
         lap('collect_exploration')
-        rl_train_scores = self.train_rl(self.gen_frames)
+
+    def train_tail(self, rl_train_scores):
+        """the rest of a generation after its RL half (train_rl's statistics): the RL validation, the actor injection, the
+        next generation's front, the validation scores; returns train()'s statistics"""
+        g, self._gen = self._gen, None
+        args = self.args
+        lap = self._lap
         lap('train_rl')
+        test_score, test_sd, pop_novelty = 1., -1., -1.
+        f_rlval, f_champ, pop_fitness, elite_index = g.f_rlval, g.f_champ, g.pop_fitness, g.elite_index
+        ep_len_avg, ep_len_sd = g.ep_len_avg, g.ep_len_sd
         if f_rlval is None:
             f_rlval = self._fly(self.rl_agent, self.validation_tests, trace=bool(args.should_log), stream=self._side2)
         # actor injection (agent.py:283-294)
@@ -456,9 +503,9 @@ class Agent:
                 self.champion_history = last_episode.get_history()
         lap('champion_validation')
         return {
-            'best_train_fitness': best_train_fitness, 'test_score': test_score, 'test_sd': test_sd,
-            'pop_avg': population_avg, 'pop_min': worst_train_fitness, 'elite_index': elite_index,
-            'avg_smoothness': sm, 'smoothness_sd': sm_sd, 'rl_reward': rl_reward, 'rl_smoothness': rl_sm,
+            'best_train_fitness': g.best_train_fitness, 'test_score': test_score, 'test_sd': test_sd,
+            'pop_avg': g.population_avg, 'pop_min': g.worst_train_fitness, 'elite_index': elite_index,
+            'avg_smoothness': g.sm, 'smoothness_sd': g.sm_sd, 'rl_reward': rl_reward, 'rl_smoothness': rl_sm,
             'rl_smoothness_std': rl_sm_sd, 'rl_std': rl_std, 'avg_ep_len': ep_len_avg, 'ep_len_sd': ep_len_sd,
             'PG_obj': rl_train_scores['PG_obj'], 'TD_loss': rl_train_scores['TD_loss'], 'pop_novelty': pop_novelty,
         }

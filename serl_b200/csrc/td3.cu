@@ -13,9 +13,11 @@
 // and however the steps are split across launches.  Plain fp32 on CUDA cores: at batch <= 128 the work per step is
 // 10-30 MFLOP (up to ~0.4 GFLOP for the widest actors), and the step is bound by the ~50 dependent phases, not by
 // arithmetic.  Actors wider than 128 run their h x h blocks as tiled phases (td3_kernel<CS, true>, fwd_wide / bwd_wide).
+// td3_group_kernel runs several independent learners in one launch, one cluster each (serl_td3_train_group).
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
+#include <stdio.h>
 
 #include "../../include/serl_td3.h"
 #include "common.cuh"
@@ -155,19 +157,28 @@ struct Net {
     __device__ float* sd(int k) const { return mu(k) + cap; }
 };
 
-template <int CS> __device__ __forceinline__ int gt() { return blockIdx.x * NT + threadIdx.x; }
-template <int CS> __device__ __forceinline__ int gw() { return (blockIdx.x * NT + threadIdx.x) >> 5; }
+// the CTA's rank in its cluster: blockIdx.x in a solo launch (the grid is one cluster), %cluster_ctarank in a group
+// launch (G: cluster g of the grid runs learner g)
+template <bool G> __device__ __forceinline__ int crank()
+{
+    if (!G) return blockIdx.x;
+    unsigned r;
+    asm("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return (int)r;
+}
+template <int CS, bool G> __device__ __forceinline__ int gt() { return crank<G>() * NT + threadIdx.x; }
+template <int CS, bool G> __device__ __forceinline__ int gw() { return (crank<G>() * NT + threadIdx.x) >> 5; }
 __host__ __device__ constexpr int GN(int CS) { return CS * NT; }
 
 // Linear part of block k for nh heads x rows rows (row rr = head * rows + r).  Input: X (row stride xs, shared by the
 // heads) for block 0, else the previous block's A.  LayerNorm blocks store Z; other blocks store act(.) in A, except the
 // last block, whose value goes to epi(head, r, o, value).
-template <int CS, class Epi>
+template <int CS, bool G, class Epi>
 __device__ void fwd_lin(const Net& n, int k, int nh, int rows, const float* X, int xs, Epi epi)
 {
     const Blk b = n.blk(k);
     const int per = rows * b.out, total = nh * per;
-    for (int e = gt<CS>(); e < total; e += GN(CS)) {
+    for (int e = gt<CS, G>(); e < total; e += GN(CS)) {
         const int hd = e / per, rem = e - hd * per, o = rem / rows, r = rem - o * rows;      // a warp shares a weight row
         const float* w = n.P + hd * n.hs + b.off + o * b.in;
         const float* x = k == 0 ? X + r * xs : n.A(k - 1) + (size_t)(hd * rows + r) * b.in;
@@ -180,19 +191,19 @@ __device__ void fwd_lin(const Net& n, int k, int nh, int rows, const float* X, i
         else epi(hd, r, o, acc);
     }
 }
-template <int CS>
+template <int CS, bool G>
 __device__ void fwd_lin(const Net& n, int k, int nh, int rows, const float* X, int xs)
 {
-    fwd_lin<CS>(n, k, nh, rows, X, xs, [](int, int, int, float) {});
+    fwd_lin<CS, G>(n, k, nh, rows, X, xs, [](int, int, int, float) {});
 }
 
 // LayerNorm + activation of block k, one warp per row: y = gamma * (z - mean) / (std + eps) + beta, Bessel-corrected std
-template <int CS>
+template <int CS, bool G>
 __device__ void fwd_ln(const Net& n, int k, int nh, int rows)
 {
     const Blk b = n.blk(k);
     const int out = b.out, lane = threadIdx.x & 31;
-    for (int rr = gw<CS>(); rr < nh * rows; rr += GN(CS) / 32) {
+    for (int rr = gw<CS, G>(); rr < nh * rows; rr += GN(CS) / 32) {
         const int hd = rr / rows;
         const float* z = n.Z(k) + rr * out;
         const float* g = n.P + hd * n.hs + b.off + out * b.in + out;
@@ -209,12 +220,12 @@ __device__ void fwd_ln(const Net& n, int k, int nh, int rows)
 }
 
 // LayerNorm backward of block k, one warp per row: dU (at the LN output) -> dZ (at the linear output); out <= 32 * NJ
-template <int CS, int NJ = 4>
+template <int CS, bool G, int NJ = 4>
 __device__ void bwd_ln(const Net& n, int k, int nh, int rows)
 {
     const Blk b = n.blk(k);
     const int out = b.out, lane = threadIdx.x & 31;
-    for (int rr = gw<CS>(); rr < nh * rows; rr += GN(CS) / 32) {
+    for (int rr = gw<CS, G>(); rr < nh * rows; rr += GN(CS) / 32) {
         const int hd = rr / rows;
         const float* z = n.Z(k) + rr * out;
         const float* du = n.dU(k) + rr * out;
@@ -268,7 +279,7 @@ __device__ __forceinline__ float vec_grad(const Net& n, const Blk& b, int k, int
 
 // Block k backward: its parameter gradients (summed over rows in row order) and, if dx, dU of block k-1 =
 // (dZ_k W_k) * act'(A_{k-1}); X / xs is block 0's input.  params = false: only dU of block k-1 (input gradients).
-template <int CS>
+template <int CS, bool G>
 __device__ void bwd_lin(const Net& n, int k, int nh, int rows, const float* X, int xs, bool params, bool dx)
 {
     const Blk b = n.blk(k);
@@ -276,7 +287,7 @@ __device__ void bwd_lin(const Net& n, int k, int nh, int rows, const float* X, i
     const int np = params ? out * in + out + (b.ln ? 2 * out : 0) : 0;
     const int tp = nh * np, total = tp + (dx ? nh * rows * in : 0);
     const float* dz = n.dZ(k);
-    for (int e = gt<CS>(); e < total; e += GN(CS)) {
+    for (int e = gt<CS, G>(); e < total; e += GN(CS)) {
         if (e < tp) {
             const int hd = e / np, j = e - hd * np;
             const float* dzh = dz + (size_t)hd * rows * out;
@@ -402,7 +413,7 @@ __device__ __forceinline__ void tile(float* sm, int m0, int n0, int M, int N, in
 }
 
 // forward of the wide actor's block k (1..L, h x h, LayerNorm): Z[r][o] = sum_i A_{k-1}[r][i] W[o][i] + b[o]
-template <int CS>
+template <int CS, bool G>
 __device__ void fwd_wide(const Net& n, int k, int rows, float* sm)
 {
     const Blk b = n.blk(k);
@@ -410,7 +421,7 @@ __device__ void fwd_wide(const Net& n, int k, int rows, float* sm)
     const float *x = n.A(k - 1), *w = n.P + b.off, *bias = w + out * in;
     float* z = n.Z(k);
     const int tn = (out + FWD_TN - 1) / FWD_TN, nt = (rows + FWD_TM - 1) / FWD_TM * tn;
-    for (int t = blockIdx.x; t < nt; t += CS)
+    for (int t = crank<G>(); t < nt; t += CS)
         tile<FWD_TM, FWD_TN, true, true>(sm, t / tn * FWD_TM, t % tn * FWD_TN, rows, out, in,
             [&](int r, int i) { return ld(x + r * in + i); },
             [&](int o, int i) { return ld(w + o * in + i); },
@@ -420,7 +431,7 @@ __device__ void fwd_wide(const Net& n, int k, int rows, float* sm)
 // backward of the wide actor's block k (1..L): the weight gradient G[o][i] = sum_r dZ[r][o] A_{k-1}[r][i] and the input
 // gradient dU_{k-1}[r][i] = (sum_o dZ[r][o] W[o][i]) * act'(A_{k-1}[r][i]) as tiles, then the bias, gamma and beta
 // gradients one per thread (vec_grad, as bwd_lin)
-template <int CS>
+template <int CS, bool G>
 __device__ void bwd_wide(const Net& n, int k, int rows, float* sm)
 {
     const Blk b = n.blk(k);
@@ -429,7 +440,7 @@ __device__ void bwd_wide(const Net& n, int k, int rows, float* sm)
     float *g = n.G + b.off, *du = n.dU(k - 1);
     const int wn = (in + WG_TN - 1) / WG_TN, nw = (out + WG_TM - 1) / WG_TM * wn;
     const int dn = (in + DG_TN - 1) / DG_TN, nd = (rows + DG_TM - 1) / DG_TM * dn;
-    for (int t = blockIdx.x; t < nw + nd; t += CS) {
+    for (int t = crank<G>(); t < nw + nd; t += CS) {
         if (t < nw)
             tile<WG_TM, WG_TN, false, false>(sm, t / wn * WG_TM, t % wn * WG_TN, out, in, rows,
                 [&](int o, int r) { return ld(dz + r * out + o); },
@@ -441,15 +452,15 @@ __device__ void bwd_wide(const Net& n, int k, int rows, float* sm)
                 [&](int i, int o) { return ld(w + o * in + i); },
                 [&](int r, int i, float s) { du[r * in + i] = s * act_d(pact, ld(x + r * in + i)); });
     }
-    for (int v = gt<CS>(); v < 3 * out; v += GN(CS)) g[out * in + v] = vec_grad(n, b, k, 0, rows, v);
+    for (int v = gt<CS, G>(); v < 3 * out; v += GN(CS)) g[out * in + v] = vec_grad(n, b, k, 0, rows, v);
 }
 
 // sum of squares of CHUNK-element slices of the gradient g[0, count)
-template <int CS>
+template <int CS, bool G>
 __device__ void norm_partials(const float* g, int count, float* part)
 {
     const int nc = (count + CHUNK - 1) / CHUNK;
-    for (int c = gt<CS>(); c < nc; c += GN(CS)) {
+    for (int c = gt<CS, G>(); c < nc; c += GN(CS)) {
         float s = 0.f;
         const int end = min(count, (c + 1) * CHUNK);
         for (int i = c * CHUNK; i < end; ++i) { const float v = ld(g + i); s = fmaf(v, v, s); }
@@ -458,8 +469,11 @@ __device__ void norm_partials(const float* g, int count, float* part)
 }
 
 // clip_grad_norm_ (coef = min(1, max / (|g| + 1e-6))) + the torch Adam step (foreach formula, bias corrections)
-// + optionally the Polyak update of the target: tgt <- tgt * (1 - tau) + tau * p
-template <int CS>
+// + optionally the Polyak update of the target: tgt <- tgt * (1 - tau) + tau * p.  Which product of these two sums of
+// two products the compiler fuses into an FFMA depends on where the operands live (tau is a kernel parameter in
+// td3_kernel, a register in td3_group_kernel), so the group kernel (G) spells out the fusion td3_kernel's code has, and
+// gives td3_kernel's bits; td3_kernel keeps its source and its code.
+template <int CS, bool G>
 __device__ void adam(float* p, float* m, float* v, float* tgt, const float* g, int count, const float* part, long long t,
                      const Args& a, bool soft, float* s_coef)
 {
@@ -475,14 +489,15 @@ __device__ void adam(float* p, float* m, float* v, float* tgt, const float* g, i
     const float step = (float)(-a.lr / (1.0 - pow(0.9, (double)t)));
     const float bc2 = (float)sqrt(1.0 - pow(0.999, (double)t));
     const float keep = (float)(1.0 - (double)a.tau);
-    for (int i = gt<CS>(); i < count; i += GN(CS)) {
+    for (int i = gt<CS, G>(); i < count; i += GN(CS)) {
         const float gi = ld(g + i) * coef;
         float mi = ld(m + i), vi = ld(v + i);
         mi = mi + 0.1f * (gi - mi);                           // exp_avg.lerp_(grad, 1 - beta1)
-        vi = vi * 0.999f + 0.001f * gi * gi;                  // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1 - beta2)
+        // exp_avg_sq.mul_(beta2).addcmul_(grad, grad, 1 - beta2)
+        vi = G ? fmaf(vi, 0.999f, 0.001f * gi * gi) : vi * 0.999f + 0.001f * gi * gi;
         const float pi = ld(p + i) + step * (mi / (sqrtf(vi) / bc2 + 1e-8f));
         m[i] = mi; v[i] = vi; p[i] = pi;
-        if (soft) tgt[i] = ld(tgt + i) * keep + a.tau * pi;
+        if (soft) tgt[i] = G ? fmaf(ld(tgt + i), keep, a.tau * pi) : ld(tgt + i) * keep + a.tau * pi;
     }
 }
 
@@ -551,9 +566,10 @@ __device__ void draw_batch(const Args& a, int k, long long it, int* pick, int* t
     }
 }
 
-// WIDE: the actor's hidden blocks take the tiled phases (fwd_wide / bwd_wide, WIDE_SMEM bytes of shared memory)
-template <int CS, bool WIDE>
-__global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_kernel(const Args a)
+// One learner's n_steps on one cluster.  WIDE: the actor's hidden blocks take the tiled phases (fwd_wide / bwd_wide,
+// WIDE_SMEM bytes of shared memory).  G: the cluster is one of a group launch's (crank).
+template <int CS, bool WIDE, bool G>
+__device__ __forceinline__ void td3_learner(const Args a)
 {
     __shared__ int pick[SERL_TD3_MAX_BATCH], tdraw[SERL_TD3_MAX_BATCH];
     __shared__ float s_coef;
@@ -580,25 +596,25 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_kernel(c
         const long long it = a.it0 + k;
         const bool actor_step = it % a.freq == 0;
         float td = 0.f, pg = __int_as_float(0x7fc00000);
-        if (blockIdx.x == 0) draw_batch(a, k, it, pick, tdraw, Xt, Xs, Xp, Xa, rw, dn);
+        if (crank<G>() == 0) draw_batch(a, k, it, pick, tdraw, Xt, Xs, Xp, Xa, rw, dn);
         csync<CS>();
         // ---- target: a' = clamp(actor_target(s') + noise, +-1); y = r + gamma * min(q1', q2') * (1 - done)
         for (int kb = 0; kb <= la; ++kb) {
-            if (WIDE && kb >= 1 && kb <= a.L) fwd_wide<CS>(actor_t, kb, B, wide_sm);
-            else fwd_lin<CS>(actor_t, kb, 1, B, Xt, CI, [&](int, int r, int o, float v) {
+            if (WIDE && kb >= 1 && kb <= a.L) fwd_wide<CS, G>(actor_t, kb, B, wide_sm);
+            else fwd_lin<CS, G>(actor_t, kb, 1, B, Xt, CI, [&](int, int r, int o, float v) {
                 float* p = Xt + r * CI + SD + o;
                 *p = fminf(fmaxf(ld(p) + tanhf(v), -1.f), 1.f);
             });
             csync<CS>();
-            if (actor_t.blk(kb).ln) { fwd_ln<CS>(actor_t, kb, 1, B); csync<CS>(); }
+            if (actor_t.blk(kb).ln) { fwd_ln<CS, G>(actor_t, kb, 1, B); csync<CS>(); }
         }
         for (int kb = 0; kb < 2; ++kb) {
-            fwd_lin<CS>(critic_t, kb, 2, B, Xt, CI); csync<CS>();
-            fwd_ln<CS>(critic_t, kb, 2, B); csync<CS>();
+            fwd_lin<CS, G>(critic_t, kb, 2, B, Xt, CI); csync<CS>();
+            fwd_ln<CS, G>(critic_t, kb, 2, B); csync<CS>();
         }
         {
             const Blk b = critic_t.blk(2);
-            for (int r = gt<CS>(); r < B; r += GN(CS)) {
+            for (int r = gt<CS, G>(); r < B; r += GN(CS)) {
                 float q[2];
                 for (int hd = 0; hd < 2; ++hd) {
                     const float* w = critic_t.P + hd * CP + b.off;
@@ -613,20 +629,20 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_kernel(c
         csync<CS>();
         // ---- critic: forward on (s, a), loss mse(q1, y) + mse(q2, y), backward
         for (int kb = 0; kb < 2; ++kb) {
-            fwd_lin<CS>(critic, kb, 2, B, Xs, CI); csync<CS>();
-            fwd_ln<CS>(critic, kb, 2, B); csync<CS>();
+            fwd_lin<CS, G>(critic, kb, 2, B, Xs, CI); csync<CS>();
+            fwd_ln<CS, G>(critic, kb, 2, B); csync<CS>();
         }
-        fwd_lin<CS>(critic, 2, 2, B, Xs, CI, [&](int hd, int r, int, float v) {
+        fwd_lin<CS, G>(critic, 2, 2, B, Xs, CI, [&](int hd, int r, int, float v) {
             critic.A(2)[hd * B + r] = v;
             critic.dU(2)[hd * B + r] = 2.f * inv_b * (v - ld(yt + r));
         });
         csync<CS>();
-        bwd_lin<CS>(critic, 2, 2, B, Xs, CI, true, true); csync<CS>();
-        bwd_ln<CS>(critic, 1, 2, B); csync<CS>();
-        bwd_lin<CS>(critic, 1, 2, B, Xs, CI, true, true); csync<CS>();
-        bwd_ln<CS>(critic, 0, 2, B); csync<CS>();
-        bwd_lin<CS>(critic, 0, 2, B, Xs, CI, true, false);
-        if (gt<CS>() == 0) {
+        bwd_lin<CS, G>(critic, 2, 2, B, Xs, CI, true, true); csync<CS>();
+        bwd_ln<CS, G>(critic, 1, 2, B); csync<CS>();
+        bwd_lin<CS, G>(critic, 1, 2, B, Xs, CI, true, true); csync<CS>();
+        bwd_ln<CS, G>(critic, 0, 2, B); csync<CS>();
+        bwd_lin<CS, G>(critic, 0, 2, B, Xs, CI, true, false);
+        if (gt<CS, G>() == 0) {
             float s1 = 0.f, s2 = 0.f;
             for (int r = 0; r < B; ++r) {
                 const float y = ld(yt + r), d1 = ld(critic.A(2) + r) - y, d2 = ld(critic.A(2) + B + r) - y;
@@ -635,28 +651,28 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_kernel(c
             td = s1 / (float)B + s2 / (float)B;
         }
         csync<CS>();
-        norm_partials<CS>(gc, 2 * CP, part); csync<CS>();
-        adam<CS>(th_c, m_c, v_c, tg_c, gc, 2 * CP, part, a.tc0 + k + 1, a, actor_step, &s_coef);
+        norm_partials<CS, G>(gc, 2 * CP, part); csync<CS>();
+        adam<CS, G>(th_c, m_c, v_c, tg_c, gc, 2 * CP, part, a.tc0 + k + 1, a, actor_step, &s_coef);
         csync<CS>();
         // ---- actor: -mean(Q1(s, pi(s))) + CAPS terms through the updated critic
         if (actor_step) {
             for (int kb = 0; kb <= la; ++kb) {
-                if (WIDE && kb >= 1 && kb <= a.L) fwd_wide<CS>(actor, kb, ra, wide_sm);
-                else fwd_lin<CS>(actor, kb, 1, ra, Xa, SD, [&](int, int r, int o, float v) {
+                if (WIDE && kb >= 1 && kb <= a.L) fwd_wide<CS, G>(actor, kb, ra, wide_sm);
+                else fwd_lin<CS, G>(actor, kb, 1, ra, Xa, SD, [&](int, int r, int o, float v) {
                     const float y = tanhf(v);
                     actor.A(la)[r * AD + o] = y;
                     if (r < B) Xp[r * CI + SD + o] = y;
                 });
                 csync<CS>();
-                if (actor.blk(kb).ln) { fwd_ln<CS>(actor, kb, 1, ra); csync<CS>(); }
+                if (actor.blk(kb).ln) { fwd_ln<CS, G>(actor, kb, 1, ra); csync<CS>(); }
             }
             for (int kb = 0; kb < 2; ++kb) {
-                fwd_lin<CS>(critic, kb, 1, B, Xp, CI); csync<CS>();
-                fwd_ln<CS>(critic, kb, 1, B); csync<CS>();
+                fwd_lin<CS, G>(critic, kb, 1, B, Xp, CI); csync<CS>();
+                fwd_ln<CS, G>(critic, kb, 1, B); csync<CS>();
             }
             {   // Q1 and the gradient of -mean(Q1) at the last hidden layer
                 const float* w = critic.P + critic.blk(2).off;
-                for (int e = gt<CS>(); e < B * CH + B; e += GN(CS)) {
+                for (int e = gt<CS, G>(); e < B * CH + B; e += GN(CS)) {
                     if (e < B * CH) {
                         const int i = e % CH;
                         critic.dU(1)[e] = (-inv_b * ld(w + i)) * act_d(a.act, ld(critic.A(1) + e));
@@ -670,12 +686,12 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_kernel(c
                 }
             }
             csync<CS>();
-            bwd_ln<CS>(critic, 1, 1, B); csync<CS>();
-            bwd_lin<CS>(critic, 1, 1, B, Xp, CI, false, true); csync<CS>();
-            bwd_ln<CS>(critic, 0, 1, B); csync<CS>();
+            bwd_ln<CS, G>(critic, 1, 1, B); csync<CS>();
+            bwd_lin<CS, G>(critic, 1, 1, B, Xp, CI, false, true); csync<CS>();
+            bwd_ln<CS, G>(critic, 0, 1, B); csync<CS>();
             {   // gradient at the actor's output: dQ1/da (critic input columns 7..9) + the CAPS terms, through tanh
                 const float* w = critic.P + critic.blk(0).off;
-                for (int e = gt<CS>(); e < ra * AD; e += GN(CS)) {
+                for (int e = gt<CS, G>(); e < ra * AD; e += GN(CS)) {
                     const int r = e / AD, j = e - r * AD;
                     const float y = ld(actor.A(la) + e), act = ld(Xs + (r % B) * CI + SD + j);
                     float g;
@@ -691,15 +707,15 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_kernel(c
                 }
             }
             csync<CS>();
-            bwd_lin<CS>(actor, la, 1, ra, Xa, SD, true, true); csync<CS>();
+            bwd_lin<CS, G>(actor, la, 1, ra, Xa, SD, true, true); csync<CS>();
             for (int kb = a.L; kb >= 1; --kb) {
-                bwd_ln<CS, NJ>(actor, kb, 1, ra); csync<CS>();
-                if (WIDE) bwd_wide<CS>(actor, kb, ra, wide_sm);
-                else bwd_lin<CS>(actor, kb, 1, ra, Xa, SD, true, true);
+                bwd_ln<CS, G, NJ>(actor, kb, 1, ra); csync<CS>();
+                if (WIDE) bwd_wide<CS, G>(actor, kb, ra, wide_sm);
+                else bwd_lin<CS, G>(actor, kb, 1, ra, Xa, SD, true, true);
                 csync<CS>();
             }
-            bwd_lin<CS>(actor, 0, 1, ra, Xa, SD, true, false);
-            if (gt<CS>() == 0) {
+            bwd_lin<CS, G>(actor, 0, 1, ra, Xa, SD, true, false);
+            if (gt<CS, G>() == 0) {
                 float sq = 0.f, st = 0.f, ss = 0.f;
                 for (int r = 0; r < B; ++r) sq += ld(q1 + r);
                 for (int e = 0; e < B * AD; ++e) {
@@ -713,16 +729,38 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_kernel(c
                 if (caps_s) pg += a.ls * (ss / (float)(B * AD));
             }
             csync<CS>();
-            norm_partials<CS>(ga, Pa, part); csync<CS>();
-            adam<CS>(th_a, m_a, v_a, tg_a, ga, Pa, part, ++ta, a, !a.champion, &s_coef);
+            norm_partials<CS, G>(ga, Pa, part); csync<CS>();
+            adam<CS, G>(th_a, m_a, v_a, tg_a, ga, Pa, part, ++ta, a, !a.champion, &s_coef);
             csync<CS>();
         }
-        if (gt<CS>() == 0) {
+        if (gt<CS, G>() == 0) {
             a.losses[2 * k] = td;
             a.losses[2 * k + 1] = pg;
             if (a.status && (!isfinite(td) || (actor_step && !isfinite(pg)))) atomicOr(a.status, SERL_STATUS_NONFINITE);
         }
     }
+}
+
+template <int CS, bool WIDE>
+__global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_kernel(const Args a)
+{
+    td3_learner<CS, WIDE, false>(a);
+}
+
+// A group launch: n learners of one actor shape, one cluster each.  Their Args travel as the kernel parameter (no
+// host-to-device copy; CUDA 12.1+ allows 32,764 bytes of parameters on sm_90), and cluster g reads entry g from the
+// constant bank (__grid_constant__: the table is never copied to local memory).  td3_learner takes its Args by value,
+// which keeps td3_kernel's code exactly what it was before the group launch existed.  Clusters never wait for each
+// other, so a group larger than the number of resident clusters is correct: later clusters start as earlier ones retire.
+struct Group { Args a[SERL_TD3_MAX_GROUP]; };
+static_assert(sizeof(Group) <= 32764, "SERL_TD3_MAX_GROUP learners' Args must fit the sm_90 kernel-parameter limit");
+
+template <int CS, bool WIDE>
+__global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_group_kernel(const __grid_constant__ Group t)
+{
+    unsigned g;
+    asm("mov.u32 %0, %%clusterid.x;" : "=r"(g));
+    td3_learner<CS, WIDE, true>(t.a[g]);
 }
 
 int64_t actor_floats(const serl_actor_shape& s)
@@ -748,30 +786,33 @@ int launch(const Args& a, cudaStream_t s)
     return serl_launch("td3_kernel", td3_kernel<CS, false>, dim3(CS), dim3(NT), 0, s, a);
 }
 
-}  // namespace
-
-extern "C" int64_t serl_td3_state_floats(const serl_actor_shape* shape)
+template <int CS>
+int launch_group(const Group& t, int n, int h, cudaStream_t s)
 {
-    if (!shape_ok(shape)) return serl_fail(SERL_ERR_ARG, "serl_td3_state_floats: unsupported actor shape");
-    return 4 * actor_floats(*shape) + 8 * (int64_t)CP;
+    if (h > 128) return serl_launch("td3_group_kernel (wide)", td3_group_kernel<CS, true>, dim3(n * CS), dim3(NT), 0, s, t);
+    return serl_launch("td3_group_kernel", td3_group_kernel<CS, false>, dim3(n * CS), dim3(NT), 0, s, t);
 }
 
-extern "C" int serl_td3_train(const serl_td3_desc* d, void* stream)
+// why a descriptor cannot be trained (nullptr: it can); the checks of serl_td3_train, made before any CUDA call
+const char* desc_error(const serl_td3_desc* d)
 {
-    if (!d) return serl_fail(SERL_ERR_ARG, "serl_td3_train: null descriptor");
     if (!shape_ok(&d->shape))
-        return serl_fail(SERL_ERR_ARG, "serl_td3_train: unsupported actor shape (state 7, action 3, hidden 32/64/72/96/128 with "
-                                       "num_layers >= 1 or hidden 129..320 with num_layers 1..8, activation 0..2)");
-    if (d->batch < 1 || d->batch > SERL_TD3_MAX_BATCH) return serl_fail(SERL_ERR_ARG, "serl_td3_train: batch must be 1..128");
+        return "unsupported actor shape (state 7, action 3, hidden 32/64/72/96/128 with num_layers >= 1 or hidden 129..320 "
+               "with num_layers 1..8, activation 0..2)";
+    if (d->batch < 1 || d->batch > SERL_TD3_MAX_BATCH) return "batch must be 1..128";
     if (d->n_steps < 0 || d->n_valid < d->batch || d->replay_cols < COLS)
-        return serl_fail(SERL_ERR_ARG, "serl_td3_train: bad n_steps / n_valid (>= batch) / replay_cols (>= 19)");
-    if (!d->d_state || !d->d_replay || !d->d_losses) return serl_fail(SERL_ERR_ARG, "serl_td3_train: null state / replay / losses");
+        return "bad n_steps / n_valid (>= batch) / replay_cols (>= 19)";
+    if (!d->d_state || !d->d_replay || !d->d_losses) return "null state / replay / losses";
     if (d->policy_update_freq < 1 || d->first_iteration < 0 || d->critic_adam_steps < 0 || d->actor_adam_steps < 0)
-        return serl_fail(SERL_ERR_ARG, "serl_td3_train: bad policy_update_freq / iteration / Adam step count");
-    if (d->flags & ~SERL_TD3_CHAMPION_TARGET) return serl_fail(SERL_ERR_ARG, "serl_td3_train: unknown flag");
-    const int cs = d->cluster_size ? d->cluster_size : 8;
-    if (cs != 1 && cs != 2 && cs != 4 && cs != 8) return serl_fail(SERL_ERR_ARG, "serl_td3_train: cluster_size must be 0, 1, 2, 4 or 8");
-    if (d->n_steps == 0) return SERL_OK;
+        return "bad policy_update_freq / iteration / Adam step count";
+    if (d->flags & ~SERL_TD3_CHAMPION_TARGET) return "unknown flag";
+    const int cs = d->cluster_size;
+    if (cs != 0 && cs != 1 && cs != 2 && cs != 4 && cs != 8) return "cluster_size must be 0, 1, 2, 4 or 8";
+    return nullptr;
+}
+
+Args make_args(const serl_td3_desc* d)
+{
     Args a;
     a.st = d->d_state; a.replay = d->d_replay; a.cols = d->replay_cols; a.n_valid = d->n_valid;
     a.B = d->batch; a.n_steps = d->n_steps; a.h = d->shape.hidden; a.L = d->shape.num_layers; a.act = d->shape.activation;
@@ -783,16 +824,90 @@ extern "C" int serl_td3_train(const serl_td3_desc* d, void* stream)
     a.seed = d->seed; a.idx_in = d->d_indices;
     a.losses = d->d_losses; a.rec_idx = d->d_rec_indices; a.rec_noise = d->d_rec_noise; a.rec_caps = d->d_rec_caps;
     a.status = d->d_status;
+    a.ws = nullptr;
+    return a;
+}
+
+size_t scratch_floats(const Args& a) { return layout(a.B, a.h, a.L, a.Pa).total; }
+
+}  // namespace
+
+extern "C" int64_t serl_td3_state_floats(const serl_actor_shape* shape)
+{
+    if (!shape_ok(shape)) return serl_fail(SERL_ERR_ARG, "serl_td3_state_floats: unsupported actor shape");
+    return 4 * actor_floats(*shape) + 8 * (int64_t)CP;
+}
+
+extern "C" int serl_td3_train(const serl_td3_desc* d, void* stream)
+{
+    if (!d) return serl_fail(SERL_ERR_ARG, "serl_td3_train: null descriptor");
+    if (const char* why = desc_error(d)) {
+        char msg[256];
+        snprintf(msg, sizeof(msg), "serl_td3_train: %s", why);
+        return serl_fail(SERL_ERR_ARG, msg);
+    }
+    if (d->n_steps == 0) return SERL_OK;
+    Args a = make_args(d);
     const cudaStream_t s = (cudaStream_t)stream;
-    const Lay l = layout(a.B, a.h, a.L, a.Pa);
     void* ws = nullptr;
-    const cudaError_t e = serl_scratch(SERL_SCRATCH_TD3, s, l.total * sizeof(float), &ws);
+    const cudaError_t e = serl_scratch(SERL_SCRATCH_TD3, s, scratch_floats(a) * sizeof(float), &ws);
     if (e != cudaSuccess) return serl_fail_cuda(e, "td3 scratch");
     a.ws = (float*)ws;
-    switch (cs) {
+    switch (d->cluster_size ? d->cluster_size : 8) {
     case 1: return launch<1>(a, s);
     case 2: return launch<2>(a, s);
     case 4: return launch<4>(a, s);
     default: return launch<8>(a, s);
+    }
+}
+
+extern "C" int serl_td3_train_group(const serl_td3_desc* descs, int n, void* stream)
+{
+    if (n < 1 || n > SERL_TD3_MAX_GROUP) return serl_fail(SERL_ERR_ARG, "serl_td3_train_group: n must be 1..SERL_TD3_MAX_GROUP (64)");
+    if (!descs) return serl_fail(SERL_ERR_ARG, "serl_td3_train_group: null descriptors");
+    char msg[256];
+    for (int i = 0; i < n; ++i)
+        if (const char* why = desc_error(descs + i)) {
+            snprintf(msg, sizeof(msg), "serl_td3_train_group: learner %d: %s", i, why);
+            return serl_fail(SERL_ERR_ARG, msg);
+        }
+    const serl_actor_shape& sh = descs[0].shape;
+    const int cs = descs[0].cluster_size ? descs[0].cluster_size : 8;
+    for (int i = 1; i < n; ++i) {
+        const serl_actor_shape& si = descs[i].shape;
+        if (si.state_dim != sh.state_dim || si.action_dim != sh.action_dim || si.hidden != sh.hidden ||
+            si.num_layers != sh.num_layers || si.activation != sh.activation) {
+            snprintf(msg, sizeof(msg), "serl_td3_train_group: learner %d: actor shape differs from learner 0's (one launch trains "
+                                       "one shape)", i);
+            return serl_fail(SERL_ERR_ARG, msg);
+        }
+        if ((descs[i].cluster_size ? descs[i].cluster_size : 8) != cs) {
+            snprintf(msg, sizeof(msg), "serl_td3_train_group: learner %d: cluster_size differs from learner 0's", i);
+            return serl_fail(SERL_ERR_ARG, msg);
+        }
+    }
+    // the learners with steps to take, each with its own slice of one scratch buffer (slices aligned to 128 bytes)
+    Group t{};
+    int m = 0;
+    size_t total = 0;
+    size_t off[SERL_TD3_MAX_GROUP];
+    for (int i = 0; i < n; ++i) {
+        if (descs[i].n_steps == 0) continue;
+        t.a[m] = make_args(descs + i);
+        off[m] = total;
+        total += (scratch_floats(t.a[m]) + 31) / 32 * 32;
+        ++m;
+    }
+    if (m == 0) return SERL_OK;
+    const cudaStream_t s = (cudaStream_t)stream;
+    void* ws = nullptr;
+    const cudaError_t e = serl_scratch(SERL_SCRATCH_TD3, s, total * sizeof(float), &ws);
+    if (e != cudaSuccess) return serl_fail_cuda(e, "td3 scratch");
+    for (int g = 0; g < m; ++g) t.a[g].ws = (float*)ws + off[g];
+    switch (cs) {
+    case 1: return launch_group<1>(t, m, sh.hidden, s);
+    case 2: return launch_group<2>(t, m, sh.hidden, s);
+    case 4: return launch_group<4>(t, m, sh.hidden, s);
+    default: return launch_group<8>(t, m, sh.hidden, s);
     }
 }

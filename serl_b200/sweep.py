@@ -1,0 +1,139 @@
+"""Several independent SERL / TD3 trainings in one process on one GPU, each giving the bits it gives when trained alone.
+
+With `fused_td3`, a generation's RL half is K7 (csrc/td3.cu), one thread-block cluster on a few of the GPU's SMs, and it is
+most of a run's wall-clock time.  `Sweep` moves S runs forward one generation at a time: the head of every run's
+generation (population rollout, SSNE epoch, exploration episode: Agent.train_head), then ONE grouped K7 launch that takes
+every run's gradient steps on its own cluster (td3_fused.train_group), then every run's tail (validation, actor injection,
+next front: Agent.train_tail).  The runs may differ in seed and in any `Parameters` attribute that keeps the actor's shape.
+
+Each run keeps its own state of the global generators the Agent draws from — stdlib `random` (the SSNE planner), legacy
+`np.random` (reference signals, exploration noise, tournaments) and torch's CPU generator (actor initialisation) — and
+every phase of a run runs with that state swapped in (`RNGState`).  Nothing on the fused path draws from torch's default
+CUDA generator (the replay buffers, SSNE and K7 have generators of their own, seeded from the run's `seed`), but
+`torch.manual_seed` also seeds it, so its state is swapped too: the caller's generators come back exactly as they were.
+"""
+import contextlib
+import copy
+import os
+import random
+
+import numpy as np
+import torch
+
+from . import td3_fused
+from .core import agent as agent_mod
+from .rollout import actor_shape
+
+
+class RNGState:
+    """the states of stdlib `random`, legacy `np.random`, torch's CPU generator and, with CUDA, torch's default generator
+    of the current device"""
+    __slots__ = ('py', 'np', 'torch', 'cuda')
+
+    @classmethod
+    def capture(cls):
+        s = cls()
+        s.py, s.np, s.torch = random.getstate(), np.random.get_state(), torch.get_rng_state()
+        s.cuda = torch.cuda.get_rng_state() if torch.cuda.is_available() else None
+        return s
+
+    def restore(self):
+        random.setstate(self.py)
+        np.random.set_state(self.np)
+        torch.set_rng_state(self.torch)
+        if self.cuda is not None:
+            torch.cuda.set_rng_state(self.cuda)
+
+
+@contextlib.contextmanager
+def rng_scope(state):
+    """run the block with the global generators in `state`, store their advanced state back in it, and give the caller's
+    generators back exactly as they were"""
+    outer = RNGState.capture()
+    state.restore()
+    try:
+        yield
+    finally:
+        now = RNGState.capture()
+        state.py, state.np, state.torch, state.cuda = now.py, now.np, now.torch, now.cuda
+        outer.restore()
+
+
+class Run:
+    """one training of a sweep: its Parameters, environment, Agent, generator states and last statistics"""
+    __slots__ = ('params', 'env', 'agent', 'rng', 'stats')
+
+    @property
+    def finished(self):
+        return self.agent.num_frames > self.params.num_frames          # base/train.py's `while num_frames <= frames`
+
+
+def _shape(p):
+    return tuple(getattr(actor_shape(p.hidden_size, p.num_layers, p.activation_actor, p.state_dim, p.action_dim), f)
+                 for f in ('state_dim', 'action_dim', 'hidden', 'num_layers', 'activation'))
+
+
+class Sweep:
+    def __init__(self, runs):
+        """runs: a list of (Parameters, env), each seeded and built as base/train.py:88-94 builds one run"""
+        runs = list(runs)
+        if not runs:
+            raise ValueError('Sweep: no runs')
+        if torch.distributed.is_available() and torch.distributed.is_initialized() and torch.distributed.get_world_size() > 1:
+            raise NotImplementedError('Sweep: runs on one GPU; a torch.distributed world larger than 1 is not supported')
+        for i, (p, _) in enumerate(runs):
+            if not getattr(p, 'fused_td3', False):
+                raise ValueError('Sweep: run %d does not set fused_td3 (the sweep trains every RL half in one K7 launch)' % i)
+            if _shape(p) != _shape(runs[0][0]):
+                raise ValueError('Sweep: run %d has actor shape %s, run 0 has %s (one K7 launch trains one shape)'
+                                 % (i, _shape(p), _shape(runs[0][0])))
+        self.runs = []
+        outer = RNGState.capture()
+        try:
+            for p, env in runs:
+                r = Run()
+                r.params, r.env, r.stats = p, env, None
+                env.seed(p.seed)
+                torch.manual_seed(p.seed)
+                np.random.seed(p.seed)
+                random.seed(p.seed)
+                r.agent = agent_mod.Agent(p, env)
+                r.rng = RNGState.capture()
+                self.runs.append(r)
+        finally:
+            outer.restore()
+
+    @property
+    def finished(self):
+        return all(r.finished for r in self.runs)
+
+    def train(self):
+        """one generation of every run that has not reached its `frames`: returns one statistics dict per run (Agent.train's),
+        None for a finished run"""
+        live = [r for r in self.runs if not r.finished]
+        for r in live:
+            with rng_scope(r.rng):
+                r.agent.train_head()
+        plans = []
+        for r in live:
+            with rng_scope(r.rng):
+                plans.append(r.agent.plan_rl_fused(r.agent.gen_frames))
+        group = [(r, n) for r, n in zip(live, plans) if n]
+        launches = td3_fused.train_group([r.agent.rl_agent for r, _ in group], [r.agent.replay_buffer for r, _ in group],
+                                         [n for _, n in group], [r.agent.rl_iteration + 1 for r, _ in group],
+                                         [r.agent.args.use_champion_target for r, _ in group])
+        losses = dict(zip((id(r) for r, _ in group), td3_fused.group_losses(launches)))
+        for r, n in zip(live, plans):
+            with rng_scope(r.rng):
+                r.stats = r.agent.train_tail(r.agent.finish_rl_fused(n, losses.get(id(r))))
+        live_ids = set(id(r) for r in live)
+        return [r.stats if id(r) in live_ids else None for r in self.runs]
+
+    def save_agent(self, folder=None):
+        """Agent.save_agent of every run into its own folder <folder or the run's save_foldername>/run<i>"""
+        for i, r in enumerate(self.runs):
+            p = copy.copy(r.params)
+            p.save_foldername = os.path.join(folder or r.params.save_foldername, 'run%d' % i) + '/'
+            os.makedirs(p.save_foldername, exist_ok=True)
+            elite = r.stats['elite_index'] if r.stats is not None else None
+            r.agent.save_agent(p, elite)
