@@ -125,7 +125,14 @@ int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shap
  *                SERL_ROLLOUT_STAGGER: K1 launches with two genome slots per CTA run slot 1 half a step behind slot 0
  *                instead of taking both slots' steps together.  Same result bits; slower on an H100 (DESIGN §5), kept to
  *                compare the two schedules in one process
+ *   d_track      optional [pop, n_envs, SERL_TRACK_COLS] f64: per trajectory, over its executed steps k, the sums
+ *                sum |e_theta|, sum |e_phi|, sum |e_beta|, sum e_beta of the tracking error of base/evaluate.py:71-100,
+ *                e_k = ref(t_k) - x[[7, 6, 5]] with x the state env.x holds when step k starts (the native output of reset()'s
+ *                step for k = 0, else of step k - 1, sensor noise included), summed in step order in fp64: nMAE
+ *                (base/core/utils.py:39-58) without a trace.  Selects kernel instantiations of their own (with the gust
+ *                schedule); a launch without it runs the same code as before the field existed
  * t_max <= 0 selects the training defaults (20 s, smooth width 3 s). */
+#define SERL_TRACK_COLS 4
 #define SERL_REPLAY_COLS 20
 #define SERL_ROLLOUT_GUST 1
 #define SERL_ROLLOUT_STAGGER 2
@@ -144,6 +151,7 @@ typedef struct {
     const int32_t* widths; int32_t n_widths;
     const float* d_sensor_noise;
     int32_t flags;                 /* SERL_ROLLOUT_* */
+    double* d_track;
 } serl_rollout_desc;
 int serl_rollout_run(const serl_rollout_desc* desc, void* stream);
 

@@ -17,6 +17,7 @@ ACTIVATIONS = {'tanh': 0, 'elu': 1, 'relu': 2}        # SERL_ACT_* ('relu' is th
 PLANT_VARIANTS = ['h2000_v90', 'ice', 'cg', 'cg_for', 'h2000_v150', 'h10000_v90', 'cg_timed', 'cg_timed_post']   # SERL_PLANT_*
 FAULTS = ['none', 'be', 'jr', 'sa', 'se']             # SERL_FAULT_*
 TRACE_COLS = 22
+TRACK_COLS = 4
 REPLAY_COLS = 20
 MODE_GUST = 1 << 24
 MODE_GUST_UP = 1 << 25
@@ -51,7 +52,7 @@ class RolloutDesc(ctypes.Structure):
                 ('d_env_order', ctypes.c_void_p), ('d_replay', ctypes.c_void_p), ('replay_env', ctypes.c_int32),
                 ('d_status', ctypes.c_void_p), ('sm_limit', ctypes.c_int32),
                 ('widths', ctypes.c_void_p), ('n_widths', ctypes.c_int32), ('d_sensor_noise', ctypes.c_void_p),
-                ('flags', ctypes.c_int32)]
+                ('flags', ctypes.c_int32), ('d_track', ctypes.c_void_p)]
 
 
 class TD3Desc(ctypes.Structure):

@@ -436,6 +436,14 @@ struct RolloutArgs {
 constexpr int PLANT_TABN = PT_TOTAL + SERL_PLANT_COUNT * PLANT_NPV;
 constexpr int PLANT_TABN2 = (PLANT_TABN + 1) & ~1;
 
+// Tracking-error accumulators of the evaluation suite (serl_rollout_desc.d_track): the kernels take them as a launch
+// argument of their own, next to the argument block, so that adding them moved no field of the training instantiations.
+//   out  [pop * n_envs][SERL_TRACK_COLS] f64, written at the end of each trajectory
+//   ho   [TRACK_CARRY][Handoff.n] f64: the sums and the carried controlled state of a trajectory K1's time-split schedule
+//        hands to another slot (the rest of its record is Handoff)
+struct TrackArgs { double* out; double* ho; };
+#define TRACK_CARRY (SERL_TRACK_COLS + 3)
+
 struct Env {
     double X[NX];
     const real* tab;         // plant tables (shared or global memory)
@@ -447,6 +455,9 @@ struct Env {
     int fault, k;
     bool done;
     int gust;                // env_mode >> 24: 1 = SERL_MODE_GUST, 3 = with SERL_MODE_GUST_UP
+    // TRACK instantiations only: sum |e_theta|, sum |e_phi|, sum |e_beta|, sum e_beta, then the controlled state
+    // (theta, phi, beta) of env.x when the next step starts
+    double trk[TRACK_CARRY];
 };
 
 // one plant step of the env (reset's zero-command step and env_step share this single plant_step instance)
@@ -514,6 +525,11 @@ __device__ __forceinline__ void traj_store(const Env& e, const RolloutArgs& a, s
     a.steps[traj] = e.k;
     if (a.status && !isfinite(e.ret + e.X[3] + e.X[7] + e.X[9])) atomicOr(a.status, SERL_STATUS_NONFINITE);
 }
+__device__ __forceinline__ void track_store(const Env& e, const TrackArgs& tk, size_t traj)
+{
+#pragma unroll
+    for (int c = 0; c < SERL_TRACK_COLS; ++c) tk.out[traj * SERL_TRACK_COLS + c] = e.trk[c];
+}
 
 // sensor-noise shim (envs/noise/citation.py:72-82, same model in envs/gust): every native step() output gets
 // p,q,r += 3e-5 + 6.3e-4 z; alpha += 4e-10 z; beta += 1.8e-3 + 2.7e-4 z; phi,theta += 4e-3 + 3.2e-5 z  (7 draws per call,
@@ -534,7 +550,8 @@ __device__ __forceinline__ void sensor_noise(const RolloutArgs& a, size_t traj, 
 // reset(): initialize(), one zero-command step returns the initial state (phlabenv.py:401-428). obs = [0,0,0,p,q,r,alpha]
 // GUST names the same plant_step instance as env_step<STAB, GUST> (call 0 has no gust stage either way), so a kernel
 // carries one copy of the step code.
-template <bool STAB = false, bool GUST = false>
+// TRACK: zero the tracking-error sums; the controlled state before step 0 is reset()'s output env.x.
+template <bool STAB = false, bool GUST = false, bool TRACK = false>
 static __device__ __forceinline__ void env_reset(Env& e, const RolloutArgs& a, int env, float* obs, size_t traj = 0)
 {
     const double* ic = plant_ic(a.env_mode[env] & 0xff);
@@ -544,6 +561,11 @@ static __device__ __forceinline__ void env_reset(Env& e, const RolloutArgs& a, i
 #pragma unroll
     for (int i = 0; i < 8; ++i) x0[i] = e.X[i];
     sensor_noise(a, traj, 0, x0);
+    if constexpr (TRACK) {      // env.x before step 0 = reset()'s step output (with the sensor noise of call 0)
+#pragma unroll
+        for (int c = 0; c < SERL_TRACK_COLS; ++c) e.trk[c] = 0.0;
+        e.trk[SERL_TRACK_COLS] = x0[7]; e.trk[SERL_TRACK_COLS + 1] = x0[6]; e.trk[SERL_TRACK_COLS + 2] = x0[5];
+    }
     obs[0] = obs[1] = obs[2] = 0.f;
     obs[3] = (float)x0[0]; obs[4] = (float)x0[1]; obs[5] = (float)x0[2]; obs[6] = (float)x0[4];
     double U[3] = {0.0, 0.0, 0.0}, cmd[3];
@@ -553,7 +575,10 @@ static __device__ __forceinline__ void env_reset(Env& e, const RolloutArgs& a, i
 }
 
 // one CitationEnv.step (phlabenv.py:430-482) + the bookkeeping of Agent.evaluate (agent.py:85-118)
-template <bool STAB = false, bool GUST = false>
+// TRACK: + the tracking error of base/evaluate.py:71-100, e = ref(t) - x_ctrl with x_ctrl = env.x[[7, 6, 5]] when the step
+// starts (the native step output of the previous step, or of reset()'s step: in the sensor-noise builds it carries the
+// noise, as the reference's env.x does), accumulated in step order in fp64
+template <bool STAB = false, bool GUST = false, bool TRACK = false>
 static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, size_t traj, int actor, bool replay, const float* a, float* obs)
 {
     const double bound = 10.0 * DEG2RAD;                       // phlabenv.py:208
@@ -593,6 +618,11 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
     const double r_th = ref_deg(e.ref_lv, e.ref_st, t, t <= ar.t_max ? e.theta_trim : 0.0, ar.smooth_w) * DEG2RAD;
     const double r_ph = ref_deg(e.ref_lv + SERL_REF_BLOCKS, e.ref_st + SERL_REF_BLOCKS, t, 0.0, ar.smooth_w) * DEG2RAD;
     const double e0 = r_th - xo[7], e1 = r_ph - xo[6], e2 = 0.0 - xo[5];
+    if constexpr (TRACK) {
+        const double et = r_th - e.trk[SERL_TRACK_COLS], ep = r_ph - e.trk[SERL_TRACK_COLS + 1], eb = 0.0 - e.trk[SERL_TRACK_COLS + 2];
+        e.trk[0] += fabs(et); e.trk[1] += fabs(ep); e.trk[2] += fabs(eb); e.trk[3] += eb;
+        e.trk[SERL_TRACK_COLS] = xo[7]; e.trk[SERL_TRACK_COLS + 1] = xo[6]; e.trk[SERL_TRACK_COLS + 2] = xo[5];
+    }
     const double c0 = fabs(fmin(fmax(k_err * e0, -1.0), 1.0));
     const double c1 = fabs(fmin(fmax(k_err * e1, -1.0), 1.0));
     const double c2 = fabs(fmin(fmax(k_err4 * e2, -1.0), 1.0));

@@ -347,9 +347,11 @@ __global__ void genome_layout_kernel(const float* __restrict__ w, float* __restr
 // 207 KB genome leaves no room for them).
 // GUST: the launch contains envs of the gust build (serl_rollout_desc.flags & SERL_ROLLOUT_GUST); the training instantiation
 // carries no trace of the feature (a gust env in it raises SERL_STATUS_GUST_FLAG)
-template <int H, bool TABS, bool GUST>
+// TRACK: the launch writes the tracking-error sums `tk` (serl_rollout_desc.d_track; instantiated with GUST only); the
+// sums travel in the hand-over records too
+template <int H, bool TABS, bool GUST, bool TRACK = false>
 __global__ void __launch_bounds__(MAX_CTA_THREADS, 1)
-rollout_kernel_persist(RolloutArgs ar)
+rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];     // same alignment as plant_smem_tab (plant_env.cuh)
     __shared__ uint64_t gbar[4];                       // one mbarrier per genome slot
@@ -441,12 +443,16 @@ rollout_kernel_persist(RolloutArgs ar)
 #pragma unroll
                         for (int i = 0; i < 7; ++i) __stcg(ar.ho.obs + (size_t)i * ar.ho.n + hx, obs[i]);
                         __stcg(ar.ho.k + hx, e.k | ((e.done ? 1 : 0) << 30));
+                        if constexpr (TRACK)
+#pragma unroll
+                            for (int i = 0; i < TRACK_CARRY; ++i) __stcg(tk.ho + (size_t)i * ar.ho.n + hx, e.trk[i]);
                     }
                     __threadfence();
                     __syncwarp();
                     if (lane == 0) atomicExch(ar.ho.flag + slot * wps + wslot, 1);
                 } else if (valid) {
                     traj_store(e, ar, traj);
+                    if constexpr (TRACK) track_store(e, tk, traj);
                 }
                 in_seg = false;
             }
@@ -513,8 +519,11 @@ rollout_kernel_persist(RolloutArgs ar)
                         for (int i = 0; i < 7; ++i) obs[i] = __ldcg(ar.ho.obs + (size_t)i * ar.ho.n + hx);
                         const int kk = __ldcg(ar.ho.k + hx);
                         e.k = kk & 0x3fffffff; e.done = ((kk >> 30) & 1) != 0;
+                        if constexpr (TRACK)
+#pragma unroll
+                            for (int i = 0; i < TRACK_CARRY; ++i) e.trk[i] = __ldcg(tk.ho + (size_t)i * ar.ho.n + hx);
                     } else {
-                        env_reset<TABS, GUST>(e, ar, env, obs, traj);
+                        env_reset<TABS, GUST, TRACK>(e, ar, env, obs, traj);
                     }
                 } else {
                     env_idle(e, ar, pv_base, obs);
@@ -528,14 +537,15 @@ rollout_kernel_persist(RolloutArgs ar)
         if (!__syncthreads_or(in_seg || pending || stage < 3)) break;
         const bool mine = in_seg && !e.done && e.k < ke;
         if (actor_half && __any_sync(0xffffffffu, mine)) actor_forward<H>(actfn, w, L, lane, xb, obs, a);
-        if ((!stagger || !actor_half) && mine) env_step<TABS, GUST>(e, ar, traj, actor, replay, a, obs);
+        if ((!stagger || !actor_half) && mine) env_step<TABS, GUST, TRACK>(e, ar, traj, actor, replay, a, obs);
         actor_half ^= stagger;
     }
 }
 
 // ---- cross-check kernel: every thread evaluates the whole MLP for its own env (any hidden size that fits) ------
+template <bool TRACK = false>
 __global__ void __launch_bounds__(128)
-rollout_kernel_simple(RolloutArgs ar)
+rollout_kernel_simple(RolloutArgs ar, TrackArgs tk)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float* w = reinterpret_cast<float*>(smem_raw);
@@ -553,14 +563,15 @@ rollout_kernel_simple(RolloutArgs ar)
     e.tab = plant_tables_blob;
     float obs[7], a[3];
     env_bind<true>(e, ar, env, &plant_pv[0][0], (size_t)actor * ar.n_envs + env);
-    env_reset<false, true>(e, ar, env, obs, (size_t)actor * ar.n_envs + env);
+    env_reset<false, true, TRACK>(e, ar, env, obs, (size_t)actor * ar.n_envs + env);
     const size_t traj = (size_t)actor * ar.n_envs + env;
     const bool replay = ar.replay != nullptr && env == ar.replay_env;
     while (!e.done) {
         actor_forward_simple(w, ar.sh, bufA, bufB, tid, 128, obs, a);
-        env_step<false, true>(e, ar, traj, actor, replay, a, obs);       // (the gust schedule costs nothing that matters here)
+        env_step<false, true, TRACK>(e, ar, traj, actor, replay, a, obs);       // (the gust schedule costs nothing that matters here)
     }
     traj_store(e, ar, traj);
+    if constexpr (TRACK) track_store(e, tk, traj);
 }
 
 // ---- Actor.forward for a batch of observations (same device functions as the rollout) --------------------------
@@ -718,7 +729,7 @@ static void choose_shape(int pop, int n_envs, int apc_max, int sms, int* apc_out
 }
 
 template <int H, bool TABS>
-static int launch_persist(RolloutArgs& ar, int apc_max, bool gust, bool stagger, cudaStream_t s)
+static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust, bool stagger, cudaStream_t s)
 {
     const int sms = ar.sm_limit > 0 && ar.sm_limit < serl_device_sms() ? ar.sm_limit : serl_device_sms();
     int apc, wps;
@@ -737,7 +748,7 @@ static int launch_persist(RolloutArgs& ar, int apc_max, bool gust, bool stagger,
     // scratch: genomes in the shared-memory layout + hand-over records of the time-split schedule (stream-ordered)
     const size_t wt_bytes = (size_t)ar.pop * ar.P4 * 4;
     const long long hn = ar.n_tasks > ar.n_slots ? ar.n_slots * wps * 32 : 0;
-    const size_t ho_bytes = (size_t)hn * (NX * 8 + 8 + 8 + 7 * 4 + 4) + (size_t)(hn / 32) * 4;
+    const size_t ho_bytes = (size_t)hn * (NX * 8 + 8 + 8 + 7 * 4 + 4) + (size_t)(hn / 32) * 4 + (tk.out ? (size_t)hn * TRACK_CARRY * 8 + 8 : 0);
     void* scratch = nullptr;
     cudaError_t e = serl_scratch(SERL_SCRATCH_K1, s, wt_bytes + ho_bytes + 512, &scratch);
     if (e != cudaSuccess) return serl_fail_cuda(e, "rollout_kernel launch");
@@ -752,7 +763,8 @@ static int launch_persist(RolloutArgs& ar, int apc_max, bool gust, bool stagger,
         ar.ho.ret = (double*)p; p += (size_t)hn * 8;
         ar.ho.obs = (float*)p; p += (size_t)hn * 7 * 4;
         ar.ho.k = (int*)p; p += (size_t)hn * 4;
-        ar.ho.flag = (int*)p;
+        ar.ho.flag = (int*)p; p += (size_t)(hn / 32) * 4;
+        if (tk.out) tk.ho = (double*)(((uintptr_t)p + 7) & ~(uintptr_t)7);
         e = cudaMemsetAsync(ar.ho.flag, 0, (size_t)(hn / 32) * 4, s);
         if (e != cudaSuccess) return serl_fail_cuda(e, "rollout_kernel launch");
     }
@@ -763,8 +775,9 @@ static int launch_persist(RolloutArgs& ar, int apc_max, bool gust, bool stagger,
     if (rc != SERL_OK) return rc;
     const size_t smem = (TABS ? (size_t)PLANT_TABN2 * sizeof(real) : 0) + (size_t)apc * ar.P4 * 4 +
                         (size_t)apc * wps * actor_xbuf_floats(H) * 4;
-    void (*const kernel)(RolloutArgs) = gust ? rollout_kernel_persist<H, TABS, true> : rollout_kernel_persist<H, TABS, false>;
-    return serl_launch("rollout_kernel launch", kernel, (unsigned)grid, apc * wps * 32, smem, s, ar);
+    void (*const kernel)(RolloutArgs, TrackArgs) = tk.out ? rollout_kernel_persist<H, TABS, true, true>
+                                                 : gust ? rollout_kernel_persist<H, TABS, true> : rollout_kernel_persist<H, TABS, false>;
+    return serl_launch("rollout_kernel launch", kernel, (unsigned)grid, apc * wps * 32, smem, s, ar, tk);
 }
 
 // the hidden sizes the warp actor is instantiated for: when H is one of them, calls f(std::integral_constant<int, H>())
@@ -814,6 +827,7 @@ extern "C" int32_t serl_actor_tc_widths(const serl_actor_shape* shape, int32_t* 
 // K1 launch: the checks only this kernel needs, then the genome part of the argument block and the kernel for the hidden size
 static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t s)
 {
+    const TrackArgs tk = {d.d_track, nullptr};
     if (!actor_shape_ok(d.shape))
         return serl_fail(SERL_ERR_ARG, "serl_rollout: unsupported actor shape (state_dim = 7, action_dim = 3, 2 <= hidden <= 256)");
     if (d.pop > 65535) return serl_fail(SERL_ERR_ARG, "serl_rollout: pop must be <= 65535 per call");       // grid.y of the simple kernel
@@ -824,7 +838,8 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
     if (!k1_warp(d.shape)) {
         if (!k1_fits(d.shape)) return serl_fail(SERL_ERR_UNSUPPORTED, "serl_rollout: genome + activations exceed 227 KB of shared memory");
         const size_t smem = (size_t)ar.P4 * 4 + 2ull * H * 128 * 4;
-        return serl_launch("rollout_kernel launch", rollout_kernel_simple, dim3((d.n_envs + 127) / 128, d.pop), 128, smem, s, ar);
+        return serl_launch("rollout_kernel launch", d.d_track ? rollout_kernel_simple<true> : rollout_kernel_simple<false>,
+                           dim3((d.n_envs + 127) / 128, d.pop), 128, smem, s, ar, tk);
     }
     // as many genome slots per CTA as shared memory holds next to the plant tables (h <= 72: two; h = 96: one);
     // h = 128 (207 KB genome) reads the tables through L1 instead.  A slot is its genome and the actor exchange buffers
@@ -841,9 +856,9 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
     warp_hidden(H, [&](auto h) {
         constexpr int HH = decltype(h)::value;
         if constexpr (HH == 128)          // the one size instantiated with the tables in global memory too
-            rc = tabs ? launch_persist<HH, true>(ar, apc_max, gust, stagger, s) : launch_persist<HH, false>(ar, apc_max, gust, stagger, s);
+            rc = tabs ? launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, s) : launch_persist<HH, false>(ar, tk, apc_max, gust, stagger, s);
         else
-            rc = launch_persist<HH, true>(ar, apc_max, gust, stagger, s);
+            rc = launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, s);
     });
     return rc;
 }

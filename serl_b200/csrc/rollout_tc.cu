@@ -622,10 +622,11 @@ __device__ __forceinline__ void tc_load_small(TcCtx& c, const TcArgs& ar, int ac
 
 // GUST as in rollout_kernel_persist: the launch has envs of the gust build, and reset and step share the one plant_step
 // instance of the kernel; without it a gust env raises SERL_STATUS_GUST_FLAG.  DEEP: more than two widths
-// (tc_actor_forward_deep); the two-width instantiations run tc_actor_forward.
-template <int ACT, bool GUST, bool DEEP>
+// (tc_actor_forward_deep); the two-width instantiations run tc_actor_forward.  TRACK: the launch writes the tracking-error
+// sums `tk` (serl_rollout_desc.d_track; instantiated with GUST only)
+template <int ACT, bool GUST, bool DEEP, bool TRACK = false>
 __global__ void __launch_bounds__(2 * TC_THREADS, 1)
-rollout_kernel_tc(const __grid_constant__ TcArgs ar)
+rollout_kernel_tc(const __grid_constant__ TcArgs ar, TrackArgs tk)
 {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     __shared__ uint64_t bars[TC_STAGES];
@@ -650,7 +651,7 @@ rollout_kernel_tc(const __grid_constant__ TcArgs ar)
         float obs[7], a[3];
         if (valid) {
             env_bind<GUST>(e, r, env, pv_base, (size_t)actor * r.n_envs + env);
-            env_reset<true, GUST>(e, r, env, obs, (size_t)actor * r.n_envs + env);
+            env_reset<true, GUST, TRACK>(e, r, env, obs, (size_t)actor * r.n_envs + env);
         } else {
             env_idle(e, r, pv_base, obs);
         }
@@ -659,9 +660,10 @@ rollout_kernel_tc(const __grid_constant__ TcArgs ar)
         while (group_any(c.grp, !e.done)) {
             if constexpr (DEEP) tc_actor_forward_deep<ACT>(c, ar, tiles_actor, obs, a);
             else tc_actor_forward<ACT>(c, ar, tiles_actor, obs, a);
-            if (!e.done) env_step<true, GUST>(e, r, traj, actor, replay, a, obs);
+            if (!e.done) env_step<true, GUST, TRACK>(e, r, traj, actor, replay, a, obs);
         }
         if (valid) traj_store(e, r, traj);
+        if constexpr (TRACK) if (valid) track_store(e, tk, traj);
     }
 }
 
@@ -768,16 +770,22 @@ int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, cudaStream
     int sms = serl_device_sms();
     if (d.sm_limit > 0 && d.sm_limit < sms) sms = d.sm_limit;
     const long long grid = (ar.n_tasks + 1) / 2 < sms ? (ar.n_tasks + 1) / 2 : sms;
-    static void (*const kernels[3][2][2])(TcArgs) = {          // [SERL_ACT_*][gust][deep]
+    static void (*const kernels[3][2][2])(TcArgs, TrackArgs) = {          // [SERL_ACT_*][gust][deep]
         {{rollout_kernel_tc<SERL_ACT_TANH, false, false>, rollout_kernel_tc<SERL_ACT_TANH, false, true>},
          {rollout_kernel_tc<SERL_ACT_TANH, true, false>, rollout_kernel_tc<SERL_ACT_TANH, true, true>}},
         {{rollout_kernel_tc<SERL_ACT_ELU, false, false>, rollout_kernel_tc<SERL_ACT_ELU, false, true>},
          {rollout_kernel_tc<SERL_ACT_ELU, true, false>, rollout_kernel_tc<SERL_ACT_ELU, true, true>}},
         {{rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true>},
          {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, false>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, true>}}};
+    static void (*const track_kernels[3][2])(TcArgs, TrackArgs) = {                                  // [SERL_ACT_*][deep]
+        {rollout_kernel_tc<SERL_ACT_TANH, true, false, true>, rollout_kernel_tc<SERL_ACT_TANH, true, true, true>},
+        {rollout_kernel_tc<SERL_ACT_ELU, true, false, true>, rollout_kernel_tc<SERL_ACT_ELU, true, true, true>},
+        {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, false, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, true, true>}};
+    const TrackArgs tk = {d.d_track, nullptr};
     // one CTA = the two groups of TC_THREADS threads
-    return serl_launch("rollout_kernel_tc launch", kernels[d.shape.activation][(d.flags & SERL_ROLLOUT_GUST) != 0][ar.n_layers > 1],
-                       (unsigned)grid, 2 * TC_THREADS, smem, s, ar);
+    return serl_launch("rollout_kernel_tc launch", d.d_track ? track_kernels[d.shape.activation][ar.n_layers > 1]
+                                                             : kernels[d.shape.activation][(d.flags & SERL_ROLLOUT_GUST) != 0][ar.n_layers > 1],
+                       (unsigned)grid, 2 * TC_THREADS, smem, s, ar, tk);
 }
 
 extern "C" int serl_actor_forward_wide(const float* d_genome, const int32_t* widths, int32_t n_widths, int32_t activation,

@@ -9,7 +9,7 @@ import numpy as np
 import torch
 
 from . import _native
-from ._native import FAULTS, MODE_GUST, MODE_GUST_UP, PLANT_VARIANTS, REPLAY_COLS, TRACE_COLS
+from ._native import FAULTS, MODE_GUST, MODE_GUST_UP, PLANT_VARIANTS, REPLAY_COLS, TRACE_COLS, TRACK_COLS
 
 HORIZON = 2001          # envs/phlabenv.py:82,181,392: t_max = 20 s, dt = 0.01, done checked before t += dt
 # trace record columns (SERL_TRACE_COLS): state before the step, commanded deflection, reward, action fed to the env, error
@@ -57,7 +57,7 @@ def num_params(shape):
 
 
 class RolloutResult:
-    __slots__ = ('returns', 'steps', 'fitness', 'trace', 'actions', 'smoothness', 'replay', 'status')
+    __slots__ = ('returns', 'steps', 'fitness', 'trace', 'actions', 'smoothness', 'replay', 'status', 'track')
 
     trace_x = property(lambda s: s.trace[..., TRACE_X])
     trace_u = property(lambda s: s.trace[..., TRACE_U])
@@ -82,13 +82,15 @@ def variant_sorted_order(env_mode):
 
 def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon=HORIZON, trace=False, out=None, action_noise=None,
                        actions=False, t_max=None, smooth_width=None, env_order=None, replay_env=None, status=True, sm_limit=0,
-                       fitness=True, widths=None, sensor_noise=None, gust=False, stagger=False):
+                       fitness=True, widths=None, sensor_noise=None, gust=False, stagger=False, track=False):
     """weights [pop,P] fp32 cuda; ref_levels/ref_starts [n_envs,2,6] f64 cuda; env_mode [n_envs] int32 cuda.
     env_order: optional int32 [n_envs] permutation (see variant_sorted_order); replay_env: record the transitions of that env
     of every actor into result.replay [pop, horizon, REPLAY_COLS]; status: carry the device status word (result.check());
     sm_limit: SMs this launch may occupy (0 = all); fitness=False skips the per-actor mean kernel.
     stagger=True: K1's two genome slots of a CTA run half a step apart instead of taking their steps together (same results,
     slower on an H100; to time the two schedules against each other).
+    track=True: result.track [pop, n_envs, TRACK_COLS] f64 holds each trajectory's tracking-error sums
+    (sum |e_theta|, sum |e_phi|, sum |e_beta|, sum e_beta; serl_rollout_desc.d_track), the nMAE of a trajectory without a trace.
     widths=[w0, w1, ..., w_{n-1}] (2 to 9 widths): width-list actors on the tensor-core kernel K1-TC (csrc/rollout_tc.cu); `shape`
     then only supplies the activation.  widths=None flies the uniform actor `shape` on K1, or on K1-TC with [h] * (L + 1) when its
     genome does not fit K1's kernels (tc_widths)."""
@@ -118,6 +120,7 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
         r.actions = torch.empty((pop, n_envs, horizon, 3), dtype=torch.float32, device=dev) if actions else None
         r.replay = torch.empty((pop, horizon, REPLAY_COLS), dtype=torch.float32, device=dev) if replay_env is not None else None
         r.status = torch.zeros((1,), dtype=torch.int32, device=dev) if status else None
+        r.track = torch.empty((pop, n_envs, TRACK_COLS), dtype=torch.float64, device=dev) if track else None
         if trace:
             r.trace = torch.full((pop, n_envs, horizon, TRACE_COLS), float('nan'), dtype=torch.float64, device=dev)
     elif r.status is not None:
@@ -134,6 +137,7 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     d.d_env_order = p(env_order)
     d.d_replay, d.replay_env = p(getattr(r, 'replay', None)), int(replay_env if replay_env is not None else 0)
     d.d_status = p(getattr(r, 'status', None))
+    d.d_track = p(getattr(r, 'track', None))
     if sm_limit < 0:         # leave -sm_limit SMs to concurrent small launches
         sm_limit = max(1, torch.cuda.get_device_properties(dev).multi_processor_count + int(sm_limit))
     d.sm_limit = int(sm_limit)

@@ -20,7 +20,7 @@ import random
 import numpy as np
 import torch
 
-from . import td3_fused
+from . import evaluation, td3_fused
 from .core import agent as agent_mod
 from .rollout import actor_shape
 
@@ -128,6 +128,18 @@ class Sweep:
                 r.stats = r.agent.train_tail(r.agent.finish_rl_fused(n, losses.get(id(r))))
         live_ids = set(id(r) for r in live)
         return [r.stats if id(r) in live_ids else None for r in self.runs]
+
+    def evaluate(self, conditions, refs, num_trails=1):
+        """evaluation.evaluate_population of every run's population on `conditions` with the references `refs`: all runs
+        share one actor shape, so their populations stack into one call.  Returns one PopulationEval per run (None for a
+        run without a population)."""
+        pops = [r.agent.pop.genomes if len(r.agent.pop) else None for r in self.runs]
+        live = [g for g in pops if g is not None]
+        if not live:
+            return [None] * len(self.runs)
+        res = evaluation.evaluate_population(torch.cat(live), self.runs[0].agent.shape, conditions, refs, num_trails)
+        parts = iter(res.split([g.shape[0] for g in live]))
+        return [next(parts) if g is not None else None for g in pops]
 
     def save_agent(self, folder=None):
         """Agent.save_agent of every run into its own folder <folder or the run's save_foldername>/run<i>"""
