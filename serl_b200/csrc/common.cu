@@ -20,6 +20,9 @@ int serl_fail(int code, const char* msg)
 int serl_fail_cuda(cudaError_t e, const char* where)
 {
     snprintf(g_err, sizeof(g_err), "%s: %s", where, cudaGetErrorString(e));
+    // consume the runtime's record of an error reported here (e.g. a refused shared-memory opt-in), so that the caller's
+    // next CUDA call does not fail with it again
+    cudaGetLastError();
     return SERL_ERR_CUDA;
 }
 

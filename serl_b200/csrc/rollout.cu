@@ -796,12 +796,25 @@ static bool warp_hidden(int H, F&& f)
 }
 static bool warp_hidden(int H) { return warp_hidden(H, [](auto) {}); }
 
-// K1's kernel for a valid shape: the warp actor when the hidden size is instantiated and the genome fits one slot, else the
-// one-thread-per-env kernel, which needs the genome and two activation buffers of 128 envs in shared memory
-static bool k1_warp(const serl_actor_shape& sh)
+// Shared memory of the warp kernel: the plant tables (unless it reads them from global memory) and `apc` genome slots, a slot
+// being the genome and the actor exchange buffers of up to 4 warps, within the opt-in limit less the static shared memory
+// (128 B) and the alignment of the dynamic part
+constexpr size_t K1_SMEM_BUDGET = SERL_SMEM_OPTIN - 256;
+constexpr size_t K1_TAB_BYTES = (size_t)PLANT_TABN2 * sizeof(real);
+static size_t k1_slot_bytes(const serl_actor_shape& sh)
 {
     const size_t P4 = ((size_t)serl_actor_num_params(&sh) + 3) & ~(size_t)3;
-    return !force_simple() && warp_hidden(sh.hidden) && P4 * 4 <= SERL_SMEM_OPTIN;
+    return P4 * 4 + 4ull * actor_xbuf_floats(sh.hidden) * 4;        // h = 128, L = 3: 218 KB
+}
+
+// K1's kernel for a valid shape: the warp actor when it can be launched — the hidden size is instantiated and one slot fits
+// next to the plant tables, or h = 128, the one size also instantiated with the tables in global memory, and one slot fits
+// alone — else the one-thread-per-env kernel, which needs the genome and two activation buffers of 128 envs in shared memory
+static bool k1_warp(const serl_actor_shape& sh)
+{
+    if (force_simple() || !warp_hidden(sh.hidden)) return false;
+    const size_t slot = k1_slot_bytes(sh);
+    return K1_TAB_BYTES + slot <= K1_SMEM_BUDGET || (sh.hidden == 128 && slot <= K1_SMEM_BUDGET);
 }
 static bool k1_fits(const serl_actor_shape& sh)
 {
@@ -841,14 +854,11 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
         return serl_launch("rollout_kernel launch", d.d_track ? rollout_kernel_simple<true> : rollout_kernel_simple<false>,
                            dim3((d.n_envs + 127) / 128, d.pop), 128, smem, s, ar, tk);
     }
-    // as many genome slots per CTA as shared memory holds next to the plant tables (h <= 72: two; h = 96: one);
-    // h = 128 (207 KB genome) reads the tables through L1 instead.  A slot is its genome and the actor exchange buffers
-    // of up to 4 warps.
-    const size_t tab_bytes = (size_t)PLANT_TABN2 * sizeof(real);
-    const size_t budget = SERL_SMEM_OPTIN - 256;       // static shared memory + alignment of the dynamic part
-    const size_t slot_bytes = (size_t)ar.P4 * 4 + 4ull * actor_xbuf_floats(H) * 4;      // h = 128: 218 KB
-    const bool tabs = tab_bytes + slot_bytes <= budget;
-    int apc_max = (int)(((tabs ? budget - tab_bytes : budget)) / slot_bytes);
+    // as many genome slots per CTA as shared memory holds next to the plant tables (L = 3: two for h <= 72, one for h = 96);
+    // h = 128 from L = 3 on (207 KB genome) reads the tables through L1 instead (k1_warp: every other shape has room for them)
+    const size_t slot_bytes = k1_slot_bytes(d.shape);
+    const bool tabs = K1_TAB_BYTES + slot_bytes <= K1_SMEM_BUDGET;
+    int apc_max = (int)(((tabs ? K1_SMEM_BUDGET - K1_TAB_BYTES : K1_SMEM_BUDGET)) / slot_bytes);
     if (apc_max > 4) apc_max = 4;
     if (apc_max > 2 && H > 32) apc_max = 2;
     const bool gust = (d.flags & SERL_ROLLOUT_GUST) != 0, stagger = (d.flags & SERL_ROLLOUT_STAGGER) != 0;
@@ -957,11 +967,13 @@ extern "C" int serl_actor_forward(const float* d_genome, const serl_actor_shape*
     const int grid = (n + 127) / 128;
     const size_t smem = (size_t)((P + 3) & ~3) * 4;
     int rc = SERL_OK;
-    const auto warp_launch = [&](auto h) {      // genome + the exchange buffers of 4 warps
-        rc = serl_launch("actor_forward_kernel", actor_forward_kernel<decltype(h)::value>, grid, 128, smem + 4ull * actor_xbuf_floats(H) * 4,
-                         s, d_genome, P, *shape, d_obs, n, d_actions);
+    const size_t warp_smem = smem + 4ull * actor_xbuf_floats(H) * 4;      // genome + the exchange buffers of 4 warps
+    const auto warp_launch = [&](auto h) {
+        rc = serl_launch("actor_forward_kernel", actor_forward_kernel<decltype(h)::value>, grid, 128, warp_smem, s, d_genome, P, *shape, d_obs,
+                         n, d_actions);
     };
-    if (!force_simple() && warp_hidden(H, warp_launch)) return rc;
+    // the warp kernel when it holds the genome, else the one-thread-per-env kernel (no static shared memory in either)
+    if (!force_simple() && warp_smem <= SERL_SMEM_OPTIN && warp_hidden(H, warp_launch)) return rc;
     const size_t sm2 = smem + 2ull * H * 128 * 4;
     if (sm2 > SERL_SMEM_OPTIN) return serl_fail(SERL_ERR_UNSUPPORTED, "serl_actor_forward: genome + activations exceed shared memory");
     return serl_launch("actor_forward_kernel", actor_forward_kernel_simple, grid, 128, sm2, s, d_genome, P, *shape, d_obs, n, d_actions);
