@@ -122,6 +122,13 @@ int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shap
  *   flags        SERL_ROLLOUT_GUST: some env of the launch flies the gust build (SERL_MODE_GUST) — selects the kernel
  *                instantiation with the gust schedule (the training instantiation carries no trace of it; a gust env in a launch
  *                without the flag sets SERL_STATUS_GUST_FLAG)
+ *                SERL_ROLLOUT_PER_ACTOR_REFS: every actor flies its own env block.  d_ref_levels / d_ref_starts are then
+ *                [pop, n_envs, 2, SERL_REF_BLOCKS] and d_env_mode is [pop, n_envs]; env e of actor a reads row a * n_envs + e
+ *                (levels, starts, mode, and the V0 of its replay rows).  The reference's own evaluation draws fresh signals for
+ *                every episode of every actor (base/core/agent.py:234-241), and independent runs can share one launch.  Not
+ *                with d_env_order (inside an actor's block a warp's lanes already share a mode) or d_track: SERL_ERR_ARG before
+ *                any CUDA call; pop * n_envs must fit int32.  Kernel instantiations of their own; a launch without the bit runs
+ *                the same code as before the bit existed
  *                SERL_ROLLOUT_STAGGER: K1 launches with two genome slots per CTA run slot 1 half a step behind slot 0
  *                instead of taking both slots' steps together.  Same result bits; slower on an H100 (DESIGN §5), kept to
  *                compare the two schedules in one process
@@ -136,6 +143,7 @@ int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shap
 #define SERL_REPLAY_COLS 20
 #define SERL_ROLLOUT_GUST 1
 #define SERL_ROLLOUT_STAGGER 2
+#define SERL_ROLLOUT_PER_ACTOR_REFS 4
 enum { SERL_STATUS_NONFINITE = 1,     /* a trajectory's state / return became NaN or infinite */
        SERL_STATUS_GUST_FLAG = 2 };   /* an env has SERL_MODE_GUST but the launch was not made with SERL_ROLLOUT_GUST */
 typedef struct {

@@ -23,6 +23,7 @@ MODE_GUST = 1 << 24
 MODE_GUST_UP = 1 << 25
 ROLLOUT_GUST = 1
 ROLLOUT_STAGGER = 2
+ROLLOUT_PER_ACTOR_REFS = 4
 STATUS_NONFINITE = 1
 STATUS_GUST_FLAG = 2
 # include/serl_td3.h (K7, the fused TD3 learner)

@@ -17,9 +17,10 @@ stats keys, with the per-generation fitness hot path on the GPU:
   * `self.evolver.epoch` runs on the device-resident genomes (core/mod_neuro_evo.py -> serl_b200/evo.py).
 
 Documented deviations from the reference (DESIGN.md): the conditions at agent.py:45,228 are read as intended
-(`if self.pop`), save_agent's `isEmpty()` works; all actors of a generation see the SAME num_envs reference signals (fair
-ranking) instead of an independent draw per episode; every trajectory starts from a fresh env (zero stale error); TD3 samples
-its batches with a device generator instead of stdlib `random` (so the SSNE planner's stream does not depend on buffer sizes).
+(`if self.pop`), save_agent's `isEmpty()` works; by default all actors of a generation see the SAME num_envs reference
+signals (fair ranking) — `independent_references` gives every episode of every actor its own draw, as the reference does;
+every trajectory starts from a fresh env (zero stale error); TD3 samples its batches with a device generator instead of
+stdlib `random` (so the SSNE planner's stream does not depend on buffer sizes).
 """
 import os
 import time
@@ -48,8 +49,23 @@ class _Generation:
 
 class _Front:
     """the launches a generation starts with: RL exploration / validation flights, speculative champion validations, the
-    population rollout — and the signature of what they read."""
-    __slots__ = ('signature', 'f_explore', 'f_rlval', 'spec', 'val_draws', 'pop')
+    population rollout — and the signature of what they read.  `pop_draws` holds the population's reference draws while
+    its launch is deferred (launch_population_group), `pop` the launched rollout."""
+    __slots__ = ('signature', 'f_explore', 'f_rlval', 'spec', 'val_draws', 'pop', 'pop_draws', 'sm_limit')
+
+
+class _PopDraws:
+    """the population's reference draws of one generation (host f64): levels / starts [n_envs, 2, 6] shared by every actor,
+    or [pop, n_envs, 2, 6] with independent_references"""
+    __slots__ = ('levels', 'starts')
+
+
+def population_draws(env, pop, n_envs, independent):
+    """the reference signals of a generation's population evaluation, drawn from the global np.random stream.
+    independent=False: n_envs draws that every actor flies (fair ranking).  independent=True: the reference's
+    `for net in pop: for i in range(num_evals): evaluate(net)` (base/core/agent.py:234-241), whose every reset() draws
+    anew — pop x n_envs draws, actor by actor, evaluation by evaluation.  Returns the list of (levels, starts) in draw order."""
+    return [env.draw_reference() for _ in range(pop * n_envs if independent else n_envs)]
 
 
 class Agent:
@@ -81,13 +97,16 @@ class Agent:
         self.champion = None
         self.champion_actor = None
         self.champion_history = None
-        self.store_population_transitions = (args.frac_frames_train > 0 or getattr(args, 'mut_type', 'normal') in ('proximal', 'safe')
-                                             or bool(getattr(args, 'distil_crossover', False)))
+        self.store_population_transitions = stores_population_transitions(args)
         # single-actor flights run next to the population rollout, each on its own high-priority stream and spare SM
         self._side, self._side2, self._champ = (torch.cuda.Stream(self.device, priority=-1) for _ in range(3))
         # launch the next generation's rollouts at the end of train() (see there); False = strictly one generation per call
         self.prefetch_generation = bool(getattr(args, 'prefetch_generation', True))
         self._prefetched = None
+        # the fronts this Agent launches leave their population rollout to the caller (Sweep: launch_population_group)
+        self.defer_population = False
+        self._front = None
+        self._front_prefetched = False
         # speculative validation of last generation's elites hides the champion's validation latency INSIDE a generation;
         # with the next generation's front launched ahead it is hidden anyway, and the spare SMs go to the population
         self.speculative_validations = int(getattr(args, 'speculative_validations', 0 if self.prefetch_generation else 3))
@@ -294,41 +313,69 @@ class Agent:
         — identical on every rank."""
         return self._finish_population(self._launch_population(sm_limit))
 
-    def _launch_population(self, sm_limit=0):
-        """the asynchronous half: reference draws, K0 + K1 (+ K6) and the per-actor record of this rank's shard, all queued
-        on the current stream; nothing here waits for the device and nothing is stored yet."""
-        n_envs = int(getattr(self.args, 'num_envs', self.args.num_evals))
-        draws = [self.env.draw_reference() for _ in range(n_envs)]
-        lv = _to_device(np.stack([d[0] for d in draws]), self.device)
-        st = _to_device(np.stack([d[1] for d in draws]), self.device)
-        md = torch.full((n_envs,), self.env.mode_code, dtype=torch.int32, device=self.device)
-        want_sm = bool(getattr(self.args, 'population_smoothness', False)) or bool(self.args.smooth_fitness)
+    def _n_envs(self):
+        return int(getattr(self.args, 'num_envs', self.args.num_evals))
+
+    def _want_population_smoothness(self):
+        return bool(getattr(self.args, 'population_smoothness', False)) or bool(self.args.smooth_fitness)
+
+    def _draw_population(self) -> _PopDraws:
+        """the population's reference draws (population_draws; the host side of _launch_population)"""
+        n_envs = self._n_envs()
+        independent = bool(getattr(self.args, 'independent_references', False))
+        draws = population_draws(self.env, len(self.pop), n_envs, independent)
+        d = _PopDraws()
+        d.levels, d.starts = np.stack([x[0] for x in draws]), np.stack([x[1] for x in draws])
+        if independent:
+            d.levels, d.starts = d.levels.reshape(len(self.pop), n_envs, 2, -1), d.starts.reshape(len(self.pop), n_envs, 2, -1)
+        return d
+
+    def _launch_population(self, sm_limit=0, draws=None):
+        """the asynchronous half: reference draws (unless given), K0 + K1 (+ K6) and the per-actor record of this rank's shard,
+        all queued on the current stream; nothing here waits for the device and nothing is stored yet.  Independent draws fly
+        as per-actor env blocks, of which this rank passes its shard's rows."""
+        draws = draws if draws is not None else self._draw_population()
+        n_envs = self._n_envs()
         store = self.store_population_transitions
         world, rank = engine.world_info()
         pop = len(self.pop)
         lo, hi = engine.shard_bounds(pop, world, rank)
-        horizon = self._horizon()
+        if draws.levels.ndim == 4:
+            lv, st = _to_device(draws.levels[lo:hi], self.device), _to_device(draws.starts[lo:hi], self.device)
+            md = torch.full((hi - lo, n_envs), self.env.mode_code, dtype=torch.int32, device=self.device)
+        else:
+            lv, st = _to_device(draws.levels, self.device), _to_device(draws.starts, self.device)
+            md = torch.full((n_envs,), self.env.mode_code, dtype=torch.int32, device=self.device)
+        want_sm = self._want_population_smoothness()
         rec = torch.zeros((hi - lo, 7), dtype=torch.float64, device=self.device)
         r = None
         if hi > lo:
-            r = rollout.population_rollout(self.pop.genomes[lo:hi], self.shape, lv, st, md, horizon=horizon, actions=want_sm,
+            r = rollout.population_rollout(self.pop.genomes[lo:hi], self.shape, lv, st, md, horizon=self._horizon(), actions=want_sm,
                                            replay_env=(n_envs - 1) if store else None, sm_limit=sm_limit, fitness=False,
                                            **self._eval_kw())
             sm_all = None
             if want_sm:
                 sm_all = rollout.smoothness(r.actions, r.steps)
                 r.actions = None
-            ret_p = r.returns + sm_all if self.args.smooth_fitness else r.returns
-            stp = r.steps.to(torch.float64)
-            rec[:, 0] = ret_p.mean(dim=1)                                     # fitness (agent.py:245)
-            rec[:, 1] = stp.sum(1)                                            # episode-length statistics
-            rec[:, 2] = (stp ** 2).sum(1)
-            rec[:, 3] = stp[:, n_envs - 1]                                    # frames of the stored evaluation
-            if sm_all is not None:
-                rec[:, 4] = sm_all.sum(1)
-                rec[:, 5] = (sm_all ** 2).sum(1)
-                rec[:, 6] = 1.0
+            rec = self._population_record(r, sm_all)
         return (r, rec, (lv, st, md))
+
+    def _population_record(self, r, sm_all):
+        """the per-actor record [fitness, sum len, sum len^2, stored frames, sum sm, sum sm^2, has sm] of the rollout result r
+        (K6 smoothness sm_all, or None), queued on the current stream"""
+        n_envs = r.returns.shape[1]
+        rec = torch.zeros((r.returns.shape[0], 7), dtype=torch.float64, device=self.device)
+        ret_p = r.returns + sm_all if self.args.smooth_fitness else r.returns
+        stp = r.steps.to(torch.float64)
+        rec[:, 0] = ret_p.mean(dim=1)                                     # fitness (agent.py:245)
+        rec[:, 1] = stp.sum(1)                                            # episode-length statistics
+        rec[:, 2] = (stp ** 2).sum(1)
+        rec[:, 3] = stp[:, n_envs - 1]                                    # frames of the stored evaluation
+        if sm_all is not None:
+            rec[:, 4] = sm_all.sum(1)
+            rec[:, 5] = (sm_all ** 2).sum(1)
+            rec[:, 6] = 1.0
+        return rec
 
     def _finish_population(self, launched):
         """the collecting half: all-gather of the record (and of the stored transitions), buffers, counters."""
@@ -367,9 +414,12 @@ class Agent:
                 id(env), env.mode_code, float(env.t_max), int(getattr(self.args, 'num_envs', self.args.num_evals)), len(self.pop))
 
     def _launch_front(self):
+        """queue a generation's front.  With defer_population the population's references are drawn at their place in the
+        front (the np.random stream advances as without it) and its launch is left to launch_population_group."""
         args = self.args
         fr = _Front()
         fr.signature = self._signature()
+        fr.pop_draws, fr.sm_limit = None, 0
         log = bool(args.should_log)
         # RL exploration episode (agent.py:267-268): independent of the population -> side stream, launched first.  The RL
         # validation (:273-275) reads the RL actor AFTER train_rl; when no gradient step can happen it joins the side stream.
@@ -389,8 +439,24 @@ class Agent:
                                                         stream=self._spec_streams[j], draws=fr.val_draws)
             # leave one SM per flight that can be in the air next to the rollout: exploration, RL validation, the previous
             # generation's champion validation, speculative validations
-            fr.pop = self._launch_population(sm_limit=-(3 + len(fr.spec) // 2))
+            fr.sm_limit = -(3 + len(fr.spec) // 2)
+            if self.defer_population:
+                fr.pop_draws = self._draw_population()
+            else:
+                fr.pop = self._launch_population(sm_limit=fr.sm_limit)
         return fr
+
+    def take_front(self):
+        """the front this generation starts with: the one the previous train_tail queued if nothing it read has changed, else
+        a new one.  train_head takes it itself unless the caller has (Sweep takes every run's front, then launches the
+        deferred populations together)."""
+        if self._front is None:
+            fr, self._prefetched = self._prefetched, None
+            if fr is not None and fr.signature != self._signature():
+                fr = None              # the population / RL actor / environment changed since it was launched: fly again
+            self._front_prefetched = fr is not None
+            self._front = fr if fr is not None else self._launch_front()
+        return self._front
 
     def train(self):
         """one generation (agent.py:211-315): its head (population, epoch, exploration episode), the RL half, its tail"""
@@ -418,12 +484,11 @@ class Agent:
         self.timing = {}
         self._t_prev = time.perf_counter()
         lap, tm = self._lap, self.timing
-        fr, self._prefetched = self._prefetched, None
-        if fr is not None and fr.signature != self._signature():
-            fr = None                  # the population / RL actor / environment changed since it was launched: fly again
-        tm['front_prefetched'] = float(fr is not None)
-        if fr is None:
-            fr = self._launch_front()
+        fr = self.take_front()
+        self._front = None
+        tm['front_prefetched'] = float(self._front_prefetched)
+        if fr.pop_draws is not None:     # deferred, and no group launch took it: it flies alone
+            fr.pop, fr.pop_draws = self._launch_population(fr.sm_limit, fr.pop_draws), None
         f_explore, g.f_rlval, spec, val_draws = fr.f_explore, fr.f_rlval, fr.spec, fr.val_draws
         lap('launch_front')
         g.f_champ = None
@@ -540,6 +605,62 @@ class Agent:
         if self.rl_history is not None:
             np.savetxt(os.path.join(parameters.save_foldername, 'rl_statehistory_episode%d.txt' % self.num_episodes),
                        self.rl_history, header=str(self.num_episodes))
+
+
+def stores_population_transitions(args):
+    """the population's stored evaluations feed a buffer: the RL half trains, or proximal / safe mutation or the
+    distillation crossover read the per-actor buffers"""
+    return (args.frac_frames_train > 0 or getattr(args, 'mut_type', 'normal') in ('proximal', 'safe')
+            or bool(getattr(args, 'distil_crossover', False)))
+
+
+def population_key(args, env):
+    """what runs must agree on to fly their populations in one launch (Sweep), None for a run without a population: actor
+    shape, envs per actor, horizon and episode length, the gust flag, whether actions are recorded for the smoothness and
+    whether transitions are stored.  Everything else (genomes, references, env mode) travels per actor."""
+    if not args.pop_size:
+        return None
+    shape = (args.state_dim, args.action_dim, args.hidden_size, args.num_layers, args.activation_actor.lower())
+    want_sm = bool(getattr(args, 'population_smoothness', False)) or bool(args.smooth_fitness)
+    return (shape, int(getattr(args, 'num_envs', args.num_evals)), int(round(env.t_max / env.dt)) + 1, float(env.t_max),
+            rollout.mode_gust(env.mode_code), want_sm, stores_population_transitions(args))
+
+
+def launch_population_group(members):
+    """ONE rollout launch for the deferred populations of several Agents on one device whose population_key agrees:
+    members = [(agent, front)], each front holding its run's reference draws.  Every actor flies its own env block
+    (SERL_ROLLOUT_PER_ACTOR_REFS): a run's shared draws repeat for each of its actors, independent ones are its actors'
+    own.  Each front gets its slice of the result (returns, steps, replay rows, K6 smoothness) and its per-actor record,
+    bit for bit what its own launch gives.  The launch has ONE status word: a non-finite trajectory in any run of it
+    raises in every run that shares it.  A group of one flies alone, as Agent.train does."""
+    a0, f0 = members[0]
+    if len(members) == 1:
+        f0.pop, f0.pop_draws = a0._launch_population(f0.sm_limit, f0.pop_draws), None
+        return
+    n_envs = a0._n_envs()
+    blocks = lambda a, x: np.broadcast_to(x, (len(a.pop), n_envs) + x.shape[-2:])
+    lv = _to_device(np.concatenate([blocks(a, f.pop_draws.levels) for a, f in members]), a0.device)
+    st = _to_device(np.concatenate([blocks(a, f.pop_draws.starts) for a, f in members]), a0.device)
+    md = _to_device(np.concatenate([np.full((len(a.pop), n_envs), a.env.mode_code, dtype=np.int32) for a, _ in members]), a0.device)
+    genomes = torch.cat([a.pop.genomes for a, _ in members])
+    want_sm = a0._want_population_smoothness()
+    r = rollout.population_rollout(genomes, a0.shape, lv, st, md, horizon=a0._horizon(), actions=want_sm,
+                                   replay_env=(n_envs - 1) if a0.store_population_transitions else None,
+                                   sm_limit=min(f.sm_limit for _, f in members), fitness=False, **a0._eval_kw())
+    sm_all = None
+    if want_sm:
+        sm_all = rollout.smoothness(r.actions, r.steps)        # one block per trajectory: the same bits in any batch
+        r.actions = None
+    lo = 0
+    for a, f in members:
+        hi = lo + len(a.pop)
+        part = rollout.RolloutResult()
+        part.returns, part.steps, part.status = r.returns[lo:hi], r.steps[lo:hi], r.status
+        part.replay = r.replay[lo:hi] if r.replay is not None else None
+        part.fitness = part.trace = part.actions = part.smoothness = part.track = None
+        f.pop = (part, a._population_record(part, sm_all[lo:hi] if sm_all is not None else None), (lv, st, md, genomes))
+        f.pop_draws = None
+        lo = hi
 
 
 def _to_device(a, device):

@@ -487,6 +487,8 @@ __device__ __forceinline__ void apply_fault(int fault, const double* u, double* 
 // bind the env's constants (plant variant row, fault shim, reference signals, trim pitch); no dynamics.
 // GUST: the kernel instantiation flies the gust schedule (serl_rollout_desc.flags & SERL_ROLLOUT_GUST).  One without it
 // carries no trace of the feature, so a gust env bound there is reported (SERL_STATUS_GUST_FLAG) instead of flown as nominal.
+// `env` is the row of env_mode / ref_levels / ref_starts: the env index, or actor * n_envs + env in the PER_ACTOR
+// instantiations (SERL_ROLLOUT_PER_ACTOR_REFS), whose callers pass that row to env_reset as well.
 template <bool GUST>
 __device__ __forceinline__ void env_bind(Env& e, const RolloutArgs& a, int env, const real* pv_base, size_t traj)
 {
@@ -578,7 +580,8 @@ static __device__ __forceinline__ void env_reset(Env& e, const RolloutArgs& a, i
 // TRACK: + the tracking error of base/evaluate.py:71-100, e = ref(t) - x_ctrl with x_ctrl = env.x[[7, 6, 5]] when the step
 // starts (the native step output of the previous step, or of reset()'s step: in the sensor-noise builds it carries the
 // noise, as the reference's env.x does), accumulated in step order in fp64
-template <bool STAB = false, bool GUST = false, bool TRACK = false>
+// PER_ACTOR: env_mode holds one row per (actor, env); the replay row's V0 comes from the actor's own replay_env row
+template <bool STAB = false, bool GUST = false, bool TRACK = false, bool PER_ACTOR = false>
 static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, size_t traj, int actor, bool replay, const float* a, float* obs)
 {
     const double bound = 10.0 * DEG2RAD;                       // phlabenv.py:208
@@ -655,7 +658,8 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
         rp[10] = o0; rp[11] = o1; rp[12] = o2; rp[13] = o3; rp[14] = o4; rp[15] = o5; rp[16] = o6;
         rp[17] = (float)reward;
         rp[18] = done ? 1.f : 0.f;
-        const double v0 = plant_ic(ar.env_mode[ar.replay_env] & 0xff)[3];
+        const int* modes = PER_ACTOR ? ar.env_mode + (size_t)actor * ar.n_envs : ar.env_mode;
+        const double v0 = plant_ic(modes[ar.replay_env] & 0xff)[3];
         const bool cost = (fabs(xo[4]) * RAD2DEG > 11.0) || (fabs(xo[6]) * RAD2DEG > 0.75 * max_phi) || (xo[3] < v0 / 3.0);
         rp[19] = cost ? 1.f : 0.f;
     }

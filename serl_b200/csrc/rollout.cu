@@ -349,7 +349,10 @@ __global__ void genome_layout_kernel(const float* __restrict__ w, float* __restr
 // carries no trace of the feature (a gust env in it raises SERL_STATUS_GUST_FLAG)
 // TRACK: the launch writes the tracking-error sums `tk` (serl_rollout_desc.d_track; instantiated with GUST only); the
 // sums travel in the hand-over records too
-template <int H, bool TABS, bool GUST, bool TRACK = false>
+// PER_ACTOR: every actor flies its own env block (SERL_ROLLOUT_PER_ACTOR_REFS): env `env` of actor `actor` binds row
+// actor * n_envs + env of env_mode / ref_levels / ref_starts, also when a slot resumes it from a hand-over record
+// (instantiated without TRACK, with both GUST values)
+template <int H, bool TABS, bool GUST, bool TRACK = false, bool PER_ACTOR = false>
 __global__ void __launch_bounds__(MAX_CTA_THREADS, 1)
 rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
 {
@@ -508,8 +511,9 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
                 valid = eslot < ar.n_envs;
                 const int env = valid ? (ar.env_order ? ar.env_order[eslot] : eslot) : 0;
                 traj = (size_t)actor * ar.n_envs + env;
+                const int row = PER_ACTOR ? (int)traj : env;
                 if (valid) {
-                    env_bind<GUST>(e, ar, env, pv_base, traj);
+                    env_bind<GUST>(e, ar, row, pv_base, traj);
                     if (from_h) {
                         const long long hx = (slot - 1) * slot_threads + wslot * 32 + lane;
 #pragma unroll
@@ -523,7 +527,7 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
 #pragma unroll
                             for (int i = 0; i < TRACK_CARRY; ++i) e.trk[i] = __ldcg(tk.ho + (size_t)i * ar.ho.n + hx);
                     } else {
-                        env_reset<TABS, GUST, TRACK>(e, ar, env, obs, traj);
+                        env_reset<TABS, GUST, TRACK>(e, ar, row, obs, traj);
                     }
                 } else {
                     env_idle(e, ar, pv_base, obs);
@@ -537,13 +541,14 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
         if (!__syncthreads_or(in_seg || pending || stage < 3)) break;
         const bool mine = in_seg && !e.done && e.k < ke;
         if (actor_half && __any_sync(0xffffffffu, mine)) actor_forward<H>(actfn, w, L, lane, xb, obs, a);
-        if ((!stagger || !actor_half) && mine) env_step<TABS, GUST, TRACK>(e, ar, traj, actor, replay, a, obs);
+        if ((!stagger || !actor_half) && mine) env_step<TABS, GUST, TRACK, PER_ACTOR>(e, ar, traj, actor, replay, a, obs);
         actor_half ^= stagger;
     }
 }
 
 // ---- cross-check kernel: every thread evaluates the whole MLP for its own env (any hidden size that fits) ------
-template <bool TRACK = false>
+// PER_ACTOR as in rollout_kernel_persist
+template <bool TRACK = false, bool PER_ACTOR = false>
 __global__ void __launch_bounds__(128)
 rollout_kernel_simple(RolloutArgs ar, TrackArgs tk)
 {
@@ -562,13 +567,14 @@ rollout_kernel_simple(RolloutArgs ar, TrackArgs tk)
     Env e;
     e.tab = plant_tables_blob;
     float obs[7], a[3];
-    env_bind<true>(e, ar, env, &plant_pv[0][0], (size_t)actor * ar.n_envs + env);
-    env_reset<false, true, TRACK>(e, ar, env, obs, (size_t)actor * ar.n_envs + env);
+    const int row = PER_ACTOR ? actor * ar.n_envs + env : env;
+    env_bind<true>(e, ar, row, &plant_pv[0][0], (size_t)actor * ar.n_envs + env);
+    env_reset<false, true, TRACK>(e, ar, row, obs, (size_t)actor * ar.n_envs + env);
     const size_t traj = (size_t)actor * ar.n_envs + env;
     const bool replay = ar.replay != nullptr && env == ar.replay_env;
     while (!e.done) {
         actor_forward_simple(w, ar.sh, bufA, bufB, tid, 128, obs, a);
-        env_step<false, true, TRACK>(e, ar, traj, actor, replay, a, obs);       // (the gust schedule costs nothing that matters here)
+        env_step<false, true, TRACK, PER_ACTOR>(e, ar, traj, actor, replay, a, obs);       // (the gust schedule costs nothing that matters here)
     }
     traj_store(e, ar, traj);
     if constexpr (TRACK) track_store(e, tk, traj);
@@ -729,7 +735,7 @@ static void choose_shape(int pop, int n_envs, int apc_max, int sms, int* apc_out
 }
 
 template <int H, bool TABS>
-static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust, bool stagger, cudaStream_t s)
+static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust, bool stagger, bool per_actor, cudaStream_t s)
 {
     const int sms = ar.sm_limit > 0 && ar.sm_limit < serl_device_sms() ? ar.sm_limit : serl_device_sms();
     int apc, wps;
@@ -775,8 +781,10 @@ static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust,
     if (rc != SERL_OK) return rc;
     const size_t smem = (TABS ? (size_t)PLANT_TABN2 * sizeof(real) : 0) + (size_t)apc * ar.P4 * 4 +
                         (size_t)apc * wps * actor_xbuf_floats(H) * 4;
-    void (*const kernel)(RolloutArgs, TrackArgs) = tk.out ? rollout_kernel_persist<H, TABS, true, true>
-                                                 : gust ? rollout_kernel_persist<H, TABS, true> : rollout_kernel_persist<H, TABS, false>;
+    void (*const kernel)(RolloutArgs, TrackArgs) =
+        tk.out      ? rollout_kernel_persist<H, TABS, true, true>
+        : per_actor ? (gust ? rollout_kernel_persist<H, TABS, true, false, true> : rollout_kernel_persist<H, TABS, false, false, true>)
+        : gust      ? rollout_kernel_persist<H, TABS, true> : rollout_kernel_persist<H, TABS, false>;
     return serl_launch("rollout_kernel launch", kernel, (unsigned)grid, apc * wps * 32, smem, s, ar, tk);
 }
 
@@ -846,12 +854,14 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
     if (d.pop > 65535) return serl_fail(SERL_ERR_ARG, "serl_rollout: pop must be <= 65535 per call");       // grid.y of the simple kernel
     if (d.horizon >= (1 << 30)) return serl_fail(SERL_ERR_ARG, "serl_rollout: horizon too long");        // Handoff.k: steps | done << 30
     const int H = d.shape.hidden;
+    const bool per_actor = (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) != 0;
     ar.weights = d.d_weights; ar.P = (int)serl_actor_num_params(&d.shape); ar.sh = d.shape;
     ar.P4 = (ar.P + 3) & ~3;
     if (!k1_warp(d.shape)) {
         if (!k1_fits(d.shape)) return serl_fail(SERL_ERR_UNSUPPORTED, "serl_rollout: genome + activations exceed 227 KB of shared memory");
         const size_t smem = (size_t)ar.P4 * 4 + 2ull * H * 128 * 4;
-        return serl_launch("rollout_kernel launch", d.d_track ? rollout_kernel_simple<true> : rollout_kernel_simple<false>,
+        return serl_launch("rollout_kernel launch",
+                           d.d_track ? rollout_kernel_simple<true> : per_actor ? rollout_kernel_simple<false, true> : rollout_kernel_simple<false>,
                            dim3((d.n_envs + 127) / 128, d.pop), 128, smem, s, ar, tk);
     }
     // as many genome slots per CTA as shared memory holds next to the plant tables (L = 3: two for h <= 72, one for h = 96);
@@ -866,9 +876,10 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
     warp_hidden(H, [&](auto h) {
         constexpr int HH = decltype(h)::value;
         if constexpr (HH == 128)          // the one size instantiated with the tables in global memory too
-            rc = tabs ? launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, s) : launch_persist<HH, false>(ar, tk, apc_max, gust, stagger, s);
+            rc = tabs ? launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, per_actor, s)
+                      : launch_persist<HH, false>(ar, tk, apc_max, gust, stagger, per_actor, s);
         else
-            rc = launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, s);
+            rc = launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, per_actor, s);
     });
     return rc;
 }
@@ -885,6 +896,12 @@ static int check_desc(const serl_rollout_desc& d)
     if (d.d_replay && (d.replay_env < 0 || d.replay_env >= d.n_envs)) return serl_fail(SERL_ERR_ARG, "serl_rollout: replay_env out of range");
     if (d.t_max > 0.0 && !(d.smooth_width > 0.0)) return serl_fail(SERL_ERR_ARG, "serl_rollout: smooth_width must be > 0");
     if (d.n_widths > 0 && !d.widths) return serl_fail(SERL_ERR_ARG, "serl_rollout: n_widths > 0 but widths is null");
+    if (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) {
+        // inside one actor's block the lanes of a warp already share a mode: no lane permutation
+        if (d.d_env_order) return serl_fail(SERL_ERR_ARG, "serl_rollout: SERL_ROLLOUT_PER_ACTOR_REFS does not take d_env_order");
+        if (d.d_track) return serl_fail(SERL_ERR_ARG, "serl_rollout: SERL_ROLLOUT_PER_ACTOR_REFS does not take d_track");
+        if ((int64_t)d.pop * d.n_envs > INT32_MAX) return serl_fail(SERL_ERR_ARG, "serl_rollout: pop * n_envs must fit int32 with per-actor refs");
+    }
     return SERL_OK;
 }
 

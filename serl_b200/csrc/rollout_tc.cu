@@ -623,8 +623,9 @@ __device__ __forceinline__ void tc_load_small(TcCtx& c, const TcArgs& ar, int ac
 // GUST as in rollout_kernel_persist: the launch has envs of the gust build, and reset and step share the one plant_step
 // instance of the kernel; without it a gust env raises SERL_STATUS_GUST_FLAG.  DEEP: more than two widths
 // (tc_actor_forward_deep); the two-width instantiations run tc_actor_forward.  TRACK: the launch writes the tracking-error
-// sums `tk` (serl_rollout_desc.d_track; instantiated with GUST only)
-template <int ACT, bool GUST, bool DEEP, bool TRACK = false>
+// sums `tk` (serl_rollout_desc.d_track; instantiated with GUST only).  PER_ACTOR: env `env` of actor `actor` binds row
+// actor * n_envs + env of env_mode / ref_levels / ref_starts (SERL_ROLLOUT_PER_ACTOR_REFS; instantiated without TRACK)
+template <int ACT, bool GUST, bool DEEP, bool TRACK = false, bool PER_ACTOR = false>
 __global__ void __launch_bounds__(2 * TC_THREADS, 1)
 rollout_kernel_tc(const __grid_constant__ TcArgs ar, TrackArgs tk)
 {
@@ -650,8 +651,9 @@ rollout_kernel_tc(const __grid_constant__ TcArgs ar, TrackArgs tk)
         e.tab = tab;
         float obs[7], a[3];
         if (valid) {
-            env_bind<GUST>(e, r, env, pv_base, (size_t)actor * r.n_envs + env);
-            env_reset<true, GUST, TRACK>(e, r, env, obs, (size_t)actor * r.n_envs + env);
+            const int row = PER_ACTOR ? actor * r.n_envs + env : env;
+            env_bind<GUST>(e, r, row, pv_base, (size_t)actor * r.n_envs + env);
+            env_reset<true, GUST, TRACK>(e, r, row, obs, (size_t)actor * r.n_envs + env);
         } else {
             env_idle(e, r, pv_base, obs);
         }
@@ -660,7 +662,7 @@ rollout_kernel_tc(const __grid_constant__ TcArgs ar, TrackArgs tk)
         while (group_any(c.grp, !e.done)) {
             if constexpr (DEEP) tc_actor_forward_deep<ACT>(c, ar, tiles_actor, obs, a);
             else tc_actor_forward<ACT>(c, ar, tiles_actor, obs, a);
-            if (!e.done) env_step<true, GUST, TRACK>(e, r, traj, actor, replay, a, obs);
+            if (!e.done) env_step<true, GUST, TRACK, PER_ACTOR>(e, r, traj, actor, replay, a, obs);
         }
         if (valid) traj_store(e, r, traj);
         if constexpr (TRACK) if (valid) track_store(e, tk, traj);
@@ -781,10 +783,19 @@ int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, cudaStream
         {rollout_kernel_tc<SERL_ACT_TANH, true, false, true>, rollout_kernel_tc<SERL_ACT_TANH, true, true, true>},
         {rollout_kernel_tc<SERL_ACT_ELU, true, false, true>, rollout_kernel_tc<SERL_ACT_ELU, true, true, true>},
         {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, false, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, true, true>}};
+    static void (*const per_actor_kernels[3][2][2])(TcArgs, TrackArgs) = {   // [SERL_ACT_*][gust][deep]
+        {{rollout_kernel_tc<SERL_ACT_TANH, false, false, false, true>, rollout_kernel_tc<SERL_ACT_TANH, false, true, false, true>},
+         {rollout_kernel_tc<SERL_ACT_TANH, true, false, false, true>, rollout_kernel_tc<SERL_ACT_TANH, true, true, false, true>}},
+        {{rollout_kernel_tc<SERL_ACT_ELU, false, false, false, true>, rollout_kernel_tc<SERL_ACT_ELU, false, true, false, true>},
+         {rollout_kernel_tc<SERL_ACT_ELU, true, false, false, true>, rollout_kernel_tc<SERL_ACT_ELU, true, true, false, true>}},
+        {{rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, true>},
+         {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, false, false, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, true, false, true>}}};
     const TrackArgs tk = {d.d_track, nullptr};
+    const bool gust = (d.flags & SERL_ROLLOUT_GUST) != 0, deep = ar.n_layers > 1;
     // one CTA = the two groups of TC_THREADS threads
-    return serl_launch("rollout_kernel_tc launch", d.d_track ? track_kernels[d.shape.activation][ar.n_layers > 1]
-                                                             : kernels[d.shape.activation][(d.flags & SERL_ROLLOUT_GUST) != 0][ar.n_layers > 1],
+    return serl_launch("rollout_kernel_tc launch", d.d_track ? track_kernels[d.shape.activation][deep]
+                                                   : (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) ? per_actor_kernels[d.shape.activation][gust][deep]
+                                                                                             : kernels[d.shape.activation][gust][deep],
                        (unsigned)grid, 2 * TC_THREADS, smem, s, ar, tk);
 }
 

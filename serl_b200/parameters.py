@@ -6,6 +6,8 @@ Differences from the reference (documented in DESIGN.md):
     classic operators (crossover_inplace / mutate_inplace); distillation and Jacobian-scaled mutation need per-actor
     replay buffers + autograd and are listed as "next" (SURVEY.md 8(f) N3).
   * num_envs: environments per actor and generation flown by the rollout kernel (defaults to num_evals = 3).
+  * independent_references: every population episode draws its own reference signals, as the reference does (default
+    False: every actor of a generation flies the same num_envs draws).
 """
 import os
 from pprint import pprint
@@ -70,6 +72,9 @@ class Parameters:
             self._verbose_crossover = g('verbose_crossover', False)
         # engine knobs
         self.num_envs = g('num_envs', getattr(self, 'num_evals', 3))
+        # every episode of every actor draws its own reference signals, as base/core/agent.py:234-241 does (the default gives
+        # all actors of a generation the same num_envs draws: fair ranking)
+        self.independent_references = bool(g('independent_refs', False))
         # Agent.train() queues the next generation's rollouts before it waits for its own validation scores (core/agent.py)
         self.prefetch_generation = bool(g('prefetch_generation', True))
         self.state_dim = None

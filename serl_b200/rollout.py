@@ -84,6 +84,8 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
                        actions=False, t_max=None, smooth_width=None, env_order=None, replay_env=None, status=True, sm_limit=0,
                        fitness=True, widths=None, sensor_noise=None, gust=False, stagger=False, track=False):
     """weights [pop,P] fp32 cuda; ref_levels/ref_starts [n_envs,2,6] f64 cuda; env_mode [n_envs] int32 cuda.
+    Per-actor env blocks: ref_levels/ref_starts [pop,n_envs,2,6] and env_mode [pop,n_envs] give every actor its own n_envs
+    envs (SERL_ROLLOUT_PER_ACTOR_REFS; the shapes select the layout; not with env_order or track).
     env_order: optional int32 [n_envs] permutation (see variant_sorted_order); replay_env: record the transitions of that env
     of every actor into result.replay [pop, horizon, REPLAY_COLS]; status: carry the device status word (result.check());
     sm_limit: SMs this launch may occupy (0 = all); fitness=False skips the per-actor mean kernel.
@@ -101,10 +103,12 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     pop, P = weights.shape
     assert weights.dtype == torch.float32 and weights.is_contiguous()
     assert P == (num_params_wide(widths) if widths else num_params(shape)), (P, widths)
-    n_envs = env_mode.shape[0]
-    assert ref_levels.shape == (n_envs, 2, 6) and ref_levels.dtype == torch.float64 and ref_levels.is_contiguous()
-    assert ref_starts.shape == (n_envs, 2, 6) and ref_starts.dtype == torch.float64 and ref_starts.is_contiguous()
-    assert env_mode.dtype == torch.int32
+    per_actor = env_mode.dim() == 2
+    n_envs = env_mode.shape[-1]
+    block = (pop, n_envs) if per_actor else (n_envs,)
+    assert env_mode.shape == block and env_mode.dtype == torch.int32 and (env_mode.is_contiguous() or not per_actor)
+    assert ref_levels.shape == block + (2, 6) and ref_levels.dtype == torch.float64 and ref_levels.is_contiguous()
+    assert ref_starts.shape == block + (2, 6) and ref_starts.dtype == torch.float64 and ref_starts.is_contiguous()
     if action_noise is not None:
         assert action_noise.shape == (pop, n_envs, horizon, 3) and action_noise.dtype == torch.float32 and action_noise.is_contiguous()
     if env_order is not None:
@@ -144,7 +148,8 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     if sensor_noise is not None:      # envs/noise/citation.py:72-82: standard-normal draws [pop, n_envs, horizon + 1, 7]
         assert sensor_noise.shape == (pop, n_envs, horizon + 1, 7) and sensor_noise.dtype == torch.float32 and sensor_noise.is_contiguous()
         d.d_sensor_noise = p(sensor_noise)
-    d.flags = (_native.ROLLOUT_GUST if gust else 0) | (_native.ROLLOUT_STAGGER if stagger else 0)   # gust: mode_code(...) & MODE_GUST
+    d.flags = ((_native.ROLLOUT_GUST if gust else 0) | (_native.ROLLOUT_STAGGER if stagger else 0)      # gust: mode_code(...) & MODE_GUST
+               | (_native.ROLLOUT_PER_ACTOR_REFS if per_actor else 0))
     if widths:
         warr = np.asarray(widths, dtype=np.int32)       # host array, alive until the call returns
         d.widths, d.n_widths = warr.ctypes.data, len(widths)

@@ -6,6 +6,15 @@ generation (population rollout, SSNE epoch, exploration episode: Agent.train_hea
 every run's gradient steps on its own cluster (td3_fused.train_group), then every run's tail (validation, actor injection,
 next front: Agent.train_tail).  The runs may differ in seed and in any `Parameters` attribute that keeps the actor's shape.
 
+A SERL10 population (10 actors x 3 envs) fills a few warps for the serial latency of one 2001-step trajectory, so the
+populations fly together too: every run draws its front's references at their usual place (its np.random stream advances
+as it would alone) and leaves the launch to the Sweep, which then makes ONE rollout launch with per-actor env blocks
+(SERL_ROLLOUT_PER_ACTOR_REFS) for each group of runs whose agent.population_key agrees (`launch_groups`), both for the
+fronts the heads take and for the next generation's fronts the tails queue.  Each run reads its slice of the result, bit
+for bit what its own launch gives.  A merged launch has ONE status word: a non-finite trajectory in any run of it raises
+in every run that shares it.  A run whose queued front is invalidated at its next head (its population, RL actor or
+environment changed) flies its population alone.
+
 Each run keeps its own state of the global generators the Agent draws from — stdlib `random` (the SSNE planner), legacy
 `np.random` (reference signals, exploration noise, tournaments) and torch's CPU generator (actor initialisation) — and
 every phase of a run runs with that state swapped in (`RNGState`).  Nothing on the fused path draws from torch's default
@@ -68,6 +77,16 @@ class Run:
         return self.agent.num_frames > self.params.num_frames          # base/train.py's `while num_frames <= frames`
 
 
+def launch_groups(keys):
+    """the runs that share one population launch: lists of run indices with equal agent.population_key, in order of first
+appearance; runs without a population (key None) are in none"""
+    groups = {}
+    for i, k in enumerate(keys):
+        if k is not None:
+            groups.setdefault(k, []).append(i)
+    return list(groups.values())
+
+
 def _shape(p):
     return tuple(getattr(actor_shape(p.hidden_size, p.num_layers, p.activation_actor, p.state_dim, p.action_dim), f)
                  for f in ('state_dim', 'action_dim', 'hidden', 'num_layers', 'activation'))
@@ -98,6 +117,7 @@ class Sweep:
                 np.random.seed(p.seed)
                 random.seed(p.seed)
                 r.agent = agent_mod.Agent(p, env)
+                r.agent.defer_population = True
                 r.rng = RNGState.capture()
                 self.runs.append(r)
         finally:
@@ -113,6 +133,10 @@ class Sweep:
         live = [r for r in self.runs if not r.finished]
         for r in live:
             with rng_scope(r.rng):
+                r.agent.take_front()
+        self._launch_populations([(r, r.agent._front) for r in live])
+        for r in live:
+            with rng_scope(r.rng):
                 r.agent.train_head()
         plans = []
         for r in live:
@@ -126,8 +150,16 @@ class Sweep:
         for r, n in zip(live, plans):
             with rng_scope(r.rng):
                 r.stats = r.agent.train_tail(r.agent.finish_rl_fused(n, losses.get(id(r))))
+        self._launch_populations([(r, r.agent._prefetched) for r in live])
         live_ids = set(id(r) for r in live)
         return [r.stats if id(r) in live_ids else None for r in self.runs]
+
+    def _launch_populations(self, fronts):
+        """one rollout launch per launch group for the fronts [(run, front)] whose population launch is still deferred"""
+        pending = [(r, f) for r, f in fronts if f is not None and f.pop_draws is not None]
+        keys = [agent_mod.population_key(r.params, r.env) for r, _ in pending]
+        for g in launch_groups(keys):
+            agent_mod.launch_population_group([(pending[i][0].agent, pending[i][1]) for i in g])
 
     def evaluate(self, conditions, refs, num_trails=1):
         """evaluation.evaluate_population of every run's population on `conditions` with the references `refs`: all runs
