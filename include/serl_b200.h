@@ -138,6 +138,10 @@ int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shap
  *                step for k = 0, else of step k - 1, sensor noise included), summed in step order in fp64: nMAE
  *                (base/core/utils.py:39-58) without a trace.  Selects kernel instantiations of their own (with the gust
  *                schedule); a launch without it runs the same code as before the field existed
+ *   d_cost       optional [pop, n_envs] int32: per trajectory, the number of its executed steps whose cost flag is set — the flag
+ *                of the replay rows' column 19 (get_cost, envs/phlabenv.py:369-375, with V0 of the env's own plant variant),
+ *                i.e. the safety cost trial_cost = sum info['cost'] of base/core/operator_runner.py:64.  Counted by the
+ *                d_track instantiations, so it needs d_track: SERL_ERR_ARG before any CUDA call without it
  * t_max <= 0 selects the training defaults (20 s, smooth width 3 s). */
 #define SERL_TRACK_COLS 4
 #define SERL_REPLAY_COLS 20
@@ -160,6 +164,7 @@ typedef struct {
     const float* d_sensor_noise;
     int32_t flags;                 /* SERL_ROLLOUT_* */
     double* d_track;
+    int32_t* d_cost;
 } serl_rollout_desc;
 int serl_rollout_run(const serl_rollout_desc* desc, void* stream);
 

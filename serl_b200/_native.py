@@ -53,7 +53,7 @@ class RolloutDesc(ctypes.Structure):
                 ('d_env_order', ctypes.c_void_p), ('d_replay', ctypes.c_void_p), ('replay_env', ctypes.c_int32),
                 ('d_status', ctypes.c_void_p), ('sm_limit', ctypes.c_int32),
                 ('widths', ctypes.c_void_p), ('n_widths', ctypes.c_int32), ('d_sensor_noise', ctypes.c_void_p),
-                ('flags', ctypes.c_int32), ('d_track', ctypes.c_void_p)]
+                ('flags', ctypes.c_int32), ('d_track', ctypes.c_void_p), ('d_cost', ctypes.c_void_p)]
 
 
 class TD3Desc(ctypes.Structure):

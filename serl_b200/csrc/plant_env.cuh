@@ -439,10 +439,13 @@ constexpr int PLANT_TABN2 = (PLANT_TABN + 1) & ~1;
 // Tracking-error accumulators of the evaluation suite (serl_rollout_desc.d_track): the kernels take them as a launch
 // argument of their own, next to the argument block, so that adding them moved no field of the training instantiations.
 //   out  [pop * n_envs][SERL_TRACK_COLS] f64, written at the end of each trajectory
-//   ho   [TRACK_CARRY][Handoff.n] f64: the sums and the carried controlled state of a trajectory K1's time-split schedule
-//        hands to another slot (the rest of its record is Handoff)
-struct TrackArgs { double* out; double* ho; };
-#define TRACK_CARRY (SERL_TRACK_COLS + 3)
+//   ho   [TRACK_CARRY][Handoff.n] f64: the sums, the carried controlled state and the cost tally of a trajectory K1's
+//        time-split schedule hands to another slot (the rest of its record is Handoff)
+//   cost optional [pop * n_envs] int32 (serl_rollout_desc.d_cost): executed steps whose cost flag is set
+struct TrackArgs { double* out; double* ho; int* cost; };
+#define TRACK_COST (SERL_TRACK_COLS + 3)      // Env::trk: steps with the cost flag set so far (an exact integer in f64)
+#define TRACK_V0 (SERL_TRACK_COLS + 4)        // Env::trk: V0 of the env's plant variant, the airspeed bound of get_cost
+#define TRACK_CARRY (SERL_TRACK_COLS + 5)
 
 struct Env {
     double X[NX];
@@ -456,7 +459,7 @@ struct Env {
     bool done;
     int gust;                // env_mode >> 24: 1 = SERL_MODE_GUST, 3 = with SERL_MODE_GUST_UP
     // TRACK instantiations only: sum |e_theta|, sum |e_phi|, sum |e_beta|, sum e_beta, then the controlled state
-    // (theta, phi, beta) of env.x when the next step starts
+    // (theta, phi, beta) of env.x when the next step starts, the cost tally and V0 (TRACK_COST, TRACK_V0)
     double trk[TRACK_CARRY];
 };
 
@@ -531,6 +534,15 @@ __device__ __forceinline__ void track_store(const Env& e, const TrackArgs& tk, s
 {
 #pragma unroll
     for (int c = 0; c < SERL_TRACK_COLS; ++c) tk.out[traj * SERL_TRACK_COLS + c] = e.trk[c];
+    if (tk.cost) tk.cost[traj] = (int)e.trk[TRACK_COST];
+}
+
+// get_cost (phlabenv.py:369-375, including its degrees-vs-radians comparison on the bank angle) of a step's output x, with
+// V0 the airspeed of the plant variant's initial condition
+__device__ __forceinline__ bool step_cost(const double* x, double v0)
+{
+    const double max_phi = 75.0 * DEG2RAD;
+    return (fabs(x[4]) * RAD2DEG > 11.0) || (fabs(x[6]) * RAD2DEG > 0.75 * max_phi) || (x[3] < v0 / 3.0);
 }
 
 // sensor-noise shim (envs/noise/citation.py:72-82, same model in envs/gust): every native step() output gets
@@ -567,6 +579,7 @@ static __device__ __forceinline__ void env_reset(Env& e, const RolloutArgs& a, i
 #pragma unroll
         for (int c = 0; c < SERL_TRACK_COLS; ++c) e.trk[c] = 0.0;
         e.trk[SERL_TRACK_COLS] = x0[7]; e.trk[SERL_TRACK_COLS + 1] = x0[6]; e.trk[SERL_TRACK_COLS + 2] = x0[5];
+        e.trk[TRACK_COST] = 0.0; e.trk[TRACK_V0] = ic[3];
     }
     obs[0] = obs[1] = obs[2] = 0.f;
     obs[3] = (float)x0[0]; obs[4] = (float)x0[1]; obs[5] = (float)x0[2]; obs[6] = (float)x0[4];
@@ -625,6 +638,7 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
         const double et = r_th - e.trk[SERL_TRACK_COLS], ep = r_ph - e.trk[SERL_TRACK_COLS + 1], eb = 0.0 - e.trk[SERL_TRACK_COLS + 2];
         e.trk[0] += fabs(et); e.trk[1] += fabs(ep); e.trk[2] += fabs(eb); e.trk[3] += eb;
         e.trk[SERL_TRACK_COLS] = xo[7]; e.trk[SERL_TRACK_COLS + 1] = xo[6]; e.trk[SERL_TRACK_COLS + 2] = xo[5];
+        if (step_cost(xo, e.trk[TRACK_V0])) e.trk[TRACK_COST] += 1.0;     // the replay row's cost flag, for every env
     }
     const double c0 = fabs(fmin(fmax(k_err * e0, -1.0), 1.0));
     const double c1 = fabs(fmin(fmax(k_err * e1, -1.0), 1.0));
@@ -650,7 +664,8 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
     const float o3 = (float)xo[0], o4 = (float)xo[1], o5 = (float)xo[2], o6 = (float)xo[4];
     if (replay) {
         // the transition Agent.evaluate stores (agent.py:101-112) + the cost flag of get_cost (phlabenv.py:369-375,
-        // including its degrees-vs-radians comparison on the bank angle)
+        // including its degrees-vs-radians comparison on the bank angle).  The same test as step_cost, spelt out: calling
+        // it here changes the code of the instantiations without TRACK
         float* rp = ar.replay + ((size_t)actor * ar.horizon + e.k) * SERL_REPLAY_COLS;
 #pragma unroll
         for (int i = 0; i < 7; ++i) rp[i] = obs[i];

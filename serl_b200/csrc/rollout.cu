@@ -848,7 +848,7 @@ extern "C" int32_t serl_actor_tc_widths(const serl_actor_shape* shape, int32_t* 
 // K1 launch: the checks only this kernel needs, then the genome part of the argument block and the kernel for the hidden size
 static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t s)
 {
-    const TrackArgs tk = {d.d_track, nullptr};
+    const TrackArgs tk = {d.d_track, nullptr, d.d_cost};
     if (!actor_shape_ok(d.shape))
         return serl_fail(SERL_ERR_ARG, "serl_rollout: unsupported actor shape (state_dim = 7, action_dim = 3, 2 <= hidden <= 256)");
     if (d.pop > 65535) return serl_fail(SERL_ERR_ARG, "serl_rollout: pop must be <= 65535 per call");       // grid.y of the simple kernel
@@ -896,6 +896,8 @@ static int check_desc(const serl_rollout_desc& d)
     if (d.d_replay && (d.replay_env < 0 || d.replay_env >= d.n_envs)) return serl_fail(SERL_ERR_ARG, "serl_rollout: replay_env out of range");
     if (d.t_max > 0.0 && !(d.smooth_width > 0.0)) return serl_fail(SERL_ERR_ARG, "serl_rollout: smooth_width must be > 0");
     if (d.n_widths > 0 && !d.widths) return serl_fail(SERL_ERR_ARG, "serl_rollout: n_widths > 0 but widths is null");
+    // the tally is counted by the tracking instantiations only
+    if (d.d_cost && !d.d_track) return serl_fail(SERL_ERR_ARG, "serl_rollout: d_cost needs d_track");
     if (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) {
         // inside one actor's block the lanes of a warp already share a mode: no lane permutation
         if (d.d_env_order) return serl_fail(SERL_ERR_ARG, "serl_rollout: SERL_ROLLOUT_PER_ACTOR_REFS does not take d_env_order");

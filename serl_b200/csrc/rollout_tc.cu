@@ -790,7 +790,7 @@ int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, cudaStream
          {rollout_kernel_tc<SERL_ACT_ELU, true, false, false, true>, rollout_kernel_tc<SERL_ACT_ELU, true, true, false, true>}},
         {{rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, true>},
          {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, false, false, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, true, false, true>}}};
-    const TrackArgs tk = {d.d_track, nullptr};
+    const TrackArgs tk = {d.d_track, nullptr, d.d_cost};
     const bool gust = (d.flags & SERL_ROLLOUT_GUST) != 0, deep = ar.n_layers > 1;
     // one CTA = the two groups of TC_THREADS threads
     return serl_launch("rollout_kernel_tc launch", d.d_track ? track_kernels[d.shape.activation][deep]

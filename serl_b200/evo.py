@@ -112,31 +112,39 @@ def plan_epoch(index_rank, offsprings_raw, table, population_size, num_elitists,
                         for w in _waves(pairs, lambda p: (p[2], p[3]), lambda p: (p[0], p[1]))]
     # :537-539 mutation of every non-elite rank (mutate_inplace :329-369)
     seg, m_off, m_kind, m_z = [], [], [], []
-    gauss = random.gauss
     for i in (index_rank[num_elitists:] if mutation_prob >= 0 else []):
         if rnd() < mutation_prob:
-            ssne_probabilities = np.random.uniform(0, 1, len(table)) * 2
-            for k, (off, rows, cols) in enumerate(table):
-                if cols == 0:
-                    continue
-                if rnd() < ssne_probabilities[k]:
-                    n = rint(0, int(math.ceil(0.1 * rows * cols)))
-                    begin = len(m_off)
-                    for _ in range(n):
-                        e = off + rrange(rows) * cols + rrange(cols)
-                        r = rnd()
-                        m_off.append(e)
-                        m_kind.append(1 if r < 0.05 else (2 if r < 0.1 else 0))
-                        m_z.append(gauss(0, 1))
-                    if n:
-                        seg.append((i, begin, n))
-    plan.mut_seg = np.asarray(seg, dtype=np.int32).reshape(-1, 3)
-    plan.mut_off = np.asarray(m_off, dtype=np.int32)
-    plan.mut_kind = np.asarray(m_kind, dtype=np.int32)
-    plan.mut_z = np.asarray(m_z, dtype=np.float64).astype(np.float32)       # fl32(z): torch casts the python scalar first
+            plan_mutate_inplace(table, i, np.random.uniform(0, 1, len(table)) * 2, seg, m_off, m_kind, m_z)
+    plan.mut_seg, plan.mut_off, plan.mut_kind, plan.mut_z = mutation_arrays(seg, m_off, m_kind, m_z)
     plan.elite = new_elitists[0]
     plan.new_elitists, plan.offsprings, plan.unselects = new_elitists, offsprings, unselects
     return plan
+
+
+def plan_mutate_inplace(table, actor, ssne_probabilities, seg, m_off, m_kind, m_z):
+    """the stdlib `random` draws of one mutate_inplace (:329-369) of genome row `actor`, given its
+    ssne_probabilities = np.random.uniform(0, 1, len(table)) * 2: appends K5's ops to the four lists."""
+    rnd, rrange, rint, gauss = random.random, random.randrange, random.randint, random.gauss
+    for k, (off, rows, cols) in enumerate(table):
+        if cols == 0:
+            continue
+        if rnd() < ssne_probabilities[k]:
+            n = rint(0, int(math.ceil(0.1 * rows * cols)))
+            begin = len(m_off)
+            for _ in range(n):
+                e = off + rrange(rows) * cols + rrange(cols)
+                r = rnd()
+                m_off.append(e)
+                m_kind.append(1 if r < 0.05 else (2 if r < 0.1 else 0))
+                m_z.append(gauss(0, 1))
+            if n:
+                seg.append((actor, begin, n))
+
+
+def mutation_arrays(seg, m_off, m_kind, m_z):
+    """K5's op arrays (mut_seg, mut_off, mut_kind, mut_z) from the lists plan_mutate_inplace fills"""
+    return (np.asarray(seg, dtype=np.int32).reshape(-1, 3), np.asarray(m_off, dtype=np.int32), np.asarray(m_kind, dtype=np.int32),
+            np.asarray(m_z, dtype=np.float64).astype(np.float32))       # fl32(z): torch casts the python scalar first
 
 
 def _plan_tail_native(plan, table, mut_order, mutation_prob):

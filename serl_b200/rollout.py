@@ -57,7 +57,7 @@ def num_params(shape):
 
 
 class RolloutResult:
-    __slots__ = ('returns', 'steps', 'fitness', 'trace', 'actions', 'smoothness', 'replay', 'status', 'track')
+    __slots__ = ('returns', 'steps', 'fitness', 'trace', 'actions', 'smoothness', 'replay', 'status', 'track', 'cost')
 
     trace_x = property(lambda s: s.trace[..., TRACE_X])
     trace_u = property(lambda s: s.trace[..., TRACE_U])
@@ -82,7 +82,7 @@ def variant_sorted_order(env_mode):
 
 def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon=HORIZON, trace=False, out=None, action_noise=None,
                        actions=False, t_max=None, smooth_width=None, env_order=None, replay_env=None, status=True, sm_limit=0,
-                       fitness=True, widths=None, sensor_noise=None, gust=False, stagger=False, track=False):
+                       fitness=True, widths=None, sensor_noise=None, gust=False, stagger=False, track=False, cost=False):
     """weights [pop,P] fp32 cuda; ref_levels/ref_starts [n_envs,2,6] f64 cuda; env_mode [n_envs] int32 cuda.
     Per-actor env blocks: ref_levels/ref_starts [pop,n_envs,2,6] and env_mode [pop,n_envs] give every actor its own n_envs
     envs (SERL_ROLLOUT_PER_ACTOR_REFS; the shapes select the layout; not with env_order or track).
@@ -93,6 +93,8 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     slower on an H100; to time the two schedules against each other).
     track=True: result.track [pop, n_envs, TRACK_COLS] f64 holds each trajectory's tracking-error sums
     (sum |e_theta|, sum |e_phi|, sum |e_beta|, sum e_beta; serl_rollout_desc.d_track), the nMAE of a trajectory without a trace.
+    cost=True (with track=True): result.cost [pop, n_envs] int32 holds each trajectory's safety cost, the number of its executed
+    steps whose cost flag (the replay rows' last column) is set (serl_rollout_desc.d_cost).
     widths=[w0, w1, ..., w_{n-1}] (2 to 9 widths): width-list actors on the tensor-core kernel K1-TC (csrc/rollout_tc.cu); `shape`
     then only supplies the activation.  widths=None flies the uniform actor `shape` on K1, or on K1-TC with [h] * (L + 1) when its
     genome does not fit K1's kernels (tc_widths)."""
@@ -125,6 +127,7 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
         r.replay = torch.empty((pop, horizon, REPLAY_COLS), dtype=torch.float32, device=dev) if replay_env is not None else None
         r.status = torch.zeros((1,), dtype=torch.int32, device=dev) if status else None
         r.track = torch.empty((pop, n_envs, TRACK_COLS), dtype=torch.float64, device=dev) if track else None
+        r.cost = torch.empty((pop, n_envs), dtype=torch.int32, device=dev) if cost else None
         if trace:
             r.trace = torch.full((pop, n_envs, horizon, TRACE_COLS), float('nan'), dtype=torch.float64, device=dev)
     elif r.status is not None:
@@ -142,6 +145,7 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     d.d_replay, d.replay_env = p(getattr(r, 'replay', None)), int(replay_env if replay_env is not None else 0)
     d.d_status = p(getattr(r, 'status', None))
     d.d_track = p(getattr(r, 'track', None))
+    d.d_cost = p(getattr(r, 'cost', None))
     if sm_limit < 0:         # leave -sm_limit SMs to concurrent small launches
         sm_limit = max(1, torch.cuda.get_device_properties(dev).multi_processor_count + int(sm_limit))
     d.sm_limit = int(sm_limit)
