@@ -181,7 +181,8 @@ int serl_actor_forward_wide(const float* d_genome, const int32_t* widths, int32_
 
 /* K6: action smoothness of n_traj trajectories (base/core/utils.py:82-120 calc_smoothness; agent.py:128-134):
  * out[t] = -sqrt(sum_i sum_k f_k |FFT(y_i)[k]|^2 dt 2/N) * 100 * 80/(N dt) over the N = d_steps[t] executed steps of
- * d_actions [n_traj, horizon, 3]. */
+ * d_actions [n_traj, horizon, 3].  horizon <= 2048: a Bluestein FFT; 2049 .. 10240: a direct DFT; longer:
+ * SERL_ERR_UNSUPPORTED.  Both remove each channel's mean (bin 0 is not part of the metric) before their fp32 transform. */
 int serl_smoothness(const float* d_actions, const int32_t* d_steps, int32_t n_traj, int32_t horizon, double dt,
                     double* d_out, void* stream);
 

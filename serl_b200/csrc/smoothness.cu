@@ -10,26 +10,39 @@
 // One CTA per trajectory: direct DFT of the three actuator signals over the executed steps N (N = 2001 is 3*23*29,
 // no radix-2 structure; 12 M fp32 MACs per trajectory), frequency-weighted power summed in double:
 //   S = sum_i sum_{k=1}^{N/2-1} f_k |Y_i[k]|^2 dt * 2/N,  f = linspace(dt, 1/(2dt), N/2-1),  result = -sqrt(S)*100*(80/(N dt)).
+// The channel means are removed first, as in smoothness_fft_kernel: bin 0 is not part of the metric, and a trimmed
+// deflection (a large constant under a small ripple) would otherwise leak through the fp32 twiddles into every bin.
 __global__ void __launch_bounds__(256)
 smoothness_kernel(const float* __restrict__ actions, const int* __restrict__ steps, int horizon, double dt, double* __restrict__ out)
 {
-    // one symbol in the three K6 kernels; 128-byte aligned, smoothness_fft_kernel's work arrays start at 2176 after its
-    // static red / mean_s (with 16: at 2064, and the kernel measured 2 % slower on an H100)
+    // one symbol in the three K6 kernels; 128-byte aligned, the work arrays start at 2176 after the static red / mean_s
+    // (with 16: at 2064, and smoothness_fft_kernel measured 2 % slower on an H100)
     extern __shared__ __align__(128) unsigned char sm_raw[];
-    const int traj = blockIdx.x;
+    __shared__ double red[256];
+    __shared__ float mean_s[3];
+    const int traj = blockIdx.x, tid = threadIdx.x;
     const int N = steps[traj];
     const int M = N / 2 - 1;
-    if (M <= 0) { if (threadIdx.x == 0) out[traj] = -0.0; return; }
+    if (M <= 0) { if (tid == 0) out[traj] = -0.0; return; }
     float2* tw = reinterpret_cast<float2*>(sm_raw);            // [N] (cos, sin)(2 pi j / N)
     float* y0 = reinterpret_cast<float*>(tw + horizon);       // [3][N]
     float* y1 = y0 + horizon;
     float* y2 = y1 + horizon;
     const float* a = actions + (size_t)traj * horizon * 3;
-    for (int n = threadIdx.x; n < N; n += blockDim.x) {
+    double s0 = 0.0, s1 = 0.0, s2 = 0.0;
+    for (int n = tid; n < N; n += 256) { s0 += a[3 * n]; s1 += a[3 * n + 1]; s2 += a[3 * n + 2]; }
+    for (int c = 0; c < 3; ++c) {
+        red[tid] = c == 0 ? s0 : (c == 1 ? s1 : s2);
+        __syncthreads();
+        for (int s = 128; s > 0; s >>= 1) { if (tid < s) red[tid] += red[tid + s]; __syncthreads(); }
+        if (tid == 0) mean_s[c] = (float)(red[0] / (double)N);
+        __syncthreads();
+    }
+    for (int n = tid; n < N; n += 256) {
         float sv, cv;
         sincospif(2.0f * (float)n / (float)N, &sv, &cv);
         tw[n] = make_float2(cv, sv);
-        y0[n] = a[3 * n]; y1[n] = a[3 * n + 1]; y2[n] = a[3 * n + 2];
+        y0[n] = a[3 * n] - mean_s[0]; y1[n] = a[3 * n + 1] - mean_s[1]; y2[n] = a[3 * n + 2] - mean_s[2];
     }
     __syncthreads();
     const double fstep = M > 1 ? (1.0 / (2.0 * dt) - dt) / (double)(M - 1) : 0.0;
@@ -66,14 +79,13 @@ smoothness_kernel(const float* __restrict__ actions, const int* __restrict__ ste
             acc += (dt + (double)(kk[q] - 1) * fstep) * p;
         }
     }
-    __shared__ double red[256];
-    red[threadIdx.x] = acc;
+    red[tid] = acc;
     __syncthreads();
     for (int s = 128; s > 0; s >>= 1) {
-        if (threadIdx.x < s) red[threadIdx.x] += red[threadIdx.x + s];
+        if (tid < s) red[tid] += red[tid + s];
         __syncthreads();
     }
-    if (threadIdx.x == 0) {
+    if (tid == 0) {
         const double S = red[0] * dt * 2.0 / (double)N;
         out[traj] = -(sqrt(S) * 100.0 * (80.0 / ((double)N * dt)));
     }
