@@ -13,7 +13,7 @@
 //
 // Two actor implementations:
 //   rollout_kernel_persist<H, TABS, GUST>  persistent grid, one CTA per SM.  The MLP is a register-tiled GEMM inside a warp
-//                           (lane = 1/4 of the output neurons x 4 envs, float2 pairs, activations exchanged through a
+//                           (lane = 1/8 of the output neurons x 8 envs, float2 pairs, activations exchanged through a
 //                           per-warp shared-memory buffer, weights broadcast from shared memory; h in {32,64,72,96,128}).  The CTA's warps take
 //                           their steps in lockstep (one barrier per step: shared instruction fetch), genomes arrive by bulk
 //                           TMA copies.
@@ -86,94 +86,171 @@ __device__ void actor_forward_simple(const float* __restrict__ w, const serl_act
 }
 
 // ---- warp-autonomous actor + env ---------------------------------------------------------------------------
-// smem: plant tables [PT_TOTAL] f64 | per actor of the CTA: transposed weights
+// smem: plant tables [PT_TOTAL] f64 | per actor of the CTA: transposed weights in row-pair blocks (pair_layout_index)
 //       Wt0[S][H] b0[H] | L x { Wt[H][H] b[H] gamma[H] beta[H] } | Wo[A][H] bo[A]
-// lane = (g = lane>>2, og = lane&3): output neurons og*TM .. og*TM+TM-1 of the envs 4g .. 4g+3 of this warp.
-// The activation of neuron k for env 4g+c lives in lane (g, og = k/TM), register in[k%TM][c].  The next layer reads
-// it from the warp's exchange buffer xb in shared memory, one source quarter at a time: before quarter so the og == so
-// lanes store their in[][] as xb[m][g][c] (one STS.128 per neuron), so that one LDS.128 per source neuron gives a
-// lane the four envs of its group and the loop over source neurons is a rolled loop with a small body (unrolled, the
-// register selection and shuffles of every neuron made the actor too large for the instruction cache next to the
-// plant).  Reductions over neurons are xor-butterflies over the two og bits, so the four lanes of a group hold
-// bit-identical means / deviations.
-// All MLP arithmetic is written on float2 pairs (am_fma2: two independent IEEE-rn fmas); a float2
-// register pair holds two consecutive output neurons (m, m+1) of one env, exactly what one LDS.64 of the transposed
-// weight row delivers, and the activation of the source neuron is broadcast into both halves.
+// lane = (g = lane>>3, og = lane&7): output neurons og*T8 .. og*T8+T8-1 (T8 = h/8) of the envs 8g .. 8g+7 of this warp.
+// The activation of neuron k for env 8g+c lives in lane (g, og = k/T8), register in[k%T8][c/2] (.x / .y).  The next
+// layer reads it from the warp's exchange buffer xb in shared memory, one source quarter (lanes og = 2q, 2q+1) at a
+// time: before quarter so its lanes store their in[][] as xb[row][8g + c] (two STS.128 per neuron), so that two LDS.128
+// per source neuron give a lane the eight envs of its group and the loop over source neurons is a rolled loop with a
+// small body (unrolled, the register selection and shuffles of every neuron made the actor too large for the
+// instruction cache next to the plant).  A weight load serves 8 envs: per pair of source rows a lane takes its 2·T8
+// weights with T8/2 LDS.128 (+ one LDS.64 when T8 is odd) and the 16 inputs with 4 LDS.128, for 16·T8 multiply-adds.
+// A quarter's sums (LayerNorm, output layer) run sequentially over its first eighth in lane og = 2q, are handed to
+// lane 2q+1 with one shuffle and continue there: the order of the kernel-order oracle's quarter blocks
+// (oracle/plant/actor_kernel_order.c).  The quarters are then combined (q0+q1)+(q2+q3) by a butterfly that also
+// transposes: each odd lane ends with the totals of two envs, takes their per-env divisions / square root, and every
+// lane of the group reads the results back by shuffles, so all eight lanes of a group hold bit-identical means /
+// deviations.  Element-wise arithmetic is written on float2 pairs of two envs of one neuron (am_fma2: two independent
+// IEEE-rn fmas), and an activation call takes the group's eight envs of one neuron.
 __host__ __device__ constexpr int actor_xbuf_floats(int H) { return H / 4 * 32; }    // exchange buffer per warp: a quarter x 32 envs
 
-// one source row: its activation for the group's four envs and the lane's h/4 weights
+// Offset of element (source row k, output neuron n) of a transposed [R][H] matrix in the kernel layout: rows in pairs, a
+// pair a block of 2H floats in which lane og's 2·T8 weights (row k's T8, then row k+1's) are its N4 float4 (at
+// 16-byte chunk i: all eight lanes' chunk i side by side, so that an LDS.128 of the warp touches 128 contiguous bytes)
+// and, for odd T8, one float2 after the chunks.  An odd last row (the observation layer: R = 7) is a plain row.
+__host__ __device__ constexpr int pair_layout_index(int k, int n, int R, int H)
+{
+    const int T8 = H / 8, N4 = T8 / 2 * 4;                 // floats of a lane's pair weights in float4 chunks
+    if (k >= (R & ~1)) return (R & ~1) * H + n;
+    const int og = n / T8, j = (k & 1) * T8 + n % T8;
+    const int base = (k >> 1) * 2 * H;
+    return j < N4 ? base + (j / 4) * 32 + og * 4 + j % 4 : base + N4 * 8 + og * 2 + (j - N4);
+}
+
+// one pair of source rows: their activations for the group's eight envs and the lane's 2·T8 weights
 template <int H>
-struct WarpRow {
-    float4 x;
-    float2 w[H / 8];
-    __device__ __forceinline__ void load(const float* __restrict__ wrow, const float* xg, int k)
+struct WarpPair {
+    static constexpr int T8 = H / 8, N4 = T8 / 2;
+    float4 x[4];                                       // row k: envs 0-3, 4-7; row k + 1: envs 0-3, 4-7
+    float4 w4[N4];
+    float2 w2;                                         // odd T8 only
+    // wl = matrix + og * 4, wt = matrix + N4 * 32 + og * 2 (pair_layout_index)
+    __device__ __forceinline__ void load(const float* __restrict__ wl, const float* __restrict__ wt, const float* xg, int p)
     {
-        x = *reinterpret_cast<const float4*>(xg + k * 32);
-        const float2* wp = reinterpret_cast<const float2*>(wrow + k * H);
 #pragma unroll
-        for (int m2 = 0; m2 < H / 8; ++m2) w[m2] = wp[m2];
+        for (int i = 0; i < 4; ++i) x[i] = *reinterpret_cast<const float4*>(xg + (2 * p + (i >> 1)) * 32 + (i & 1) * 4);
+#pragma unroll
+        for (int i = 0; i < N4; ++i) w4[i] = *reinterpret_cast<const float4*>(wl + p * 2 * H + i * 32);
+        if (T8 & 1) w2 = *reinterpret_cast<const float2*>(wt + p * 2 * H);
     }
-    __device__ __forceinline__ void fma(float2 (&acc)[H / 8][4]) const
+    __device__ __forceinline__ float w(int j) const
+    {
+        if (j >= 4 * N4) return j == 4 * N4 ? w2.x : w2.y;
+        const float4 v = w4[j / 4];
+        return j % 4 == 0 ? v.x : j % 4 == 1 ? v.y : j % 4 == 2 ? v.z : v.w;
+    }
+    __device__ __forceinline__ void fma(float2 (&acc)[T8][4]) const
     {
 #pragma unroll
-        for (int m2 = 0; m2 < H / 8; ++m2) {
-            acc[m2][0] = am_fma2(w[m2], am_splat(x.x), acc[m2][0]);
-            acc[m2][1] = am_fma2(w[m2], am_splat(x.y), acc[m2][1]);
-            acc[m2][2] = am_fma2(w[m2], am_splat(x.z), acc[m2][2]);
-            acc[m2][3] = am_fma2(w[m2], am_splat(x.w), acc[m2][3]);
-        }
+        for (int r = 0; r < 2; ++r)
+#pragma unroll
+            for (int m = 0; m < T8; ++m) {
+                const float2 wv = am_splat(w(r * T8 + m));
+                const float4 a = x[2 * r], b = x[2 * r + 1];
+                acc[m][0] = am_fma2(wv, make_float2(a.x, a.y), acc[m][0]);
+                acc[m][1] = am_fma2(wv, make_float2(a.z, a.w), acc[m][1]);
+                acc[m][2] = am_fma2(wv, make_float2(b.x, b.y), acc[m][2]);
+                acc[m][3] = am_fma2(wv, make_float2(b.z, b.w), acc[m][3]);
+            }
     }
 };
 
-// acc[m2][c] += sum over source rows k < nk (in order from 0) of wrow[k*H + 2*m2 (+1)] * xg[k*32 + c].
-// Two rows per trip, each row's loads issued before the multiply-adds of the row ahead of it: the shared-memory latency
-// is hidden without unrolling the loop.
+// acc[m][c] += sum over source rows k < nk (in order from 0) of W[k][og*T8 + m] * xg[k*32 + c] for the matrix at `wm`
+// (pair_layout_index).  Two row pairs per trip, each pair's loads issued before the multiply-adds of the pair ahead of
+// it: the shared-memory latency is hidden without unrolling the loop.
 template <int H>
-__device__ __forceinline__ void warp_rows(const float* __restrict__ wrow, int nk, const float* xg, float2 (&acc)[H / 8][4])
+__device__ __forceinline__ void warp_rows(const float* __restrict__ wm, int nk, const float* xg, int og, float2 (&acc)[H / 8][4])
 {
-    WarpRow<H> ra, rb;
-    ra.load(wrow, xg, 0);
-    int k = 0;
+    using P = WarpPair<H>;
+    const float* wl = wm + og * 4;
+    const float* wt = wm + P::N4 * 32 + og * 2;
+    const int np = nk >> 1;
+    P ra, rb;
+    ra.load(wl, wt, xg, 0);
+    int p = 0;
 #pragma unroll 1
-    for (; k + 2 <= nk; k += 2) {
-        rb.load(wrow, xg, k + 1);
+    for (; p + 2 <= np; p += 2) {
+        rb.load(wl, wt, xg, p + 1);
         ra.fma(acc);
-        ra.load(wrow, xg, k + 2 < nk ? k + 2 : k + 1);      // (the last trip re-reads row k + 1: stays in bounds)
+        ra.load(wl, wt, xg, p + 2 < np ? p + 2 : p + 1);      // (the last trip re-reads pair p + 1: stays in bounds)
         rb.fma(acc);
     }
-    if (k < nk) ra.fma(acc);
+    if (p < np) ra.fma(acc);
+    if (nk & 1) {                                      // a plain last row
+        const int k = nk - 1;
+        const float4 a = *reinterpret_cast<const float4*>(xg + k * 32), b = *reinterpret_cast<const float4*>(xg + k * 32 + 4);
+#pragma unroll
+        for (int m = 0; m < P::T8; ++m) {
+            const float2 wv = am_splat(wm[k * H + og * P::T8 + m]);
+            acc[m][0] = am_fma2(wv, make_float2(a.x, a.y), acc[m][0]);
+            acc[m][1] = am_fma2(wv, make_float2(a.z, a.w), acc[m][1]);
+            acc[m][2] = am_fma2(wv, make_float2(b.x, b.y), acc[m][2]);
+            acc[m][3] = am_fma2(wv, make_float2(b.z, b.w), acc[m][3]);
+        }
+    }
 }
 
 template <int H>
 __device__ __forceinline__ void warp_layer(const float* __restrict__ Wt, const float2 (&in)[H / 8][4], float2 (&acc)[H / 8][4],
                                            int og, int g, float* xb)
 {
-    constexpr int TM = H / 4, TM2 = H / 8;
+    constexpr int TM = H / 4, T8 = H / 8;
 #pragma unroll
-    for (int m = 0; m < TM2; ++m)
+    for (int m = 0; m < T8; ++m)
 #pragma unroll
         for (int c = 0; c < 4; ++c) acc[m][c] = make_float2(0.f, 0.f);
+    float* xs = xb + (og & 1) * T8 * 32 + g * 8;       // this lane's rows of its quarter
 #pragma unroll 1
     for (int so = 0; so < 4; ++so) {
         __syncwarp();                                  // the previous quarter has been read
-        if (og == so) {
+        if ((og >> 1) == so) {
 #pragma unroll
-            for (int m2 = 0; m2 < TM2; ++m2) {
-                *reinterpret_cast<float4*>(xb + (2 * m2) * 32 + g * 4) = make_float4(in[m2][0].x, in[m2][1].x, in[m2][2].x, in[m2][3].x);
-                *reinterpret_cast<float4*>(xb + (2 * m2 + 1) * 32 + g * 4) = make_float4(in[m2][0].y, in[m2][1].y, in[m2][2].y, in[m2][3].y);
+            for (int m = 0; m < T8; ++m) {
+                *reinterpret_cast<float4*>(xs + m * 32) = make_float4(in[m][0].x, in[m][0].y, in[m][1].x, in[m][1].y);
+                *reinterpret_cast<float4*>(xs + m * 32 + 4) = make_float4(in[m][2].x, in[m][2].y, in[m][3].x, in[m][3].y);
             }
         }
         __syncwarp();
-        warp_rows<H>(Wt + (size_t)(so * TM) * H + og * TM, TM, xb + g * 4, acc);
+        warp_rows<H>(Wt + (size_t)(so * TM) * H, TM, xb + g * 8, og, acc);
     }
 }
 
-__device__ __forceinline__ float group_sum(float v)
+__device__ __forceinline__ float env_of(const float2 (&v)[4], int c) { return c & 1 ? v[c >> 1].y : v[c >> 1].x; }
+
+// Sum over the group's quarter blocks for each of its eight envs.  f(m, c, s) adds the lane's neuron m of env c to s;
+// the quarter's first eighth (lane og = 2q) is summed from 0 and continued in lane 2q + 1.  The quarters are combined
+// (q0+q1)+(q2+q3) (fadd is commutative, so both lanes of a butterfly pair get the same bits) while each round halves the
+// envs a lane keeps: odd lane og ends with the totals of envs 4·og[1] + 2·og[2] + i, i = 0, 1, in tot[i]
+// (quarter_src_lane).  The other lanes' tot is meaningless.
+template <int T8, typename F>
+__device__ __forceinline__ void quarter_totals(F f, int og, float (&tot)[2])
 {
-    v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 1));
-    v = __fadd_rn(v, __shfl_xor_sync(0xffffffffu, v, 2));
-    return v;
+    float s[8];
+#pragma unroll
+    for (int c = 0; c < 8; ++c) s[c] = 0.f;
+#pragma unroll 1
+    for (int pass = 0; pass < 2; ++pass) {             // rolled: the sums are written once in the code
+        if (pass)
+#pragma unroll
+            for (int c = 0; c < 8; ++c) s[c] = __shfl_xor_sync(0xffffffffu, s[c], 1);
+#pragma unroll
+        for (int m = 0; m < T8; ++m)
+#pragma unroll
+            for (int c = 0; c < 8; ++c) s[c] = f(m, c, s[c]);
+    }
+    const bool hi1 = (og & 2) != 0, hi2 = (og & 4) != 0;
+    float r[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+        r[i] = __fadd_rn(hi1 ? s[4 + i] : s[i], __shfl_xor_sync(0xffffffffu, hi1 ? s[i] : s[4 + i], 2));
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+        tot[i] = __fadd_rn(hi2 ? r[2 + i] : r[i], __shfl_xor_sync(0xffffffffu, hi2 ? r[i] : r[2 + i], 4));
 }
+
+// the lane of group g whose tot[c & 1] holds env c's total
+__device__ __forceinline__ int quarter_src_lane(int g, int c) { return g * 8 + 1 + ((c >> 2) & 1) * 2 + ((c >> 1) & 1) * 4; }
 
 // observation in, action out: by value (registers) rather than through pointers, which put them in local memory
 struct ActorObs { float v[7]; };
@@ -183,35 +260,35 @@ struct ActorAct { float v[3]; };
 template <int H, int ACT>
 __device__ __noinline__ ActorAct actor_forward_warp(const float* __restrict__ w, int L, int lane, float* xb, ActorObs obs)
 {
-    constexpr int TM = H / 4, TM2 = H / 8;
+    constexpr int TM = H / 4, T8 = H / 8;
     constexpr int S = 7, A = 3;
     static_assert(TM >= S, "the observation rows fit the exchange buffer");
-    const int og = lane & 3, g = lane >> 2;
+    const int og = lane & 7, g = lane >> 3, n0 = og * T8;
     const float* Wt0 = w;
     const float* b0 = Wt0 + S * H;
     const float* hid = b0 + H;
     const float* Wo = hid + (size_t)L * (H * H + 3 * H);
     const float* bo = Wo + A * H;
-    float2 in[TM2][4], acc[TM2][4];
-    // input layer: the observation of env lane = 4g+c goes to xb[k][g][c]
+    float2 in[T8][4], acc[T8][4];
+    // input layer: the observation of env lane = 8g+c goes to xb[k][8g + c]
 #pragma unroll
-    for (int m = 0; m < TM2; ++m)
+    for (int m = 0; m < T8; ++m)
 #pragma unroll
         for (int c = 0; c < 4; ++c) acc[m][c] = make_float2(0.f, 0.f);
     __syncwarp();                                      // the previous call has read the buffer
 #pragma unroll
     for (int k = 0; k < S; ++k) xb[k * 32 + lane] = obs.v[k];
     __syncwarp();
-    warp_rows<H>(Wt0 + og * TM, S, xb + g * 4, acc);
+    warp_rows<H>(Wt0, S, xb + g * 8, og, acc);
 #pragma unroll
-    for (int m2 = 0; m2 < TM2; ++m2) {
-        const float2 b = *reinterpret_cast<const float2*>(b0 + og * TM + 2 * m2);
+    for (int m = 0; m < T8; ++m) {
+        const float2 b = am_splat(b0[n0 + m]);
         AmF2x4 v;
 #pragma unroll
-        for (int c = 0; c < 4; ++c) v.v[c] = am_fma2(acc[m2][c], am_splat(1.0f), b);
+        for (int c = 0; c < 4; ++c) v.v[c] = am_fma2(acc[m][c], am_splat(1.0f), b);
         v = am_act2x4<ACT>(v);
 #pragma unroll
-        for (int c = 0; c < 4; ++c) in[m2][c] = v.v[c];
+        for (int c = 0; c < 4; ++c) in[m][c] = v.v[c];
     }
     // hidden layers: Linear -> LayerNorm (unbiased std, eps on std; mod_utils.py:47-50) -> activation
 #pragma unroll 1
@@ -221,62 +298,53 @@ __device__ __noinline__ ActorAct actor_forward_warp(const float* __restrict__ w,
         const float* gamma = bb + H;
         const float* beta = gamma + H;
         warp_layer<H>(Wt, in, acc, og, g, xb);
-        float s[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll
-        for (int m2 = 0; m2 < TM2; ++m2) {
-            const float2 b = *reinterpret_cast<const float2*>(bb + og * TM + 2 * m2);
+        for (int m = 0; m < T8; ++m) {
+            const float2 b = am_splat(bb[n0 + m]);
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                acc[m2][c] = am_fma2(acc[m2][c], am_splat(1.0f), b);
-                s[c] = __fadd_rn(s[c], acc[m2][c].x);
-                s[c] = __fadd_rn(s[c], acc[m2][c].y);
-            }
+            for (int c = 0; c < 4; ++c) acc[m][c] = am_fma2(acc[m][c], am_splat(1.0f), b);
         }
-        float mean[4], den[4];
+        float t[2], mean[8], den[8];
+        quarter_totals<T8>([&](int m, int c, float s) { return __fadd_rn(s, env_of(acc[m], c)); }, og, t);
 #pragma unroll
-        for (int c = 0; c < 4; ++c) mean[c] = __fdiv_rn(group_sum(s[c]), (float)H);
-        float q[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int i = 0; i < 2; ++i) t[i] = __fdiv_rn(t[i], (float)H);
 #pragma unroll
-        for (int m2 = 0; m2 < TM2; ++m2)
+        for (int c = 0; c < 8; ++c) mean[c] = __shfl_sync(0xffffffffu, t[c & 1], quarter_src_lane(g, c));
 #pragma unroll
-            for (int c = 0; c < 4; ++c) {
-                acc[m2][c] = am_fma2(acc[m2][c], am_splat(1.0f), am_splat(-mean[c]));
-                q[c] = __fmaf_rn(acc[m2][c].x, acc[m2][c].x, q[c]);
-                q[c] = __fmaf_rn(acc[m2][c].y, acc[m2][c].y, q[c]);
-            }
+        for (int m = 0; m < T8; ++m)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) acc[m][c] = am_fma2(acc[m][c], am_splat(1.0f), make_float2(-mean[2 * c], -mean[2 * c + 1]));
+        quarter_totals<T8>([&](int m, int c, float s) { const float d = env_of(acc[m], c); return __fmaf_rn(d, d, s); }, og, t);
         // gamma * (x - mean) / (std + eps) + beta as fma(gamma * d, 1 / (std + eps), beta): one reciprocal per env instead
-        // of H/4 divisions per lane (<= 1 ulp from the reference's expression, the order of its summation-order freedom)
+        // of h divisions (<= 1 ulp from the reference's expression, the order of its summation-order freedom)
 #pragma unroll
-        for (int c = 0; c < 4; ++c)
-            den[c] = __fdiv_rn(1.0f, __fadd_rn(__fsqrt_rn(__fdiv_rn(group_sum(q[c]), (float)(H - 1))), 1e-6f));
+        for (int i = 0; i < 2; ++i) t[i] = __fdiv_rn(1.0f, __fadd_rn(__fsqrt_rn(__fdiv_rn(t[i], (float)(H - 1))), 1e-6f));
 #pragma unroll
-        for (int m2 = 0; m2 < TM2; ++m2) {
-            const float2 g = *reinterpret_cast<const float2*>(gamma + og * TM + 2 * m2);
-            const float2 be = *reinterpret_cast<const float2*>(beta + og * TM + 2 * m2);
+        for (int c = 0; c < 8; ++c) den[c] = __shfl_sync(0xffffffffu, t[c & 1], quarter_src_lane(g, c));
+#pragma unroll
+        for (int m = 0; m < T8; ++m) {
+            const float2 gm = am_splat(gamma[n0 + m]), be = am_splat(beta[n0 + m]);
             AmF2x4 v;
 #pragma unroll
-            for (int c = 0; c < 4; ++c) v.v[c] = am_fma2(am_fma2(g, acc[m2][c], am_splat(-0.0f)), am_splat(den[c]), be);
+            for (int c = 0; c < 4; ++c)
+                v.v[c] = am_fma2(am_fma2(gm, acc[m][c], am_splat(-0.0f)), make_float2(den[2 * c], den[2 * c + 1]), be);
             v = am_act2x4<ACT>(v);
 #pragma unroll
-            for (int c = 0; c < 4; ++c) in[m2][c] = v.v[c];
+            for (int c = 0; c < 4; ++c) in[m][c] = v.v[c];
         }
     }
-    // output layer: partial dot products over this lane's neurons, reduced over the group; lane og keeps env 4g+og.
+    // output layer: quarter-block dot products over the group, combined like the LayerNorm sums; lane og keeps env 8g+og.
     // The three tanh go through two pair calls.
     float y[A];
 #pragma unroll
     for (int j = 0; j < A; ++j) {
-        float p[4] = {0.f, 0.f, 0.f, 0.f};
+        float wv[T8], t[2];
 #pragma unroll
-        for (int m2 = 0; m2 < TM2; ++m2) {
-            const float2 wv = *reinterpret_cast<const float2*>(Wo + j * H + og * TM + 2 * m2);
-#pragma unroll
-            for (int c = 0; c < 4; ++c) { p[c] = __fmaf_rn(wv.x, in[m2][c].x, p[c]); p[c] = __fmaf_rn(wv.y, in[m2][c].y, p[c]); }
-        }
-#pragma unroll
-        for (int c = 0; c < 4; ++c) p[c] = group_sum(p[c]);
-        const float mine = og == 0 ? p[0] : (og == 1 ? p[1] : (og == 2 ? p[2] : p[3]));
-        y[j] = __fadd_rn(mine, bo[j]);
+        for (int m = 0; m < T8; ++m) wv[m] = Wo[j * H + n0 + m];
+        quarter_totals<T8>([&](int m, int c, float s) { return __fmaf_rn(wv[m], env_of(in[m], c), s); }, og, t);
+        const int src = quarter_src_lane(g, og);
+        const float t0 = __shfl_sync(0xffffffffu, t[0], src), t1 = __shfl_sync(0xffffffffu, t[1], src);
+        y[j] = __fadd_rn(og & 1 ? t1 : t0, bo[j]);
     }
     static_assert(A == 3, "two tanh pairs");
     const float2 t01 = am_tanh2(make_float2(y[0], y[1])), t2 = am_tanh2(make_float2(y[2], y[2]));
@@ -303,12 +371,13 @@ __device__ __forceinline__ void actor_forward(int act, const float* __restrict__
 
 
 // ---- genome layout in shared memory -------------------------------------------------------------------------
-// parameters() order in HBM (row-major [out][in]) -> the kernel's layout (matrices transposed to [in][out]):
+// parameters() order in HBM (row-major [out][in]) -> the kernel's layout (matrices transposed to [in][out], in the
+// row-pair blocks of pair_layout_index):
 //   Wt0[S][H] b0[H] | L x { Wt[H][H] b[H] gamma[H] beta[H] } | Wo[A][H] bo[A]
 __device__ __forceinline__ int genome_layout_index(int i, int S, int H, int L)
 {
     int r = i;
-    if (r < S * H) { const int j = r / S, k = r % S; return k * H + j; }
+    if (r < S * H) { const int j = r / S, k = r % S; return pair_layout_index(k, j, S, H); }
     r -= S * H;
     if (r < H) return S * H + r;
     r -= H;
@@ -316,7 +385,7 @@ __device__ __forceinline__ int genome_layout_index(int i, int S, int H, int L)
     if (r < L * per) {
         const int l = r / per, q = r % per;
         const int base = S * H + H + l * per;
-        if (q < H * H) { const int j = q / H, k = q % H; return base + k * H + j; }
+        if (q < H * H) { const int j = q / H, k = q % H; return base + pair_layout_index(k, j, H, H); }
         return base + q;
     }
     return i;      // Wo [A][H] then bo[A]: unchanged
