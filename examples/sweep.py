@@ -1,8 +1,11 @@
 """Train several SERL / TD3 runs in one process on one GPU: examples/train.py's flags, plus the seeds and a grid of
 `Parameters` attributes whose Cartesian product makes the runs.  Every run's RL half shares one grouped K7 launch per
-generation (serl_b200/sweep.py), and every run computes exactly what it computes when trained alone.
+generation (serl_b200/sweep.py), and every run computes exactly what it computes when trained alone.  The runs may differ
+in actor shape (hidden_size, num_layers, activation_actor): narrow and wide learners share the K7 launch, and each
+shape's population flies in a launch of its own.
 
     python examples/sweep.py -frames 20000 -pop_size 10 -seeds 7 8 9 -grid lr=0.0002,0.0004 noise_sd=0.2,0.3
+    python examples/sweep.py -frames 20000 -pop_size 10 -grid hidden_size=72,96 activation_actor=tanh,relu
 """
 import itertools
 import os
@@ -62,7 +65,7 @@ def make_runs(cla):
 if __name__ == '__main__':
     cla = parser.parse_args()
     runs = make_runs(cla)
-    sweep = Sweep([(p, env) for _, p, env in runs])
+    sweep = Sweep([(p, env) for _, p, env in runs], mixed_shapes=True)
     print('Sweep of %d runs on' % len(runs), runs[0][1].env_name)
     start_time = time.time()
     while not sweep.finished:

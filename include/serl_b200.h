@@ -248,4 +248,6 @@ const char* serl_last_error(void);
 #include "serl_td3.h"
 /* the kernel of a uniform actor: K1, or K1-TC with the widths [h] * (L + 1) (serl_actor_tc_widths) */
 #include "serl_route.h"
+/* K7 for learners of different actor shapes in one launch (serl_td3_train_mixed) */
+#include "serl_td3_mixed.h"
 #endif

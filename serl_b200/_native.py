@@ -3,7 +3,7 @@ fallback: importing succeeds without a GPU (so host logic is testable), but the 
 fails loudly when CUDA is unavailable.  tests/test_capi.py holds the signatures and constants below to the header,
 tests/test_td3_oracle.py those of include/serl_td3.h (TD3_SIGNATURES, TD3Desc, TD3_*), tests/test_deep_actor.py those of
 include/serl_route.h (ROUTE_SIGNATURES), tests/test_td3_group.py those of include/serl_td3_group.h (TD3_GROUP_SIGNATURES,
-TD3_MAX_GROUP)."""
+TD3_MAX_GROUP), tests/test_td3_mixed.py those of include/serl_td3_mixed.h (TD3_MIXED_SIGNATURES)."""
 import ctypes
 import os
 
@@ -106,6 +106,10 @@ TD3_SIGNATURES = {
 TD3_GROUP_SIGNATURES = {
     'serl_td3_train_group': (_int, [ctypes.POINTER(TD3Desc), _i32, _vp]),
 }
+# include/serl_td3_mixed.h: n descriptors of any actor shapes trained in one launch
+TD3_MIXED_SIGNATURES = {
+    'serl_td3_train_mixed': (_int, [ctypes.POINTER(TD3Desc), _i32, _vp]),
+}
 # include/serl_route.h: the kernel of a uniform actor (host only, no stream)
 ROUTE_SIGNATURES = {
     'serl_actor_tc_widths': (_i32, [_shape, _vp, _i32]),
@@ -124,7 +128,8 @@ def lib():
             raise NativeError('serl_b200: %s is missing — build it with `python -m serl_b200.build` '
                               '(there is no CPU fallback)' % LIB_PATH)
         L = ctypes.CDLL(LIB_PATH)
-        for name, (restype, argtypes) in {**SIGNATURES, **TD3_SIGNATURES, **TD3_GROUP_SIGNATURES, **ROUTE_SIGNATURES}.items():
+        for name, (restype, argtypes) in {**SIGNATURES, **TD3_SIGNATURES, **TD3_GROUP_SIGNATURES, **TD3_MIXED_SIGNATURES,
+                                         **ROUTE_SIGNATURES}.items():
             f = getattr(L, name)
             f.restype, f.argtypes = restype, argtypes
         _lib = L

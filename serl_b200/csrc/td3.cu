@@ -13,13 +13,15 @@
 // and however the steps are split across launches.  Plain fp32 on CUDA cores: at batch <= 128 the work per step is
 // 10-30 MFLOP (up to ~0.4 GFLOP for the widest actors), and the step is bound by the ~50 dependent phases, not by
 // arithmetic.  Actors wider than 128 run their h x h blocks as tiled phases (td3_kernel<CS, true>, fwd_wide / bwd_wide).
-// td3_group_kernel runs several independent learners in one launch, one cluster each (serl_td3_train_group).
+// td3_group_kernel runs several independent learners of one hidden class in one launch, one cluster each
+// (serl_td3_train_group); td3_mixed_kernel runs narrow and wide learners together (serl_td3_train_mixed).
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
 #include <stdio.h>
 
 #include "../../include/serl_td3.h"
+#include "../../include/serl_td3_mixed.h"
 #include "common.cuh"
 
 namespace {
@@ -763,6 +765,24 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_group_ke
     td3_learner<CS, WIDE, true>(t.a[g]);
 }
 
+// A group of narrow and wide learners in one launch (serl_td3_train_mixed): cluster g branches once, uniformly for the
+// whole cluster, on its learner's hidden width into td3_group_kernel's learner of that class, so each learner gets the
+// bits its solo launch gives.  Every cluster reserves both branches' static shared memory (the wide tiles' WIDE_SMEM
+// included; with one CTA per SM that costs no residency).  The narrow learner is a call: with both learners inlined,
+// ptxas spills registers on the narrow path (64-68 bytes), which neither td3_group_kernel does; as a call it spills
+// nothing and reads its Args from a 184-byte stack copy.
+template <int CS>
+__device__ __noinline__ void narrow_learner(const Args& a) { td3_learner<CS, false, true>(a); }
+
+template <int CS>
+__global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_mixed_kernel(const __grid_constant__ Group t)
+{
+    unsigned g;
+    asm("mov.u32 %0, %%clusterid.x;" : "=r"(g));
+    if (t.a[g].h > 128) td3_learner<CS, true, true>(t.a[g]);
+    else narrow_learner<CS>(t.a[g]);
+}
+
 int64_t actor_floats(const serl_actor_shape& s)
 {
     const int64_t h = s.hidden;
@@ -786,10 +806,13 @@ int launch(const Args& a, cudaStream_t s)
     return serl_launch("td3_kernel", td3_kernel<CS, false>, dim3(CS), dim3(NT), 0, s, a);
 }
 
+// one launch of the group's n learners with steps: td3_group_kernel of their hidden class, td3_mixed_kernel when they
+// hold both narrow and wide actors
 template <int CS>
-int launch_group(const Group& t, int n, int h, cudaStream_t s)
+int launch_group(const Group& t, int n, bool narrow, bool wide, cudaStream_t s)
 {
-    if (h > 128) return serl_launch("td3_group_kernel (wide)", td3_group_kernel<CS, true>, dim3(n * CS), dim3(NT), 0, s, t);
+    if (narrow && wide) return serl_launch("td3_mixed_kernel", td3_mixed_kernel<CS>, dim3(n * CS), dim3(NT), 0, s, t);
+    if (wide) return serl_launch("td3_group_kernel (wide)", td3_group_kernel<CS, true>, dim3(n * CS), dim3(NT), 0, s, t);
     return serl_launch("td3_group_kernel", td3_group_kernel<CS, false>, dim3(n * CS), dim3(NT), 0, s, t);
 }
 
@@ -861,39 +884,49 @@ extern "C" int serl_td3_train(const serl_td3_desc* d, void* stream)
     }
 }
 
-extern "C" int serl_td3_train_group(const serl_td3_desc* descs, int n, void* stream)
+namespace {
+
+// serl_td3_train_group (same_shape: every learner has learner 0's actor shape) and serl_td3_train_mixed (any shapes of
+// K7's domain); `name` prefixes the error messages
+int train_group(const char* name, const serl_td3_desc* descs, int n, void* stream, bool same_shape)
 {
-    if (n < 1 || n > SERL_TD3_MAX_GROUP) return serl_fail(SERL_ERR_ARG, "serl_td3_train_group: n must be 1..SERL_TD3_MAX_GROUP (64)");
-    if (!descs) return serl_fail(SERL_ERR_ARG, "serl_td3_train_group: null descriptors");
     char msg[256];
+    if (n < 1 || n > SERL_TD3_MAX_GROUP) {
+        snprintf(msg, sizeof(msg), "%s: n must be 1..SERL_TD3_MAX_GROUP (64)", name);
+        return serl_fail(SERL_ERR_ARG, msg);
+    }
+    if (!descs) {
+        snprintf(msg, sizeof(msg), "%s: null descriptors", name);
+        return serl_fail(SERL_ERR_ARG, msg);
+    }
     for (int i = 0; i < n; ++i)
         if (const char* why = desc_error(descs + i)) {
-            snprintf(msg, sizeof(msg), "serl_td3_train_group: learner %d: %s", i, why);
+            snprintf(msg, sizeof(msg), "%s: learner %d: %s", name, i, why);
             return serl_fail(SERL_ERR_ARG, msg);
         }
     const serl_actor_shape& sh = descs[0].shape;
     const int cs = descs[0].cluster_size ? descs[0].cluster_size : 8;
     for (int i = 1; i < n; ++i) {
         const serl_actor_shape& si = descs[i].shape;
-        if (si.state_dim != sh.state_dim || si.action_dim != sh.action_dim || si.hidden != sh.hidden ||
-            si.num_layers != sh.num_layers || si.activation != sh.activation) {
-            snprintf(msg, sizeof(msg), "serl_td3_train_group: learner %d: actor shape differs from learner 0's (one launch trains "
-                                       "one shape)", i);
+        if (same_shape && (si.state_dim != sh.state_dim || si.action_dim != sh.action_dim || si.hidden != sh.hidden ||
+                           si.num_layers != sh.num_layers || si.activation != sh.activation)) {
+            snprintf(msg, sizeof(msg), "%s: learner %d: actor shape differs from learner 0's (one launch trains one shape)", name, i);
             return serl_fail(SERL_ERR_ARG, msg);
         }
         if ((descs[i].cluster_size ? descs[i].cluster_size : 8) != cs) {
-            snprintf(msg, sizeof(msg), "serl_td3_train_group: learner %d: cluster_size differs from learner 0's", i);
+            snprintf(msg, sizeof(msg), "%s: learner %d: cluster_size differs from learner 0's", name, i);
             return serl_fail(SERL_ERR_ARG, msg);
         }
     }
     // the learners with steps to take, each with its own slice of one scratch buffer (slices aligned to 128 bytes)
     Group t{};
-    int m = 0;
+    int m = 0, wide = 0;             // learners with steps, and how many of them are wide
     size_t total = 0;
     size_t off[SERL_TD3_MAX_GROUP];
     for (int i = 0; i < n; ++i) {
         if (descs[i].n_steps == 0) continue;
         t.a[m] = make_args(descs + i);
+        wide += t.a[m].h > 128;
         off[m] = total;
         total += (scratch_floats(t.a[m]) + 31) / 32 * 32;
         ++m;
@@ -905,9 +938,21 @@ extern "C" int serl_td3_train_group(const serl_td3_desc* descs, int n, void* str
     if (e != cudaSuccess) return serl_fail_cuda(e, "td3 scratch");
     for (int g = 0; g < m; ++g) t.a[g].ws = (float*)ws + off[g];
     switch (cs) {
-    case 1: return launch_group<1>(t, m, sh.hidden, s);
-    case 2: return launch_group<2>(t, m, sh.hidden, s);
-    case 4: return launch_group<4>(t, m, sh.hidden, s);
-    default: return launch_group<8>(t, m, sh.hidden, s);
+    case 1: return launch_group<1>(t, m, wide < m, wide > 0, s);
+    case 2: return launch_group<2>(t, m, wide < m, wide > 0, s);
+    case 4: return launch_group<4>(t, m, wide < m, wide > 0, s);
+    default: return launch_group<8>(t, m, wide < m, wide > 0, s);
     }
+}
+
+}  // namespace
+
+extern "C" int serl_td3_train_group(const serl_td3_desc* descs, int n, void* stream)
+{
+    return train_group("serl_td3_train_group", descs, n, stream, true);
+}
+
+extern "C" int serl_td3_train_mixed(const serl_td3_desc* descs, int n, void* stream)
+{
+    return train_group("serl_td3_train_mixed", descs, n, stream, false);
 }

@@ -4,14 +4,18 @@ With `fused_td3`, a generation's RL half is K7 (csrc/td3.cu), one thread-block c
 most of a run's wall-clock time.  `Sweep` moves S runs forward one generation at a time: the head of every run's
 generation (population rollout, SSNE epoch, exploration episode: Agent.train_head), then ONE grouped K7 launch that takes
 every run's gradient steps on its own cluster (td3_fused.train_group), then every run's tail (validation, actor injection,
-next front: Agent.train_tail).  The runs may differ in seed and in any `Parameters` attribute that keeps the actor's shape.
+next front: Agent.train_tail).  The runs may differ in seed and in any `Parameters` attribute that keeps the actor's shape;
+with `mixed_shapes` they may differ in actor shape too (hidden_size, num_layers, activation_actor, anywhere K7 trains):
+the K7 launch then trains narrow and wide actors together (serl_td3_train_mixed).
 
 A SERL10 population (10 actors x 3 envs) fills a few warps for the serial latency of one 2001-step trajectory, so the
 populations fly together too: every run draws its front's references at their usual place (its np.random stream advances
 as it would alone) and leaves the launch to the Sweep, which then makes ONE rollout launch with per-actor env blocks
 (SERL_ROLLOUT_PER_ACTOR_REFS) for each group of runs whose agent.population_key agrees (`launch_groups`), both for the
-fronts the heads take and for the next generation's fronts the tails queue.  Each run reads its slice of the result, bit
-for bit what its own launch gives.  A merged launch has ONE status word: a non-finite trajectory in any run of it raises
+fronts the heads take and for the next generation's fronts the tails queue.  Runs of different actor shapes fall into
+different launch groups; the first group's launch is queued on the current stream and every further group's on a stream
+of its own, so that they run side by side.  Each run reads its slice of the result, bit for bit what its own launch
+gives.  A merged launch has ONE status word: a non-finite trajectory in any run of it raises
 in every run that shares it.  A run whose queued front is invalidated at its next head (its population, RL actor or
 environment changed) flies its population alone.
 
@@ -31,6 +35,7 @@ import torch
 
 from . import evaluation, td3_fused
 from .core import agent as agent_mod
+from ._native import NativeError
 from .rollout import actor_shape
 
 
@@ -93,8 +98,9 @@ def _shape(p):
 
 
 class Sweep:
-    def __init__(self, runs):
-        """runs: a list of (Parameters, env), each seeded and built as base/train.py:88-94 builds one run"""
+    def __init__(self, runs, mixed_shapes=False):
+        """runs: a list of (Parameters, env), each seeded and built as base/train.py:88-94 builds one run.  mixed_shapes: the
+        runs' actor shapes may differ (each inside K7's domain); without it they must agree."""
         runs = list(runs)
         if not runs:
             raise ValueError('Sweep: no runs')
@@ -103,9 +109,16 @@ class Sweep:
         for i, (p, _) in enumerate(runs):
             if not getattr(p, 'fused_td3', False):
                 raise ValueError('Sweep: run %d does not set fused_td3 (the sweep trains every RL half in one K7 launch)' % i)
-            if _shape(p) != _shape(runs[0][0]):
+            if mixed_shapes:
+                try:
+                    td3_fused.state_floats(actor_shape(p.hidden_size, p.num_layers, p.activation_actor, p.state_dim, p.action_dim))
+                except NativeError as e:
+                    raise ValueError('Sweep: run %d has actor shape %s, which K7 does not train (%s)' % (i, _shape(p), e)) from None
+            elif _shape(p) != _shape(runs[0][0]):
                 raise ValueError('Sweep: run %d has actor shape %s, run 0 has %s (one K7 launch trains one shape)'
                                  % (i, _shape(p), _shape(runs[0][0])))
+        self.mixed_shapes = bool(mixed_shapes)
+        self._streams = []             # the population launch groups' streams after the first, created once and kept
         self.runs = []
         outer = RNGState.capture()
         try:
@@ -145,7 +158,7 @@ class Sweep:
         group = [(r, n) for r, n in zip(live, plans) if n]
         launches = td3_fused.train_group([r.agent.rl_agent for r, _ in group], [r.agent.replay_buffer for r, _ in group],
                                          [n for _, n in group], [r.agent.rl_iteration + 1 for r, _ in group],
-                                         [r.agent.args.use_champion_target for r, _ in group])
+                                         [r.agent.args.use_champion_target for r, _ in group], mixed_shapes=self.mixed_shapes)
         losses = dict(zip((id(r) for r, _ in group), td3_fused.group_losses(launches)))
         for r, n in zip(live, plans):
             with rng_scope(r.rng):
@@ -155,23 +168,42 @@ class Sweep:
         return [r.stats if id(r) in live_ids else None for r in self.runs]
 
     def _launch_populations(self, fronts):
-        """one rollout launch per launch group for the fronts [(run, front)] whose population launch is still deferred"""
+        """one rollout launch per launch group for the fronts [(run, front)] whose population launch is still deferred: the
+        first group's on the current stream, each further group's on a stream of its own, so that launches of different
+        shapes do not queue behind each other"""
         pending = [(r, f) for r, f in fronts if f is not None and f.pop_draws is not None]
         keys = [agent_mod.population_key(r.params, r.env) for r, _ in pending]
-        for g in launch_groups(keys):
-            agent_mod.launch_population_group([(pending[i][0].agent, pending[i][1]) for i in g])
+        groups = launch_groups(keys)
+        if not groups:
+            return
+        dev = pending[0][0].agent.device
+        cur = torch.cuda.current_stream(dev)
+        while len(self._streams) < len(groups) - 1:
+            self._streams.append(torch.cuda.Stream(dev))
+        side = self._streams[:len(groups) - 1]
+        for s in side:                 # fork before anything is queued: the genomes are written on the current stream
+            s.wait_stream(cur)
+        for g, s in zip(groups, [None] + side):
+            with torch.cuda.stream(s) if s is not None else contextlib.nullcontext():
+                agent_mod.launch_population_group([(pending[i][0].agent, pending[i][1]) for i in g])
+        # join before anything reads a front: SSNE rewrites the genomes in place on the current stream, and the caching
+        # allocator hands the side streams' blocks out again once their tensors are freed
+        for s in side:
+            cur.wait_stream(s)
 
     def evaluate(self, conditions, refs, num_trails=1):
-        """evaluation.evaluate_population of every run's population on `conditions` with the references `refs`: all runs
-        share one actor shape, so their populations stack into one call.  Returns one PopulationEval per run (None for a
-        run without a population)."""
-        pops = [r.agent.pop.genomes if len(r.agent.pop) else None for r in self.runs]
-        live = [g for g in pops if g is not None]
-        if not live:
-            return [None] * len(self.runs)
-        res = evaluation.evaluate_population(torch.cat(live), self.runs[0].agent.shape, conditions, refs, num_trails)
-        parts = iter(res.split([g.shape[0] for g in live]))
-        return [next(parts) if g is not None else None for g in pops]
+        """evaluation.evaluate_population of every run's population on `conditions` with the references `refs`: the
+        populations of one actor shape stack into one call, one call per shape in order of first appearance (runs in run
+        order within it), so the sensor-noise draws continue on the np.random stream in that order.  Returns one
+        PopulationEval per run (None for a run without a population)."""
+        out = [None] * len(self.runs)
+        shapes = [_shape(r.params) if len(r.agent.pop) else None for r in self.runs]
+        for g in launch_groups(shapes):
+            res = evaluation.evaluate_population(torch.cat([self.runs[i].agent.pop.genomes for i in g]), self.runs[g[0]].agent.shape,
+                                                 conditions, refs, num_trails)
+            for i, part in zip(g, res.split([self.runs[i].agent.pop.genomes.shape[0] for i in g])):
+                out[i] = part
+        return out
 
     def save_agent(self, folder=None):
         """Agent.save_agent of every run into its own folder <folder or the run's save_foldername>/run<i>"""

@@ -149,12 +149,13 @@ def _rows(replay):
     return (replay.data, len(replay)) if hasattr(replay, 'data') else (replay, replay.shape[0])
 
 
-def train_group(learners, replays, ns, firsts, champion_targets, record=False):
+def train_group(learners, replays, ns, firsts, champion_targets, record=False, mixed_shapes=False):
     """learner g takes ns[g] gradient steps on global iterations firsts[g].. sampling from replays[g] (as
     learners[g].train_steps would), all learners in the same K7 launches (serl_td3_train_group): one cluster per learner,
-    lockstep chunks of LAUNCH_STEPS steps, at most TD3_MAX_GROUP learners per launch.  The learners must share actor shape
-    and cluster size; each gets exactly the bits its solo run gives.  Returns one TD3Launch per learner; their losses are
-    views into one device buffer, so `group_losses` reads them back in one copy."""
+    lockstep chunks of LAUNCH_STEPS steps, at most TD3_MAX_GROUP learners per launch.  The learners must share cluster
+    size, and actor shape unless `mixed_shapes` (serl_td3_train_mixed: narrow and wide actors of any shape K7 trains, in
+    the same launches); each gets exactly the bits its solo run gives.  Returns one TD3Launch per learner; their losses
+    are views into one device buffer, so `group_losses` reads them back in one copy."""
     G = len(learners)
     assert G == len(replays) == len(ns) == len(firsts) == len(champion_targets)
     assert len(set(id(f) for f in learners)) == G, 'a learner appears twice in the group'
@@ -179,7 +180,7 @@ def train_group(learners, replays, ns, firsts, champion_targets, record=False):
             for j, g in enumerate(part):
                 m = min(LAUNCH_STEPS, ns[g] - k0)
                 descs[j] = learners[g]._desc(rows[g][0], rows[g][1], m, firsts[g] + k0, champion_targets[g], None, out[g], k0)
-            _native.call('serl_td3_train_group', descs, len(part), device=dev)
+            _native.call('serl_td3_train_mixed' if mixed_shapes else 'serl_td3_train_group', descs, len(part), device=dev)
             for g in part:
                 learners[g]._advance(firsts[g] + k0, min(LAUNCH_STEPS, ns[g] - k0))
         k0 += LAUNCH_STEPS
