@@ -142,12 +142,25 @@ int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shap
  *                of the replay rows' column 19 (get_cost, envs/phlabenv.py:369-375, with V0 of the env's own plant variant),
  *                i.e. the safety cost trial_cost = sum info['cost'] of base/core/operator_runner.py:64.  Counted by the
  *                d_track instantiations, so it needs d_track: SERL_ERR_ARG before any CUDA call without it
+ *                SERL_ROLLOUT_INCREMENTAL: incremental control (envs/phlabenv.py:174-220, 377-380, 443-466; the env
+ *                PHlab_attitude_incremental).  The actor's three outputs are actuator RATES scaled to +-25 deg/s; every step
+ *                integrates them in fp64, u = last_u + rate * 0.01 (no clip: the plant's input saturation acts as usual), the
+ *                fault shim and the plant take u, and last_u = u.  The observation is the 7 of the absolute mode followed by
+ *                (float)last_u: shape.state_dim must be 10 with the flag and 7 without it.  Replay rows then have
+ *                SERL_REPLAY_COLS_OF(10) = 26 columns: 0-9 obs, 10-12 action, 13-22 next_obs, 23 reward, 24 done, 25 cost;
+ *                the trace's columns 12-14 and d_actions record the integrated u (the reference's env.last_u).  Not with
+ *                d_track, d_cost, SERL_ROLLOUT_GUST or d_sensor_noise: SERL_ERR_ARG before any CUDA call.  With widths (K1-TC) the genome
+ *                has 10 * w0 layer-0 weights: serl_actor_num_params_wide(widths) + 3 * w0 floats per actor.
+ *                The env modes are device data the host does not read: the reference flies incremental control on the
+ *                nominal build only (any mode containing 'incremental' selects h2000-v90, no fault, no gust, no noise)
  * t_max <= 0 selects the training defaults (20 s, smooth width 3 s). */
 #define SERL_TRACK_COLS 4
-#define SERL_REPLAY_COLS 20
+#define SERL_REPLAY_COLS 20                       /* = SERL_REPLAY_COLS_OF(7) */
+#define SERL_REPLAY_COLS_OF(S) (2 * (S) + 6)      /* obs S | action 3 | next_obs S | reward | done | cost */
 #define SERL_ROLLOUT_GUST 1
 #define SERL_ROLLOUT_STAGGER 2
 #define SERL_ROLLOUT_PER_ACTOR_REFS 4
+#define SERL_ROLLOUT_INCREMENTAL 8
 enum { SERL_STATUS_NONFINITE = 1,     /* a trajectory's state / return became NaN or infinite */
        SERL_STATUS_GUST_FLAG = 2 };   /* an env has SERL_MODE_GUST but the launch was not made with SERL_ROLLOUT_GUST */
 typedef struct {

@@ -24,6 +24,7 @@ MODE_GUST_UP = 1 << 25
 ROLLOUT_GUST = 1
 ROLLOUT_STAGGER = 2
 ROLLOUT_PER_ACTOR_REFS = 4
+ROLLOUT_INCREMENTAL = 8
 STATUS_NONFINITE = 1
 STATUS_GUST_FLAG = 2
 # include/serl_td3.h (K7, the fused TD3 learner)

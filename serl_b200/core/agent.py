@@ -72,6 +72,9 @@ class Agent:
     def __init__(self, args, environment):
         self.args = args
         self.env = environment
+        if bool(getattr(environment, 'incremental', False)) != (args.state_dim == rollout.INCREMENTAL_STATE_DIM):
+            raise ValueError('Agent: args.state_dim = %s does not match the env: the observation of incremental control has 10 entries, '
+                             'that of absolute control 7' % args.state_dim)
         if not torch.cuda.is_available():
             from .._native import NativeError
             raise NativeError('serl_b200.Agent needs a CUDA device: the rollout / evolution engine has no CPU fallback')
@@ -82,7 +85,8 @@ class Agent:
             self.rl_agent = FusedTD3(args)
         else:
             self.rl_agent = td3.TD3(args)
-        self.replay_buffer = replay_memory.DeviceReplayMemory(args.buffer_size, self.device, seed=int(getattr(args, 'seed', 7)))
+        self.replay_buffer = replay_memory.DeviceReplayMemory(args.buffer_size, self.device, seed=int(getattr(args, 'seed', 7)),
+                                                              state_dim=args.state_dim)
         self.noise_process = mod_utils.GaussianNoise(args.action_dim, sd=args.noise_sd)
         if len(self.pop):
             self.evolver = utils_ne.SSNE(self.args, self.rl_agent.critic, self.evaluate)
@@ -180,7 +184,7 @@ class Agent:
         rows = rows[:n]
         self.replay_buffer.add_rows(rows)
         agent.buffer.add_rows(rows)
-        crit = rows[rows[:, rollout.REPLAY_COST] > 0.5]
+        crit = rows[rows[:, rollout.transition_cols(self.shape.state_dim)] > 0.5]
         if crit.shape[0]:
             agent.critical_buffer.add_rows(crit)
         self.num_frames += n
@@ -388,14 +392,15 @@ class Agent:
         self._last_result = r
         if store:
             # the stored transitions of EVERY actor reach EVERY rank (identical shared / per-actor buffers on all ranks)
-            rows = r.replay if r is not None else torch.zeros((0, horizon, rollout.REPLAY_COLS), dtype=torch.float32, device=self.device)
-            rows_all = engine.gather_rows(rows.reshape(rows.shape[0], -1), pop, world, rank).reshape(pop, horizon, rollout.REPLAY_COLS)
+            cols = rollout.replay_cols(self.shape.state_dim)
+            rows = r.replay if r is not None else torch.zeros((0, horizon, cols), dtype=torch.float32, device=self.device)
+            rows_all = engine.gather_rows(rows.reshape(rows.shape[0], -1), pop, world, rank).reshape(pop, horizon, cols)
             steps_all = rec_all[:, 3].to(torch.int64)
             sel = torch.arange(horizon, device=self.device)[None, :] < steps_all[:, None]
             self.replay_buffer.add_rows(rows_all[sel])
             actors = torch.arange(pop, device=self.device)
             self.pop.buffers.append(actors, rows_all, sel)
-            self.pop.critical_buffers.append(actors, rows_all, sel & (rows_all[..., rollout.REPLAY_COST] > 0.5))
+            self.pop.critical_buffers.append(actors, rows_all, sel & (rows_all[..., rollout.transition_cols(self.shape.state_dim)] > 0.5))
         rec_host = rec_all.cpu().numpy()
         if r is not None:
             r.check()

@@ -9,7 +9,7 @@ from collections import namedtuple
 import numpy as np
 import torch
 
-from ..rollout import TRANSITION_COLS
+from ..rollout import replay_dims, transition_cols
 
 Transition = namedtuple('Transition', ('state', 'action', 'next_state', 'reward', 'done'))
 
@@ -76,12 +76,10 @@ class ReplayMemory:
         return tuple(torch.from_numpy(self._store[f][pick]).to(self.device) for f in Transition._fields)
 
 
-REPLAY_DIMS = (7, 3, 7, 1, 1)        # obs, action, next_obs, reward, done = the first TRANSITION_COLS columns of a K1 replay row
-
-
-def _split(rows):
+def _split(rows, state_dim):
+    """the Transition fields (obs, action, next_obs, reward, done) of stored transitions [n, transition_cols(state_dim)]"""
     out, off = [], 0
-    for d in REPLAY_DIMS:
+    for d in replay_dims(state_dim)[:5]:
         out.append(rows[:, off:off + d])
         off += d
     return tuple(out)
@@ -89,12 +87,14 @@ def _split(rows):
 
 class DeviceReplayMemory:
     """Ring buffer on the GPU with ReplayMemory's interface.  Rows are K1 replay rows (include/serl_b200.h
-    SERL_REPLAY_COLS: obs 7 | action 3 | next_obs 7 | reward | done | cost); sampling uses a device generator, so the
-    stdlib `random` stream the SSNE planner consumes does not depend on the buffer (every rank holds identical buffers and
-    identical generators -> identical batches)."""
+    SERL_REPLAY_COLS_OF(state_dim): obs | action 3 | next_obs | reward | done | cost; rollout.replay_dims) without the cost
+    flag; sampling uses a device generator, so the stdlib `random` stream the SSNE planner consumes does not depend on the
+    buffer (every rank holds identical buffers and identical generators -> identical batches)."""
 
-    def __init__(self, capacity, device, seed=0):
+    def __init__(self, capacity, device, seed=0, state_dim=7):
         self.capacity, self.device = int(capacity), torch.device(device)
+        self.state_dim = int(state_dim)
+        self.cols = transition_cols(self.state_dim)
         self.data = None
         self._count, self.position = 0, 0
         self.gen = None
@@ -108,17 +108,17 @@ class DeviceReplayMemory:
 
     def _alloc(self):
         if self.data is None:
-            self.data = torch.zeros((self.capacity, TRANSITION_COLS), dtype=torch.float32, device=self.device)
+            self.data = torch.zeros((self.capacity, self.cols), dtype=torch.float32, device=self.device)
             self.gen = torch.Generator(device=self.device)
             self.gen.manual_seed(self._seed)
 
     def add_rows(self, rows):
-        """append n transitions [n, >=TRANSITION_COLS] (device tensor, chronological order) with ring semantics."""
+        """append n transitions [n, >=cols] (device tensor, chronological order) with ring semantics."""
         n = int(rows.shape[0])
         if n == 0:
             return
         self._alloc()
-        rows = rows[:, :TRANSITION_COLS].to(self.device, torch.float32)
+        rows = rows[:, :self.cols].to(self.device, torch.float32)
         if n > self.capacity:
             skip = n - self.capacity
             rows = rows[skip:]
@@ -146,14 +146,14 @@ class DeviceReplayMemory:
     def _chronological_rows(self):
         n = len(self)
         if n == 0:
-            return torch.zeros((0, TRANSITION_COLS), dtype=torch.float32, device=self.device)
+            return torch.zeros((0, self.cols), dtype=torch.float32, device=self.device)
         if self._count <= self.capacity:
             return self.data[:n]
         return torch.cat((self.data[self.position:], self.data[:self.position]))
 
     def get_latest(self, latest):
         rows = self._chronological_rows()[-int(latest):]
-        return [Transition(*_split(rows[i:i + 1])) for i in range(rows.shape[0])]
+        return [Transition(*_split(rows[i:i + 1], self.state_dim)) for i in range(rows.shape[0])]
 
     def add_content_of(self, other):
         rows = other._chronological_rows() if hasattr(other, '_chronological_rows') else None
@@ -168,16 +168,18 @@ class DeviceReplayMemory:
         self._alloc()
         n = len(self)
         pick = torch.randperm(n, device=self.device, generator=self.gen)[:int(batch_size)]
-        return _split(self.data[pick])
+        return _split(self.data[pick], self.state_dim)
 
 
 class PopulationBuffers:
     """The per-actor replay buffers of the whole population (GeneticAgent.buffer / .critical_buffer,
-    base/core/genetic_agent.py:14-16) as ONE device tensor [pop, capacity, TRANSITION_COLS] with per-actor ring positions, filled
-    for all actors of a generation by one vectorised scatter."""
+    base/core/genetic_agent.py:14-16) as ONE device tensor [pop, capacity, cols] with per-actor ring positions, filled
+    for all actors of a generation by one vectorised scatter (cols: the transition of an observation of state_dim entries)."""
 
-    def __init__(self, pop, capacity, device):
+    def __init__(self, pop, capacity, device, state_dim=7):
         self.pop, self.capacity, self.device = int(pop), int(capacity), torch.device(device)
+        self.state_dim = int(state_dim)
+        self.cols = transition_cols(self.state_dim)
         self.data = None
         self.pos = torch.zeros(self.pop, dtype=torch.int64, device=self.device)
         self.count = torch.zeros(self.pop, dtype=torch.int64, device=self.device)
@@ -185,12 +187,12 @@ class PopulationBuffers:
 
     def _alloc(self):
         if self.data is None:
-            self.data = torch.zeros((self.pop, self.capacity, TRANSITION_COLS), dtype=torch.float32, device=self.device)
+            self.data = torch.zeros((self.pop, self.capacity, self.cols), dtype=torch.float32, device=self.device)
             self.gen = torch.Generator(device=self.device)
             self.gen.manual_seed(1)
 
     def append(self, actors, rows, select):
-        """rows [n, horizon, >=TRANSITION_COLS]; select [n, horizon] bool (time order): the selected rows of rows[i] go to actor actors[i]."""
+        """rows [n, horizon, >=cols]; select [n, horizon] bool (time order): the selected rows of rows[i] go to actor actors[i]."""
         self._alloc()
         n, h = select.shape
         cnt = select.sum(1)
@@ -198,7 +200,7 @@ class PopulationBuffers:
         keep = select & (rank >= (cnt - self.capacity)[:, None])
         a_idx = actors.to(torch.int64)[:, None].expand(n, h)
         slot = (self.pos[actors][:, None] + rank) % self.capacity
-        self.data[a_idx[keep], slot[keep]] = rows[..., :TRANSITION_COLS][keep].to(torch.float32)
+        self.data[a_idx[keep], slot[keep]] = rows[..., :self.cols][keep].to(torch.float32)
         self.pos[actors] = (self.pos[actors] + cnt) % self.capacity
         self.count[actors] += cnt
 
@@ -211,7 +213,7 @@ class PopulationBuffers:
     def rows_of(self, i):
         n = int(min(int(self.count[i]), self.capacity))
         if n == 0 or self.data is None:
-            return torch.zeros((0, TRANSITION_COLS), dtype=torch.float32, device=self.device)
+            return torch.zeros((0, self.cols), dtype=torch.float32, device=self.device)
         if int(self.count[i]) <= self.capacity:
             return self.data[i, :n]
         p = int(self.pos[i])
@@ -242,7 +244,7 @@ class ActorBuffer:
             return
         o = self.owner
         o._alloc()
-        rows = rows[-o.capacity:, :TRANSITION_COLS].to(o.device, torch.float32)
+        rows = rows[-o.capacity:, :o.cols].to(o.device, torch.float32)
         m = int(rows.shape[0])
         slot = (o.pos[self.index] + (n - m) + torch.arange(m, device=o.device)) % o.capacity
         o.data[self.index, slot] = rows
@@ -262,10 +264,10 @@ class ActorBuffer:
 
     def get_latest(self, latest):
         rows = self._chronological_rows()[-int(latest):]
-        return [Transition(*_split(rows[i:i + 1])) for i in range(rows.shape[0])]
+        return [Transition(*_split(rows[i:i + 1], self.owner.state_dim)) for i in range(rows.shape[0])]
 
     def sample(self, batch_size):
         self.owner._alloc()
         rows = self._chronological_rows()
         pick = torch.randperm(rows.shape[0], device=rows.device, generator=self.owner.gen)[:int(batch_size)]
-        return _split(rows[pick])
+        return _split(rows[pick], self.owner.state_dim)

@@ -42,7 +42,10 @@ class Critic(nn.Module):
 class TD3:
     def __init__(self, args):
         self.args = args
-        mem = replay_memory.DeviceReplayMemory if torch.device(args.device).type == 'cuda' else replay_memory.ReplayMemory
+        if torch.device(args.device).type == 'cuda':
+            mem = lambda capacity, device: replay_memory.DeviceReplayMemory(capacity, device, state_dim=args.state_dim)
+        else:
+            mem = replay_memory.ReplayMemory
         self.buffer = mem(args.individual_bs, args.device)
         self.critical_buffer = mem(args.individual_bs, args.device)
         self.actor = Actor(args, init=True).to(args.device)

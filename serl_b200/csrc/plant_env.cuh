@@ -400,7 +400,7 @@ struct Handoff {
     double* X;      // [NX][n]
     double* t;      // [n]
     double* ret;    // [n]
-    float* obs;     // [7][n]
+    float* obs;     // [7][n]; incremental launches (INC): [10][n], followed by last_u [3][n] f64
     int* k;         // [n]  executed steps | done << 30
     int* flag;      // [n / 32] one word per warp, 1 when the record is complete
     long long n;
@@ -511,8 +511,15 @@ __device__ __forceinline__ void env_bind(Env& e, const RolloutArgs& a, int env, 
     if (!GUST && e.gust && a.status) atomicOr(a.status, SERL_STATUS_GUST_FLAG);
 }
 
+// observation entries of a kernel instantiation: 7, or 10 with incremental control (INC).  A namespace-scope constant because
+// a local constexpr declaration in a kernel body moved the instruction schedule of the instantiations without INC
+template <bool INC> constexpr int OBS_DIM = INC ? 10 : 7;
+
 // a lane without an env: done from the start, with a zero state and observation (it still takes part in the actor)
-__device__ __forceinline__ void env_idle(Env& e, const RolloutArgs& a, const real* pv_base, float* obs)
+// INC: incremental control (SERL_ROLLOUT_INCREMENTAL): the observation has 10 entries and the env carries last_u[3], the
+// deflection the rates were integrated into (kept by the kernel next to Env, which the other instantiations share unchanged)
+template <bool INC = false>
+__device__ __forceinline__ void env_idle(Env& e, const RolloutArgs& a, const real* pv_base, float* obs, double* last_u = nullptr)
 {
     e.done = true; e.k = 0; e.ret = 0.0; e.t = 0.0; e.fault = 0; e.gust = 0; e.pv = pv_base; e.pv_post = nullptr; e.theta_trim = 0.0;
     e.ref_lv = a.ref_levels; e.ref_st = a.ref_starts;
@@ -520,6 +527,9 @@ __device__ __forceinline__ void env_idle(Env& e, const RolloutArgs& a, const rea
     for (int i = 0; i < NX; ++i) e.X[i] = 0.0;
 #pragma unroll
     for (int i = 0; i < 7; ++i) obs[i] = 0.f;
+    if constexpr (INC)
+#pragma unroll
+        for (int i = 0; i < 3; ++i) { obs[7 + i] = 0.f; last_u[i] = 0.0; }
 }
 
 // end of a trajectory: return and executed steps.  A NaN action poisons the state at once, so a non-finite return or
@@ -565,8 +575,10 @@ __device__ __forceinline__ void sensor_noise(const RolloutArgs& a, size_t traj, 
 // GUST names the same plant_step instance as env_step<STAB, GUST> (call 0 has no gust stage either way), so a kernel
 // carries one copy of the step code.
 // TRACK: zero the tracking-error sums; the controlled state before step 0 is reset()'s output env.x.
-template <bool STAB = false, bool GUST = false, bool TRACK = false>
-static __device__ __forceinline__ void env_reset(Env& e, const RolloutArgs& a, int env, float* obs, size_t traj = 0)
+// INC: last_u = 0 and obs[7..9] = last_u (phlabenv.py:425-426)
+template <bool STAB = false, bool GUST = false, bool TRACK = false, bool INC = false>
+static __device__ __forceinline__ void env_reset(Env& e, const RolloutArgs& a, int env, float* obs, size_t traj = 0,
+                                                 double* last_u = nullptr)
 {
     const double* ic = plant_ic(a.env_mode[env] & 0xff);
 #pragma unroll
@@ -583,6 +595,9 @@ static __device__ __forceinline__ void env_reset(Env& e, const RolloutArgs& a, i
     }
     obs[0] = obs[1] = obs[2] = 0.f;
     obs[3] = (float)x0[0]; obs[4] = (float)x0[1]; obs[5] = (float)x0[2]; obs[6] = (float)x0[4];
+    if constexpr (INC)
+#pragma unroll
+        for (int i = 0; i < 3; ++i) { obs[7 + i] = 0.f; last_u[i] = 0.0; }
     double U[3] = {0.0, 0.0, 0.0}, cmd[3];
     apply_fault(e.fault, U, cmd);
     plant_step_env<STAB, GUST>(e, cmd, a.trace != nullptr, 0);      // call 0: no gust stage
@@ -594,10 +609,14 @@ static __device__ __forceinline__ void env_reset(Env& e, const RolloutArgs& a, i
 // starts (the native step output of the previous step, or of reset()'s step: in the sensor-noise builds it carries the
 // noise, as the reference's env.x does), accumulated in step order in fp64
 // PER_ACTOR: env_mode holds one row per (actor, env); the replay row's V0 comes from the actor's own replay_env row
-template <bool STAB = false, bool GUST = false, bool TRACK = false, bool PER_ACTOR = false>
-static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, size_t traj, int actor, bool replay, const float* a, float* obs)
+// INC: incremental control (phlabenv.py:443-466): the scaled action is a rate (bound 25 deg/s, :205-206), integrated as
+// u = last_u + rate * dt in fp64 in the reference's operation order (:377-380; no contraction to fma), u drives the fault
+// shim and the plant, last_u = u, obs[7..9] = (float)u; replay rows of SERL_REPLAY_COLS_OF(10) columns
+template <bool STAB = false, bool GUST = false, bool TRACK = false, bool PER_ACTOR = false, bool INC = false>
+static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, size_t traj, int actor, bool replay, const float* a, float* obs,
+                                                double* last_u = nullptr)
 {
-    const double bound = 10.0 * DEG2RAD;                       // phlabenv.py:208
+    const double bound = INC ? 25.0 * DEG2RAD : 10.0 * DEG2RAD;      // phlabenv.py:205-208
     const double max_theta = 60.0 * DEG2RAD, max_phi = 75.0 * DEG2RAD;
     const double k_err = 6.0 / 3.141592653589793;              // phlabenv.py:226-231
     const double k_err4 = k_err * 4.0;
@@ -608,7 +627,8 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
 #pragma unroll
         for (int i = 0; i < 3; ++i) {
             act_d[i] = fmin(fmax((double)a[i] + (double)nz[i], -1.0), 1.0);
-            U[i] = -bound + 0.5 * (act_d[i] + 1.0) * (bound - (-bound));
+            if constexpr (INC) U[i] = __dadd_rn(-bound, __dmul_rn(0.5 * __dadd_rn(act_d[i], 1.0), bound - (-bound)));
+            else U[i] = -bound + 0.5 * (act_d[i] + 1.0) * (bound - (-bound));
         }
     } else {
         // scale_action: low + 0.5*(a + 1.0)*(high - low) with a float32: (a + 1.0) and the halving round in fp32 (:72-73)
@@ -617,9 +637,13 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
             act_d[i] = (double)a[i];
             const float t1 = __fadd_rn(a[i], 1.0f);
             const float t2 = __fmul_rn(0.5f, t1);
-            U[i] = -bound + (double)t2 * (bound - (-bound));
+            if constexpr (INC) U[i] = __dadd_rn(-bound, __dmul_rn((double)t2, bound - (-bound)));
+            else U[i] = -bound + (double)t2 * (bound - (-bound));
         }
     }
+    if constexpr (INC)
+#pragma unroll
+        for (int i = 0; i < 3; ++i) U[i] = __dadd_rn(last_u[i], __dmul_rn(U[i], 0.01));
     // a NaN action would be squashed to a bound by the plant's input saturation (as in the reference binary): report it
     if (ar.status && !isfinite(act_d[0] + act_d[1] + act_d[2])) atomicOr(ar.status, SERL_STATUS_NONFINITE);
     apply_fault(e.fault, U, cmd);
@@ -666,19 +690,25 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
         // the transition Agent.evaluate stores (agent.py:101-112) + the cost flag of get_cost (phlabenv.py:369-375,
         // including its degrees-vs-radians comparison on the bank angle).  The same test as step_cost, spelt out: calling
         // it here changes the code of the instantiations without TRACK
-        float* rp = ar.replay + ((size_t)actor * ar.horizon + e.k) * SERL_REPLAY_COLS;
+        constexpr int S = INC ? 10 : 7;
+        float* rp = ar.replay + ((size_t)actor * ar.horizon + e.k) * SERL_REPLAY_COLS_OF(S);
 #pragma unroll
-        for (int i = 0; i < 7; ++i) rp[i] = obs[i];
-        rp[7] = (float)act_d[0]; rp[8] = (float)act_d[1]; rp[9] = (float)act_d[2];
-        rp[10] = o0; rp[11] = o1; rp[12] = o2; rp[13] = o3; rp[14] = o4; rp[15] = o5; rp[16] = o6;
-        rp[17] = (float)reward;
-        rp[18] = done ? 1.f : 0.f;
+        for (int i = 0; i < S; ++i) rp[i] = obs[i];
+        rp[S] = (float)act_d[0]; rp[S + 1] = (float)act_d[1]; rp[S + 2] = (float)act_d[2];
+        float* rn = rp + S + 3;
+        rn[0] = o0; rn[1] = o1; rn[2] = o2; rn[3] = o3; rn[4] = o4; rn[5] = o5; rn[6] = o6;
+        if constexpr (INC) { rn[7] = (float)U[0]; rn[8] = (float)U[1]; rn[9] = (float)U[2]; }
+        rn[S] = (float)reward;
+        rn[S + 1] = done ? 1.f : 0.f;
         const int* modes = PER_ACTOR ? ar.env_mode + (size_t)actor * ar.n_envs : ar.env_mode;
         const double v0 = plant_ic(modes[ar.replay_env] & 0xff)[3];
         const bool cost = (fabs(xo[4]) * RAD2DEG > 11.0) || (fabs(xo[6]) * RAD2DEG > 0.75 * max_phi) || (xo[3] < v0 / 3.0);
-        rp[19] = cost ? 1.f : 0.f;
+        rn[S + 2] = cost ? 1.f : 0.f;
     }
     obs[0] = o0; obs[1] = o1; obs[2] = o2; obs[3] = o3; obs[4] = o4; obs[5] = o5; obs[6] = o6;
+    if constexpr (INC)
+#pragma unroll
+        for (int i = 0; i < 3; ++i) { last_u[i] = U[i]; obs[7 + i] = (float)U[i]; }
     e.t = t + 0.01;
     e.k += 1;
     e.done = done || (e.k >= ar.horizon);

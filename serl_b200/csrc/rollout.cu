@@ -104,11 +104,14 @@ __device__ void actor_forward_simple(const float* __restrict__ w, const serl_act
 // deviations.  Element-wise arithmetic is written on float2 pairs of two envs of one neuron (am_fma2: two independent
 // IEEE-rn fmas), and an activation call takes the group's eight envs of one neuron.
 __host__ __device__ constexpr int actor_xbuf_floats(int H) { return H / 4 * 32; }    // exchange buffer per warp: a quarter x 32 envs
+// ... and for an observation of S entries, which the input layer stages there too (S = 10 exceeds a quarter at h = 32)
+__host__ __device__ constexpr int actor_xbuf_floats(int H, int S) { return (H / 4 > S ? H / 4 : S) * 32; }
 
 // Offset of element (source row k, output neuron n) of a transposed [R][H] matrix in the kernel layout: rows in pairs, a
 // pair a block of 2H floats in which lane og's 2·T8 weights (row k's T8, then row k+1's) are its N4 float4 (at
 // 16-byte chunk i: all eight lanes' chunk i side by side, so that an LDS.128 of the warp touches 128 contiguous bytes)
-// and, for odd T8, one float2 after the chunks.  An odd last row (the observation layer: R = 7) is a plain row.
+// and, for odd T8, one float2 after the chunks.  An odd last row (the observation layer: R = 7) is a plain row; the
+// incremental-control observation (R = 10) is five pairs.
 __host__ __device__ constexpr int pair_layout_index(int k, int n, int R, int H)
 {
     const int T8 = H / 8, N4 = T8 / 2 * 4;                 // floats of a lane's pair weights in float4 chunks
@@ -253,16 +256,18 @@ __device__ __forceinline__ void quarter_totals(F f, int og, float (&tot)[2])
 __device__ __forceinline__ int quarter_src_lane(int g, int c) { return g * 8 + 1 + ((c >> 2) & 1) * 2 + ((c >> 1) & 1) * 4; }
 
 // observation in, action out: by value (registers) rather than through pointers, which put them in local memory
-struct ActorObs { float v[7]; };
+template <int S> struct ActorObs { float v[S]; };     // S = 7, or 10 with incremental control (+ last_u)
 struct ActorAct { float v[3]; };
 
-// xb: this warp's exchange buffer, actor_xbuf_floats(H) floats in shared memory, 16-byte aligned
-template <int H, int ACT>
-__device__ __noinline__ ActorAct actor_forward_warp(const float* __restrict__ w, int L, int lane, float* xb, ActorObs obs)
+// xb: this warp's exchange buffer, actor_xbuf_floats(H) floats in shared memory (actor_xbuf_floats(H, 10) for S = 10),
+// 16-byte aligned.  The observation layer sums its S inputs with fma from 0 in index order, then adds the bias (the
+// kernel-order specification)
+template <int H, int ACT, int S = 7>
+__device__ __noinline__ ActorAct actor_forward_warp(const float* __restrict__ w, int L, int lane, float* xb, ActorObs<S> obs)
 {
     constexpr int TM = H / 4, T8 = H / 8;
-    constexpr int S = 7, A = 3;
-    static_assert(TM >= S, "the observation rows fit the exchange buffer");
+    constexpr int A = 3;
+    static_assert(S == 10 || TM >= S, "the observation rows fit the exchange buffer");
     const int og = lane & 7, g = lane >> 3, n0 = og * T8;
     const float* Wt0 = w;
     const float* b0 = Wt0 + S * H;
@@ -354,17 +359,17 @@ __device__ __noinline__ ActorAct actor_forward_warp(const float* __restrict__ w,
 }
 
 // one instantiation per activation: the choice is compiled into the 4 x h/4 activation calls of every layer
-template <int H>
-__device__ __forceinline__ void actor_forward(int act, const float* __restrict__ w, int L, int lane, float* xb, const float (&obs)[7],
+template <int H, int S>
+__device__ __forceinline__ void actor_forward(int act, const float* __restrict__ w, int L, int lane, float* xb, const float (&obs)[S],
                                               float (&a)[3])
 {
-    ActorObs o;
+    ActorObs<S> o;
 #pragma unroll
-    for (int k = 0; k < 7; ++k) o.v[k] = obs[k];
+    for (int k = 0; k < S; ++k) o.v[k] = obs[k];
     ActorAct r;
-    if (act == SERL_ACT_TANH) r = actor_forward_warp<H, SERL_ACT_TANH>(w, L, lane, xb, o);
-    else if (act == SERL_ACT_ELU) r = actor_forward_warp<H, SERL_ACT_ELU>(w, L, lane, xb, o);
-    else r = actor_forward_warp<H, SERL_ACT_LEAKY_RELU>(w, L, lane, xb, o);
+    if (act == SERL_ACT_TANH) r = actor_forward_warp<H, SERL_ACT_TANH, S>(w, L, lane, xb, o);
+    else if (act == SERL_ACT_ELU) r = actor_forward_warp<H, SERL_ACT_ELU, S>(w, L, lane, xb, o);
+    else r = actor_forward_warp<H, SERL_ACT_LEAKY_RELU, S>(w, L, lane, xb, o);
 #pragma unroll
     for (int j = 0; j < 3; ++j) a[j] = r.v[j];
 }
@@ -421,7 +426,9 @@ __global__ void genome_layout_kernel(const float* __restrict__ w, float* __restr
 // PER_ACTOR: every actor flies its own env block (SERL_ROLLOUT_PER_ACTOR_REFS): env `env` of actor `actor` binds row
 // actor * n_envs + env of env_mode / ref_levels / ref_starts, also when a slot resumes it from a hand-over record
 // (instantiated without TRACK, with both GUST values)
-template <int H, bool TABS, bool GUST, bool TRACK = false, bool PER_ACTOR = false>
+// INC: incremental control (SERL_ROLLOUT_INCREMENTAL; instantiated without GUST and TRACK): a 10-entry observation and the
+// env's last_u, both carried in the hand-over records too (OBS_DIM: plant_env.cuh).
+template <int H, bool TABS, bool GUST, bool TRACK = false, bool PER_ACTOR = false, bool INC = false>
 __global__ void __launch_bounds__(MAX_CTA_THREADS, 1)
 rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
 {
@@ -451,7 +458,7 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
     }
     __syncthreads();
     float* w = wbase + (size_t)slot_l * ar.P4;
-    float* xb = wbase + (size_t)ar.apc * ar.P4 + warp * actor_xbuf_floats(H);     // after the genomes of all slots
+    float* xb = wbase + (size_t)ar.apc * ar.P4 + warp * (INC ? actor_xbuf_floats(H, OBS_DIM<INC>) : actor_xbuf_floats(H));     // after the genomes
     const int slot_threads = wps * 32;
     const int actfn = ar.sh.activation;
     const int horizon = ar.horizon;
@@ -487,7 +494,9 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
     Env e;
     e.tab = tab;
     e.done = true; e.k = 0;
-    float obs[7], a[3];
+    float obs[OBS_DIM<INC>], a[3];
+    double last_u[3];                                  // INC only
+    double* const ho_u = INC ? reinterpret_cast<double*>(ar.ho.obs + (size_t)OBS_DIM<INC> * ar.ho.n) : nullptr;
     bool in_seg = false, pending = false, to_h = false, valid = false, replay = false;
     int ke = 0, actor = 0;
     size_t traj = 0;
@@ -513,7 +522,10 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
                         for (int i = 0; i < NX; ++i) __stcg(ar.ho.X + (size_t)i * ar.ho.n + hx, e.X[i]);
                         __stcg(ar.ho.t + hx, e.t); __stcg(ar.ho.ret + hx, e.ret);
 #pragma unroll
-                        for (int i = 0; i < 7; ++i) __stcg(ar.ho.obs + (size_t)i * ar.ho.n + hx, obs[i]);
+                        for (int i = 0; i < OBS_DIM<INC>; ++i) __stcg(ar.ho.obs + (size_t)i * ar.ho.n + hx, obs[i]);
+                        if constexpr (INC)
+#pragma unroll
+                            for (int i = 0; i < 3; ++i) __stcg(ho_u + (size_t)i * ar.ho.n + hx, last_u[i]);
                         __stcg(ar.ho.k + hx, e.k | ((e.done ? 1 : 0) << 30));
                         if constexpr (TRACK)
 #pragma unroll
@@ -589,17 +601,20 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
                         for (int i = 0; i < NX; ++i) e.X[i] = __ldcg(ar.ho.X + (size_t)i * ar.ho.n + hx);
                         e.t = __ldcg(ar.ho.t + hx); e.ret = __ldcg(ar.ho.ret + hx);
 #pragma unroll
-                        for (int i = 0; i < 7; ++i) obs[i] = __ldcg(ar.ho.obs + (size_t)i * ar.ho.n + hx);
+                        for (int i = 0; i < OBS_DIM<INC>; ++i) obs[i] = __ldcg(ar.ho.obs + (size_t)i * ar.ho.n + hx);
+                        if constexpr (INC)
+#pragma unroll
+                            for (int i = 0; i < 3; ++i) last_u[i] = __ldcg(ho_u + (size_t)i * ar.ho.n + hx);
                         const int kk = __ldcg(ar.ho.k + hx);
                         e.k = kk & 0x3fffffff; e.done = ((kk >> 30) & 1) != 0;
                         if constexpr (TRACK)
 #pragma unroll
                             for (int i = 0; i < TRACK_CARRY; ++i) e.trk[i] = __ldcg(tk.ho + (size_t)i * ar.ho.n + hx);
                     } else {
-                        env_reset<TABS, GUST, TRACK>(e, ar, row, obs, traj);
+                        env_reset<TABS, GUST, TRACK, INC>(e, ar, row, obs, traj, last_u);
                     }
                 } else {
-                    env_idle(e, ar, pv_base, obs);
+                    env_idle<INC>(e, ar, pv_base, obs, last_u);
                 }
                 replay = valid && ar.replay != nullptr && env == ar.replay_env;
                 in_seg = true;
@@ -610,14 +625,15 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
         if (!__syncthreads_or(in_seg || pending || stage < 3)) break;
         const bool mine = in_seg && !e.done && e.k < ke;
         if (actor_half && __any_sync(0xffffffffu, mine)) actor_forward<H>(actfn, w, L, lane, xb, obs, a);
-        if ((!stagger || !actor_half) && mine) env_step<TABS, GUST, TRACK, PER_ACTOR>(e, ar, traj, actor, replay, a, obs);
+        if ((!stagger || !actor_half) && mine) env_step<TABS, GUST, TRACK, PER_ACTOR, INC>(e, ar, traj, actor, replay, a, obs, last_u);
         actor_half ^= stagger;
     }
 }
 
 // ---- cross-check kernel: every thread evaluates the whole MLP for its own env (any hidden size that fits) ------
 // PER_ACTOR as in rollout_kernel_persist
-template <bool TRACK = false, bool PER_ACTOR = false>
+// INC as in rollout_kernel_persist (instantiated without TRACK)
+template <bool TRACK = false, bool PER_ACTOR = false, bool INC = false>
 __global__ void __launch_bounds__(128)
 rollout_kernel_simple(RolloutArgs ar, TrackArgs tk)
 {
@@ -635,22 +651,24 @@ rollout_kernel_simple(RolloutArgs ar, TrackArgs tk)
     const int env = ar.env_order ? ar.env_order[eslot] : eslot;
     Env e;
     e.tab = plant_tables_blob;
-    float obs[7], a[3];
+    float obs[INC ? 10 : 7], a[3];
+    double last_u[3];                                  // INC only
     const int row = PER_ACTOR ? actor * ar.n_envs + env : env;
     env_bind<true>(e, ar, row, &plant_pv[0][0], (size_t)actor * ar.n_envs + env);
-    env_reset<false, true, TRACK>(e, ar, row, obs, (size_t)actor * ar.n_envs + env);
+    env_reset<false, true, TRACK, INC>(e, ar, row, obs, (size_t)actor * ar.n_envs + env, last_u);
     const size_t traj = (size_t)actor * ar.n_envs + env;
     const bool replay = ar.replay != nullptr && env == ar.replay_env;
     while (!e.done) {
         actor_forward_simple(w, ar.sh, bufA, bufB, tid, 128, obs, a);
-        env_step<false, true, TRACK, PER_ACTOR>(e, ar, traj, actor, replay, a, obs);       // (the gust schedule costs nothing that matters here)
+        env_step<false, true, TRACK, PER_ACTOR, INC>(e, ar, traj, actor, replay, a, obs, last_u);   // (the gust schedule costs nothing that matters here)
     }
     traj_store(e, ar, traj);
     if constexpr (TRACK) track_store(e, tk, traj);
 }
 
 // ---- Actor.forward for a batch of observations (same device functions as the rollout) --------------------------
-template <int H>
+// S: observation entries (7, or 10 with incremental control)
+template <int H, int S = 7>
 __global__ void __launch_bounds__(128)
 actor_forward_kernel(const float* __restrict__ genome, int P, serl_actor_shape sh, const float* __restrict__ obs_in, int n,
                      float* __restrict__ act_out)
@@ -658,19 +676,20 @@ actor_forward_kernel(const float* __restrict__ genome, int P, serl_actor_shape s
     extern __shared__ __align__(128) unsigned char smem_raw[];
     float* w = reinterpret_cast<float*>(smem_raw);
     const int tid = threadIdx.x, lane = tid & 31;
-    float* xb = w + ((P + 3) & ~3) + (tid >> 5) * actor_xbuf_floats(H);      // after the genome
+    float* xb = w + ((P + 3) & ~3) + (tid >> 5) * (S == 7 ? actor_xbuf_floats(H) : actor_xbuf_floats(H, S));      // after the genome
     for (int i = tid; i < P; i += 128) w[genome_layout_index(i, sh.state_dim, H, sh.num_layers)] = genome[i];
     __syncthreads();
     const int base = (blockIdx.x * 128 + (tid & ~31));
     if (base >= n) return;
     const int i = base + lane;
-    float obs[7], a[3];
+    float obs[S], a[3];
 #pragma unroll
-    for (int k = 0; k < 7; ++k) obs[k] = i < n ? obs_in[(size_t)i * 7 + k] : 0.f;
+    for (int k = 0; k < S; ++k) obs[k] = i < n ? obs_in[(size_t)i * S + k] : 0.f;
     actor_forward<H>(sh.activation, w, sh.num_layers, lane, xb, obs, a);
     if (i < n) { act_out[(size_t)i * 3] = a[0]; act_out[(size_t)i * 3 + 1] = a[1]; act_out[(size_t)i * 3 + 2] = a[2]; }
 }
 
+template <int S = 7>
 __global__ void __launch_bounds__(128)
 actor_forward_kernel_simple(const float* __restrict__ genome, int P, serl_actor_shape sh, const float* __restrict__ obs_in, int n,
                             float* __restrict__ act_out)
@@ -684,8 +703,8 @@ actor_forward_kernel_simple(const float* __restrict__ genome, int P, serl_actor_
     __syncthreads();
     const int i = blockIdx.x * 128 + tid;
     if (i >= n) return;
-    float obs[7], a[3];
-    for (int k = 0; k < 7; ++k) obs[k] = obs_in[(size_t)i * 7 + k];
+    float obs[S], a[3];
+    for (int k = 0; k < S; ++k) obs[k] = obs_in[(size_t)i * S + k];
     actor_forward_simple(w, sh, bufA, bufB, tid, 128, obs, a);
     act_out[(size_t)i * 3] = a[0]; act_out[(size_t)i * 3 + 1] = a[1]; act_out[(size_t)i * 3 + 2] = a[2];
 }
@@ -770,10 +789,10 @@ static bool force_simple()
     return v;
 }
 
-// the uniform actors of the PH-LAB attitude task the kernels of this file implement
+// the uniform actors of the PH-LAB attitude task the kernels of this file implement (state_dim 10: incremental control)
 static bool actor_shape_ok(const serl_actor_shape& sh)
 {
-    return sh.state_dim == 7 && sh.action_dim == 3 && sh.hidden >= 2 && sh.hidden <= 256 && sh.num_layers >= 0 &&
+    return (sh.state_dim == 7 || sh.state_dim == 10) && sh.action_dim == 3 && sh.hidden >= 2 && sh.hidden <= 256 && sh.num_layers >= 0 &&
            sh.activation >= 0 && sh.activation <= 2;
 }
 
@@ -804,7 +823,7 @@ static void choose_shape(int pop, int n_envs, int apc_max, int sms, int* apc_out
 }
 
 template <int H, bool TABS>
-static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust, bool stagger, bool per_actor, cudaStream_t s)
+static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust, bool stagger, bool per_actor, bool inc, cudaStream_t s)
 {
     const int sms = ar.sm_limit > 0 && ar.sm_limit < serl_device_sms() ? ar.sm_limit : serl_device_sms();
     int apc, wps;
@@ -823,7 +842,9 @@ static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust,
     // scratch: genomes in the shared-memory layout + hand-over records of the time-split schedule (stream-ordered)
     const size_t wt_bytes = (size_t)ar.pop * ar.P4 * 4;
     const long long hn = ar.n_tasks > ar.n_slots ? ar.n_slots * wps * 32 : 0;
-    const size_t ho_bytes = (size_t)hn * (NX * 8 + 8 + 8 + 7 * 4 + 4) + (size_t)(hn / 32) * 4 + (tk.out ? (size_t)hn * TRACK_CARRY * 8 + 8 : 0);
+    // a record's observation: 7 floats, or 10 floats and last_u (3 f64) with incremental control (Handoff.obs)
+    const size_t ho_obs = inc ? 10 * 4 + 3 * 8 : 7 * 4;
+    const size_t ho_bytes = (size_t)hn * (NX * 8 + 8 + 8 + ho_obs + 4) + (size_t)(hn / 32) * 4 + (tk.out ? (size_t)hn * TRACK_CARRY * 8 + 8 : 0);
     void* scratch = nullptr;
     cudaError_t e = serl_scratch(SERL_SCRATCH_K1, s, wt_bytes + ho_bytes + 512, &scratch);
     if (e != cudaSuccess) return serl_fail_cuda(e, "rollout_kernel launch");
@@ -836,7 +857,7 @@ static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust,
         ar.ho.X = (double*)p; p += (size_t)hn * NX * 8;
         ar.ho.t = (double*)p; p += (size_t)hn * 8;
         ar.ho.ret = (double*)p; p += (size_t)hn * 8;
-        ar.ho.obs = (float*)p; p += (size_t)hn * 7 * 4;
+        ar.ho.obs = (float*)p; p += (size_t)hn * ho_obs;
         ar.ho.k = (int*)p; p += (size_t)hn * 4;
         ar.ho.flag = (int*)p; p += (size_t)(hn / 32) * 4;
         if (tk.out) tk.ho = (double*)(((uintptr_t)p + 7) & ~(uintptr_t)7);
@@ -849,9 +870,10 @@ static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust,
                                ar.sh.state_dim, H, ar.sh.num_layers);
     if (rc != SERL_OK) return rc;
     const size_t smem = (TABS ? (size_t)PLANT_TABN2 * sizeof(real) : 0) + (size_t)apc * ar.P4 * 4 +
-                        (size_t)apc * wps * actor_xbuf_floats(H) * 4;
+                        (size_t)apc * wps * (inc ? actor_xbuf_floats(H, 10) : actor_xbuf_floats(H)) * 4;
     void (*const kernel)(RolloutArgs, TrackArgs) =
-        tk.out      ? rollout_kernel_persist<H, TABS, true, true>
+        inc         ? (per_actor ? rollout_kernel_persist<H, TABS, false, false, true, true> : rollout_kernel_persist<H, TABS, false, false, false, true>)
+        : tk.out    ? rollout_kernel_persist<H, TABS, true, true>
         : per_actor ? (gust ? rollout_kernel_persist<H, TABS, true, false, true> : rollout_kernel_persist<H, TABS, false, false, true>)
         : gust      ? rollout_kernel_persist<H, TABS, true> : rollout_kernel_persist<H, TABS, false>;
     return serl_launch("rollout_kernel launch", kernel, (unsigned)grid, apc * wps * 32, smem, s, ar, tk);
@@ -881,7 +903,8 @@ constexpr size_t K1_TAB_BYTES = (size_t)PLANT_TABN2 * sizeof(real);
 static size_t k1_slot_bytes(const serl_actor_shape& sh)
 {
     const size_t P4 = ((size_t)serl_actor_num_params(&sh) + 3) & ~(size_t)3;
-    return P4 * 4 + 4ull * actor_xbuf_floats(sh.hidden) * 4;        // h = 128, L = 3: 218 KB
+    const int xb = sh.state_dim == 10 ? actor_xbuf_floats(sh.hidden, 10) : actor_xbuf_floats(sh.hidden);
+    return P4 * 4 + 4ull * xb * 4;        // h = 128, L = 3: 218 KB
 }
 
 // K1's kernel for a valid shape: the warp actor when it can be launched — the hidden size is instantiated and one slot fits
@@ -905,7 +928,7 @@ extern "C" int32_t serl_actor_tc_widths(const serl_actor_shape* shape, int32_t* 
 {
     if (!shape) return serl_fail(SERL_ERR_ARG, "serl_actor_tc_widths: null shape");
     const serl_actor_shape& sh = *shape;
-    const bool task = sh.state_dim == 7 && sh.action_dim == 3 && sh.hidden >= 2 && sh.num_layers >= 1 && sh.activation >= 0 &&
+    const bool task = (sh.state_dim == 7 || sh.state_dim == 10) && sh.action_dim == 3 && sh.hidden >= 2 && sh.num_layers >= 1 && sh.activation >= 0 &&
                       sh.activation <= 2;
     if (!task || (actor_shape_ok(sh) && k1_fits(sh))) return 0;
     const int n = sh.num_layers + 1;
@@ -919,18 +942,19 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
 {
     const TrackArgs tk = {d.d_track, nullptr, d.d_cost};
     if (!actor_shape_ok(d.shape))
-        return serl_fail(SERL_ERR_ARG, "serl_rollout: unsupported actor shape (state_dim = 7, action_dim = 3, 2 <= hidden <= 256)");
+        return serl_fail(SERL_ERR_ARG, "serl_rollout: unsupported actor shape (state_dim = 7 or 10, action_dim = 3, 2 <= hidden <= 256)");
     if (d.pop > 65535) return serl_fail(SERL_ERR_ARG, "serl_rollout: pop must be <= 65535 per call");       // grid.y of the simple kernel
     if (d.horizon >= (1 << 30)) return serl_fail(SERL_ERR_ARG, "serl_rollout: horizon too long");        // Handoff.k: steps | done << 30
     const int H = d.shape.hidden;
-    const bool per_actor = (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) != 0;
+    const bool per_actor = (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) != 0, inc = (d.flags & SERL_ROLLOUT_INCREMENTAL) != 0;
     ar.weights = d.d_weights; ar.P = (int)serl_actor_num_params(&d.shape); ar.sh = d.shape;
     ar.P4 = (ar.P + 3) & ~3;
     if (!k1_warp(d.shape)) {
         if (!k1_fits(d.shape)) return serl_fail(SERL_ERR_UNSUPPORTED, "serl_rollout: genome + activations exceed 227 KB of shared memory");
         const size_t smem = (size_t)ar.P4 * 4 + 2ull * H * 128 * 4;
         return serl_launch("rollout_kernel launch",
-                           d.d_track ? rollout_kernel_simple<true> : per_actor ? rollout_kernel_simple<false, true> : rollout_kernel_simple<false>,
+                           inc         ? (per_actor ? rollout_kernel_simple<false, true, true> : rollout_kernel_simple<false, false, true>)
+                           : d.d_track ? rollout_kernel_simple<true> : per_actor ? rollout_kernel_simple<false, true> : rollout_kernel_simple<false>,
                            dim3((d.n_envs + 127) / 128, d.pop), 128, smem, s, ar, tk);
     }
     // as many genome slots per CTA as shared memory holds next to the plant tables (L = 3: two for h <= 72, one for h = 96);
@@ -945,10 +969,10 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
     warp_hidden(H, [&](auto h) {
         constexpr int HH = decltype(h)::value;
         if constexpr (HH == 128)          // the one size instantiated with the tables in global memory too
-            rc = tabs ? launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, per_actor, s)
-                      : launch_persist<HH, false>(ar, tk, apc_max, gust, stagger, per_actor, s);
+            rc = tabs ? launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, per_actor, inc, s)
+                      : launch_persist<HH, false>(ar, tk, apc_max, gust, stagger, per_actor, inc, s);
         else
-            rc = launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, per_actor, s);
+            rc = launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, per_actor, inc, s);
     });
     return rc;
 }
@@ -972,6 +996,15 @@ static int check_desc(const serl_rollout_desc& d)
         if (d.d_env_order) return serl_fail(SERL_ERR_ARG, "serl_rollout: SERL_ROLLOUT_PER_ACTOR_REFS does not take d_env_order");
         if (d.d_track) return serl_fail(SERL_ERR_ARG, "serl_rollout: SERL_ROLLOUT_PER_ACTOR_REFS does not take d_track");
         if ((int64_t)d.pop * d.n_envs > INT32_MAX) return serl_fail(SERL_ERR_ARG, "serl_rollout: pop * n_envs must fit int32 with per-actor refs");
+    }
+    // incremental control: a 10-entry observation, on the training instantiations of K1 and K1-TC only
+    if (d.flags & SERL_ROLLOUT_INCREMENTAL) {
+        if (d.shape.state_dim != 10) return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) needs state_dim = 10");
+        if (d.d_track || d.d_cost) return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) does not take d_track / d_cost");
+        if (d.flags & SERL_ROLLOUT_GUST) return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) does not take SERL_ROLLOUT_GUST");
+        if (d.d_sensor_noise) return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) does not take d_sensor_noise");
+    } else if (d.n_widths == 0 && d.shape.state_dim == 10) {
+        return serl_fail(SERL_ERR_ARG, "serl_rollout: state_dim = 10 is the observation of incremental control: it needs SERL_ROLLOUT_INCREMENTAL");
     }
     return SERL_OK;
 }
@@ -1052,17 +1085,19 @@ extern "C" int serl_actor_forward(const float* d_genome, const serl_actor_shape*
     if (!actor_shape_ok(*shape)) return serl_fail(SERL_ERR_ARG, "serl_actor_forward: unsupported actor shape");
     cudaStream_t s = (cudaStream_t)stream;
     const int P = (int)serl_actor_num_params(shape), H = shape->hidden;
+    const bool inc = shape->state_dim == 10;        // the observation of incremental control
     const int grid = (n + 127) / 128;
     const size_t smem = (size_t)((P + 3) & ~3) * 4;
     int rc = SERL_OK;
-    const size_t warp_smem = smem + 4ull * actor_xbuf_floats(H) * 4;      // genome + the exchange buffers of 4 warps
+    const size_t warp_smem = smem + 4ull * (inc ? actor_xbuf_floats(H, 10) : actor_xbuf_floats(H)) * 4;      // genome + 4 warps' buffers
     const auto warp_launch = [&](auto h) {
-        rc = serl_launch("actor_forward_kernel", actor_forward_kernel<decltype(h)::value>, grid, 128, warp_smem, s, d_genome, P, *shape, d_obs,
-                         n, d_actions);
+        rc = serl_launch("actor_forward_kernel", inc ? actor_forward_kernel<decltype(h)::value, 10> : actor_forward_kernel<decltype(h)::value>,
+                         grid, 128, warp_smem, s, d_genome, P, *shape, d_obs, n, d_actions);
     };
     // the warp kernel when it holds the genome, else the one-thread-per-env kernel (no static shared memory in either)
     if (!force_simple() && warp_smem <= SERL_SMEM_OPTIN && warp_hidden(H, warp_launch)) return rc;
     const size_t sm2 = smem + 2ull * H * 128 * 4;
     if (sm2 > SERL_SMEM_OPTIN) return serl_fail(SERL_ERR_UNSUPPORTED, "serl_actor_forward: genome + activations exceed shared memory");
-    return serl_launch("actor_forward_kernel", actor_forward_kernel_simple, grid, 128, sm2, s, d_genome, P, *shape, d_obs, n, d_actions);
+    return serl_launch("actor_forward_kernel", inc ? actor_forward_kernel_simple<10> : actor_forward_kernel_simple<>, grid, 128, sm2, s, d_genome,
+                       P, *shape, d_obs, n, d_actions);
 }

@@ -72,12 +72,17 @@ __device__ __forceinline__ float rn_tf32(float x)       // round to nearest TF32
     return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
 }
 
-// small block layout (floats): W0p[w0pad][8] (7 weights + bias) | per layer l: b[npad] gamma[npad] beta[npad] |
+// Row width of W0p in the small block and of the group's observations in shared memory: 8 floats for the 7-entry
+// observation, 12 for the 10 of incremental control (SERL_ROLLOUT_INCREMENTAL: + last_u); float4-aligned either way
+__host__ __device__ constexpr int tc_row(int S) { return S == 7 ? 8 : 12; }
+
+// small block layout (floats): W0p[w0pad][8] (7 weights + bias; S = 10: [w0pad][12], 10 weights + bias + 0) | per layer l: b[npad] gamma[npad] beta[npad] |
 // Wo[3][npad of the last layer] | bo[4].  With two widths [w1, w2] this is W0p[w1][8] | b1 | gamma | beta | Wo | bo.
 // Tile block: per layer l, n_stages K-slabs of stage_floats (pre-split TF32 hi / lo, canonical K-major core matrices).
 
-// K0-TC: genome (parameters() order: W0[w0,7] b0[w0], per layer W_l[w_l,w_{l-1}] b gamma beta, Wo[3,w_last] bo[3]) -> small
+// K0-TC: genome (parameters() order: W0[w0,S] b0[w0], per layer W_l[w_l,w_{l-1}] b gamma beta, Wo[3,w_last] bo[3]) -> small
 // block + tile block.  Rows and columns past a layer's real width are zero neurons: zero weights, bias, gamma and beta.
+template <int S = 7>
 __global__ void tc_layout_kernel(const float* __restrict__ w, int pop, int P, const __grid_constant__ TcArgs ar, float* __restrict__ small,
                                  float* __restrict__ tiles)
 {
@@ -91,9 +96,12 @@ __global__ void tc_layout_kernel(const float* __restrict__ w, int pop, int P, co
         const int i = (int)(g - (long long)a * per);
         const float* ga = w + (size_t)a * P;
         float v = 0.f;
-        if (i < w0pad * 8) {
+        if (S == 7 && i < w0pad * 8) {
             const int k = i >> 3, c = i & 7;
             v = k >= w0 ? 0.f : (c < 7 ? ga[k * 7 + c] : ga[7 * w0 + k]);
+        } else if (S != 7 && i < w0pad * tc_row(S)) {
+            const int k = i / tc_row(S), c = i - k * tc_row(S);
+            v = k >= w0 || c > S ? 0.f : (c < S ? ga[k * S + c] : ga[S * w0 + k]);
         } else if (i < wo) {
             int l = 0;
             while (i >= ar.ly[l].vec + 3 * ar.ly[l].npad) ++l;
@@ -192,10 +200,33 @@ __device__ __forceinline__ void tc_release(TcCtx& c)
     }
 }
 
+// layer 0 of neuron row `wr` of W0p (CUDA cores): bias, then fma over the S observation entries in index order
+template <int S>
+__device__ __forceinline__ float tc_layer0(const float* wr, const float (&ob)[S])
+{
+    const float4 wa = *reinterpret_cast<const float4*>(wr);
+    const float4 wb = *reinterpret_cast<const float4*>(wr + 4);
+    if constexpr (S == 7) {
+        float a = wb.w;                                              // bias
+        a = __fmaf_rn(wa.x, ob[0], a); a = __fmaf_rn(wa.y, ob[1], a); a = __fmaf_rn(wa.z, ob[2], a);
+        a = __fmaf_rn(wa.w, ob[3], a); a = __fmaf_rn(wb.x, ob[4], a); a = __fmaf_rn(wb.y, ob[5], a);
+        a = __fmaf_rn(wb.z, ob[6], a);
+        return a;
+    } else {
+        const float4 wc = *reinterpret_cast<const float4*>(wr + 8);
+        float a = wc.z;                                              // bias
+        a = __fmaf_rn(wa.x, ob[0], a); a = __fmaf_rn(wa.y, ob[1], a); a = __fmaf_rn(wa.z, ob[2], a);
+        a = __fmaf_rn(wa.w, ob[3], a); a = __fmaf_rn(wb.x, ob[4], a); a = __fmaf_rn(wb.y, ob[5], a);
+        a = __fmaf_rn(wb.z, ob[6], a); a = __fmaf_rn(wb.w, ob[7], a); a = __fmaf_rn(wc.x, ob[8], a);
+        a = __fmaf_rn(wc.y, ob[9], a);
+        return a;
+    }
+}
+
 // one actor forward for the 128 envs of the group; every thread passes its own observation and receives its own action.
 // The group's rows are done in two halves of TC_M = 64 (the M of one wgmma); each half streams all W1 slabs, so the
 // accumulator of a thread is n2pad / 2 registers.
-template <int ACT>
+template <int ACT, int S = 7>
 __device__ __forceinline__ void tc_actor_forward(TcCtx& c, const TcArgs& ar, const float* tiles_actor, const float* obs, float* action)
 {
     const int tid = c.gtid, warp = tid >> 5, lane = tid & 31;
@@ -205,9 +236,9 @@ __device__ __forceinline__ void tc_actor_forward(TcCtx& c, const TcArgs& ar, con
     constexpr int A_STAGE_FLOATS = 2 * TC_CH * TC_M * 4;                   // hi + lo, TC_CH chunks x 64 rows x 4 floats
     const float* W0p = c.small;
     float* obs_s = c.io;
-    float* act_s = c.io + TC_THREADS * 8;
+    float* act_s = c.io + TC_THREADS * tc_row(S);
 #pragma unroll
-    for (int k = 0; k < 7; ++k) obs_s[tid * 8 + k] = obs[k];
+    for (int k = 0; k < S; ++k) obs_s[tid * tc_row(S) + k] = obs[k];
     tc_acquire(c);                                                         // (its barrier publishes obs_s)
     const uint32_t g0 = c.g;
     // W1 slabs of the first two stages (their slots' MMAs retired before the lock was released)
@@ -219,16 +250,16 @@ __device__ __forceinline__ void tc_actor_forward(TcCtx& c, const TcArgs& ar, con
         }
     }
     const int rr = tid & (TC_M - 1), jj = tid >> 6;                         // layer 1: row rr of the half, K chunk jj of the slab
-    const float* b1 = c.small + ar.w1 * 8;
+    const float* b1 = c.small + ar.w1 * tc_row(S);
     const float* gamma = b1 + n2pad;
     const float* beta = gamma + n2pad;
     const float* Wo = beta + n2pad;
     const float* bo = Wo + 3 * n2pad;
     float acc[TC_MAXN / 2];
     for (int h = 0; h < 2; ++h) {
-        float ob[7];
+        float ob[S];
 #pragma unroll
-        for (int k = 0; k < 7; ++k) ob[k] = obs_s[(h * TC_M + rr) * 8 + k];
+        for (int k = 0; k < S; ++k) ob[k] = obs_s[(h * TC_M + rr) * tc_row(S) + k];
         for (int s = 0; s < n_stages; ++s) {
             const int q = h * n_stages + s;
             const uint32_t g = g0 + q, slot = g % TC_STAGES;
@@ -238,15 +269,7 @@ __device__ __forceinline__ void tc_actor_forward(TcCtx& c, const TcArgs& ar, con
             float* a_lo = a_hi + TC_CH * TC_M * 4;
             float hv[4];
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-                const float4 wa = *reinterpret_cast<const float4*>(W0p + (size_t)(s * TC_KSLAB + jj * 4 + kk) * 8);
-                const float4 wb = *reinterpret_cast<const float4*>(W0p + (size_t)(s * TC_KSLAB + jj * 4 + kk) * 8 + 4);
-                float a = wb.w;                                              // bias
-                a = __fmaf_rn(wa.x, ob[0], a); a = __fmaf_rn(wa.y, ob[1], a); a = __fmaf_rn(wa.z, ob[2], a);
-                a = __fmaf_rn(wa.w, ob[3], a); a = __fmaf_rn(wb.x, ob[4], a); a = __fmaf_rn(wb.y, ob[5], a);
-                a = __fmaf_rn(wb.z, ob[6], a);
-                hv[kk] = a;
-            }
+            for (int kk = 0; kk < 4; ++kk) hv[kk] = tc_layer0<S>(W0p + (size_t)(s * TC_KSLAB + jj * 4 + kk) * tc_row(S), ob);
             const float2 p0 = am_act2<ACT>(make_float2(hv[0], hv[1])), p1 = am_act2<ACT>(make_float2(hv[2], hv[3]));
             const float4 hi = make_float4(rn_tf32(p0.x), rn_tf32(p0.y), rn_tf32(p1.x), rn_tf32(p1.y));
             const float4 lo = make_float4(rn_tf32(p0.x - hi.x), rn_tf32(p0.y - hi.y), rn_tf32(p1.x - hi.z), rn_tf32(p1.y - hi.w));
@@ -424,7 +447,7 @@ __device__ __forceinline__ void tc_fetch_deep(TcCtx& c, const TcArgs& ar, const 
 // activation) writes its rows to the fp32 activation buffer, zero past w_l; layer l+1 then builds each A slab from that
 // buffer (TF32 hi / lo split) instead of from layer 0.  The last layer has the epilogue of tc_actor_forward with the output
 // layer folded in.  The small block is read from global memory (L1).
-template <int ACT>
+template <int ACT, int S = 7>
 __device__ __forceinline__ void tc_actor_forward_deep(TcCtx& c, const TcArgs& ar, const float* tiles_actor, const float* obs, float* action)
 {
     const int tid = c.gtid, warp = tid >> 5, lane = tid & 31;
@@ -432,11 +455,11 @@ __device__ __forceinline__ void tc_actor_forward_deep(TcCtx& c, const TcArgs& ar
     constexpr int A_STAGE_FLOATS = 2 * TC_CH * TC_M * 4;
     const float* W0p = c.small;
     float* obs_s = c.io;
-    float* act_s = c.io + TC_THREADS * 8;
+    float* act_s = c.io + TC_THREADS * tc_row(S);
     float* abuf = c.abuf;
     const int as = ar.abuf_stride;
 #pragma unroll
-    for (int k = 0; k < 7; ++k) obs_s[tid * 8 + k] = obs[k];
+    for (int k = 0; k < S; ++k) obs_s[tid * tc_row(S) + k] = obs[k];
     tc_acquire(c);                                                         // (its barrier publishes obs_s)
     const uint32_t g0 = c.g;
     if (tid == 0)
@@ -446,9 +469,9 @@ __device__ __forceinline__ void tc_actor_forward_deep(TcCtx& c, const TcArgs& ar
     float acc[TC_MAXN / 2];
     int q = 0;
     for (int h = 0; h < 2; ++h) {
-        float ob[7];
+        float ob[S];
 #pragma unroll
-        for (int k = 0; k < 7; ++k) ob[k] = obs_s[(h * TC_M + rr) * 8 + k];
+        for (int k = 0; k < S; ++k) ob[k] = obs_s[(h * TC_M + rr) * tc_row(S) + k];
         for (int l = 0; l < ar.n_layers; ++l) {
             const int npad = ar.ly[l].npad, nch = npad / TC_NCH, w = ar.ly[l].w, n_stages = ar.ly[l].n_stages;
             for (int s = 0; s < n_stages; ++s, ++q) {
@@ -459,15 +482,7 @@ __device__ __forceinline__ void tc_actor_forward_deep(TcCtx& c, const TcArgs& ar
                 if (l == 0) {
                     float hv[4];
 #pragma unroll
-                    for (int kk = 0; kk < 4; ++kk) {
-                        const float4 wa = *reinterpret_cast<const float4*>(W0p + (size_t)(s * TC_KSLAB + jj * 4 + kk) * 8);
-                        const float4 wb = *reinterpret_cast<const float4*>(W0p + (size_t)(s * TC_KSLAB + jj * 4 + kk) * 8 + 4);
-                        float a = wb.w;
-                        a = __fmaf_rn(wa.x, ob[0], a); a = __fmaf_rn(wa.y, ob[1], a); a = __fmaf_rn(wa.z, ob[2], a);
-                        a = __fmaf_rn(wa.w, ob[3], a); a = __fmaf_rn(wb.x, ob[4], a); a = __fmaf_rn(wb.y, ob[5], a);
-                        a = __fmaf_rn(wb.z, ob[6], a);
-                        hv[kk] = a;
-                    }
+                    for (int kk = 0; kk < 4; ++kk) hv[kk] = tc_layer0<S>(W0p + (size_t)(s * TC_KSLAB + jj * 4 + kk) * tc_row(S), ob);
                     const float2 p0 = am_act2<ACT>(make_float2(hv[0], hv[1])), p1 = am_act2<ACT>(make_float2(hv[2], hv[3]));
                     x = make_float4(p0.x, p0.y, p1.x, p1.y);
                 } else {
@@ -576,10 +591,12 @@ __device__ __forceinline__ void tc_actor_forward_deep(TcCtx& c, const TcArgs& ar
 
 constexpr int TC_TABN2 = (PLANT_TABN + 15) & ~15;                       // keeps the float regions 128-byte aligned
 constexpr int TC_IO_FLOATS = TC_THREADS * 12;                           // per group: observations [128][8], actions [128][4]
+// ... for an observation of S entries: observations [128][tc_row(S)], actions [128][4]
+__host__ __device__ constexpr int tc_io_floats(int S) { return S == 7 ? TC_IO_FLOATS : TC_THREADS * (tc_row(S) + 4); }
 
 // dynamic shared memory: plant tables | two small blocks (two widths only) | io of both groups | A ring | B ring |
 // activation buffer (deep lists only)
-template <bool DEEP>
+template <bool DEEP, int S = 7>
 __device__ __forceinline__ void tc_setup(TcCtx& c, const TcArgs& ar, unsigned char* smem_raw, uint64_t* bars, uint32_t* shared_state)
 {
     constexpr int A_STAGE_FLOATS = 2 * TC_CH * TC_M * 4;
@@ -591,8 +608,8 @@ __device__ __forceinline__ void tc_setup(TcCtx& c, const TcArgs& ar, unsigned ch
     c.grp = threadIdx.x >> 7;
     c.gtid = threadIdx.x & (TC_THREADS - 1);
     c.small = f + (size_t)c.grp * small_pad;
-    c.io = f + 2 * (size_t)small_pad + (size_t)c.grp * TC_IO_FLOATS;
-    c.a_ring = f + 2 * (size_t)small_pad + 2 * TC_IO_FLOATS;
+    c.io = f + 2 * (size_t)small_pad + (size_t)c.grp * tc_io_floats(S);
+    c.a_ring = f + 2 * (size_t)small_pad + 2 * tc_io_floats(S);
     c.b_ring = c.a_ring + TC_STAGES * A_STAGE_FLOATS;
     c.abuf = c.b_ring + (size_t)TC_STAGES * ar.stage_floats;
     c.full_b = bars;
@@ -624,8 +641,10 @@ __device__ __forceinline__ void tc_load_small(TcCtx& c, const TcArgs& ar, int ac
 // instance of the kernel; without it a gust env raises SERL_STATUS_GUST_FLAG.  DEEP: more than two widths
 // (tc_actor_forward_deep); the two-width instantiations run tc_actor_forward.  TRACK: the launch writes the tracking-error
 // sums `tk` (serl_rollout_desc.d_track; instantiated with GUST only).  PER_ACTOR: env `env` of actor `actor` binds row
-// actor * n_envs + env of env_mode / ref_levels / ref_starts (SERL_ROLLOUT_PER_ACTOR_REFS; instantiated without TRACK)
-template <int ACT, bool GUST, bool DEEP, bool TRACK = false, bool PER_ACTOR = false>
+// actor * n_envs + env of env_mode / ref_levels / ref_starts (SERL_ROLLOUT_PER_ACTOR_REFS; instantiated without TRACK).
+// INC: incremental control (SERL_ROLLOUT_INCREMENTAL; instantiated without GUST and TRACK): a 10-entry observation, layer 0
+// with 10 inputs, and the env's last_u
+template <int ACT, bool GUST, bool DEEP, bool TRACK = false, bool PER_ACTOR = false, bool INC = false>
 __global__ void __launch_bounds__(2 * TC_THREADS, 1)
 rollout_kernel_tc(const __grid_constant__ TcArgs ar, TrackArgs tk)
 {
@@ -634,7 +653,7 @@ rollout_kernel_tc(const __grid_constant__ TcArgs ar, TrackArgs tk)
     __shared__ uint32_t shared_state[2];
     TcCtx c;
     plant_tab_check(smem_raw);
-    tc_setup<DEEP>(c, ar, smem_raw, bars, shared_state);
+    tc_setup<DEEP, OBS_DIM<INC>>(c, ar, smem_raw, bars, shared_state);
     const RolloutArgs& r = ar.r;
     const real* tab = reinterpret_cast<const real*>(smem_raw);
     const real* pv_base = tab + PT_TOTAL;
@@ -649,20 +668,21 @@ rollout_kernel_tc(const __grid_constant__ TcArgs ar, TrackArgs tk)
         const int env = valid ? (r.env_order ? r.env_order[eslot] : eslot) : 0;
         Env e;
         e.tab = tab;
-        float obs[7], a[3];
+        float obs[OBS_DIM<INC>], a[3];
+        double last_u[3];                              // INC only
         if (valid) {
             const int row = PER_ACTOR ? actor * r.n_envs + env : env;
             env_bind<GUST>(e, r, row, pv_base, (size_t)actor * r.n_envs + env);
-            env_reset<true, GUST, TRACK>(e, r, row, obs, (size_t)actor * r.n_envs + env);
+            env_reset<true, GUST, TRACK, INC>(e, r, row, obs, (size_t)actor * r.n_envs + env, last_u);
         } else {
-            env_idle(e, r, pv_base, obs);
+            env_idle<INC>(e, r, pv_base, obs, last_u);
         }
         const size_t traj = (size_t)actor * r.n_envs + env;
         const bool replay = valid && r.replay != nullptr && env == r.replay_env;
         while (group_any(c.grp, !e.done)) {
-            if constexpr (DEEP) tc_actor_forward_deep<ACT>(c, ar, tiles_actor, obs, a);
-            else tc_actor_forward<ACT>(c, ar, tiles_actor, obs, a);
-            if (!e.done) env_step<true, GUST, TRACK, PER_ACTOR>(e, r, traj, actor, replay, a, obs);
+            if constexpr (DEEP) tc_actor_forward_deep<ACT, OBS_DIM<INC>>(c, ar, tiles_actor, obs, a);
+            else tc_actor_forward<ACT, OBS_DIM<INC>>(c, ar, tiles_actor, obs, a);
+            if (!e.done) env_step<true, GUST, TRACK, PER_ACTOR, INC>(e, r, traj, actor, replay, a, obs, last_u);
         }
         if (valid) traj_store(e, r, traj);
         if constexpr (TRACK) if (valid) track_store(e, tk, traj);
@@ -703,7 +723,9 @@ extern "C" int64_t serl_actor_num_params_wide(const int32_t* widths, int32_t n_w
 
 // Checks the widths and sizes the layer table, the kernel layout and the shared memory (all before any CUDA call), then
 // brings the genomes into the kernel layout (K0-TC) in the stream's scratch buffer.
-static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t* widths, int n_widths, cudaStream_t s, size_t* smem_out)
+// S: observation entries (7, or 10 with incremental control)
+static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t* widths, int n_widths, cudaStream_t s, size_t* smem_out,
+                      int S = 7)
 {
     if (!widths || n_widths < 2 || n_widths > TC_MAXL + 1)
         return serl_fail(SERL_ERR_UNSUPPORTED, "wide actors: the tensor-core path takes 2 to 9 widths [w0, w1, ..., w_{n-1}]");
@@ -715,7 +737,7 @@ static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t
     ar.w1 = pad(widths[0], TC_KSLAB);
     ar.w2 = widths[1]; ar.n2pad = pad(widths[1], TC_NCH);
     ar.n_layers = n_widths - 1;
-    int vec = ar.w1 * 8, tile = 0, gW = 8 * widths[0], kmax = 0;
+    int vec = ar.w1 * tc_row(S), tile = 0, gW = (S + 1) * widths[0], kmax = 0;
     ar.stages = 0; ar.stage_floats = 0;
     for (int l = 0; l < ar.n_layers; ++l) {
         TcLayer& L = ar.ly[l];
@@ -739,12 +761,12 @@ static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t
     ar.abuf_stride = deep ? kmax + 4 : 0;
     constexpr int A_STAGE_FLOATS = 2 * TC_CH * TC_M * 4;
     *smem_out = (size_t)TC_TABN2 * sizeof(real) +
-                (size_t)(2 * (deep ? 0 : (ar.small_floats + 31) & ~31) + 2 * TC_IO_FLOATS + TC_STAGES * A_STAGE_FLOATS +
+                (size_t)(2 * (deep ? 0 : (ar.small_floats + 31) & ~31) + 2 * tc_io_floats(S) + TC_STAGES * A_STAGE_FLOATS +
                          TC_STAGES * ar.stage_floats + TC_M * ar.abuf_stride) * 4;
     if (*smem_out > SERL_SMEM_OPTIN - 256)
         return serl_fail(SERL_ERR_UNSUPPORTED, deep ? "wide actors: tables + rings + activation buffer exceed the shared memory of an SM"
                                                     : "wide actors: tables + parameters + rings exceed the shared memory of an SM");
-    const int P = (int)serl_actor_num_params_wide(widths, n_widths);
+    const int P = (int)serl_actor_num_params_wide(widths, n_widths) + (S - 7) * widths[0];
     const size_t small_bytes = (size_t)pop * ar.small_floats * 4;
     const size_t tile_bytes = (size_t)pop * ar.tile_floats * 4;
     void* scratch = nullptr;
@@ -755,7 +777,8 @@ static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t
     ar.small = small; ar.tiles = tiles;
     const long long total = (long long)pop * ((long long)ar.small_floats + ar.tile_floats);
     const int grid = (int)((total + 255) / 256 < 8192 ? (total + 255) / 256 : 8192);
-    return serl_launch("tc_layout_kernel", tc_layout_kernel, grid, 256, 0, s, d_weights, pop, P, ar, small, tiles);
+    return serl_launch("tc_layout_kernel", S == 7 ? tc_layout_kernel<7> : tc_layout_kernel<10>, grid, 256, 0, s, d_weights, pop, P, ar,
+                       small, tiles);
 }
 
 // K1-TC launch (serl_rollout_run has checked the descriptor and built the env / output arguments `r`)
@@ -765,7 +788,8 @@ int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, cudaStream
     memset(&ar, 0, sizeof(ar));
     ar.r = r;
     size_t smem = 0;
-    const int rc = tc_prepare(ar, d.d_weights, d.pop, d.widths, d.n_widths, s, &smem);
+    const bool inc = (d.flags & SERL_ROLLOUT_INCREMENTAL) != 0;
+    const int rc = tc_prepare(ar, d.d_weights, d.pop, d.widths, d.n_widths, s, &smem, inc ? 10 : 7);
     if (rc != SERL_OK) return rc;
     ar.n_chunks = (d.n_envs + TC_THREADS - 1) / TC_THREADS;
     ar.n_tasks = (long long)d.pop * ar.n_chunks;
@@ -790,10 +814,19 @@ int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, cudaStream
          {rollout_kernel_tc<SERL_ACT_ELU, true, false, false, true>, rollout_kernel_tc<SERL_ACT_ELU, true, true, false, true>}},
         {{rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, true>},
          {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, false, false, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, true, false, true>}}};
+    static void (*const inc_kernels[3][2][2])(TcArgs, TrackArgs) = {   // [SERL_ACT_*][per actor][deep]
+        {{rollout_kernel_tc<SERL_ACT_TANH, false, false, false, false, true>, rollout_kernel_tc<SERL_ACT_TANH, false, true, false, false, true>},
+         {rollout_kernel_tc<SERL_ACT_TANH, false, false, false, true, true>, rollout_kernel_tc<SERL_ACT_TANH, false, true, false, true, true>}},
+        {{rollout_kernel_tc<SERL_ACT_ELU, false, false, false, false, true>, rollout_kernel_tc<SERL_ACT_ELU, false, true, false, false, true>},
+         {rollout_kernel_tc<SERL_ACT_ELU, false, false, false, true, true>, rollout_kernel_tc<SERL_ACT_ELU, false, true, false, true, true>}},
+        {{rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, false, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, false, true>},
+         {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, true, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, true, true>}}};
     const TrackArgs tk = {d.d_track, nullptr, d.d_cost};
     const bool gust = (d.flags & SERL_ROLLOUT_GUST) != 0, deep = ar.n_layers > 1;
+    const bool per_actor = (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) != 0;
     // one CTA = the two groups of TC_THREADS threads
-    return serl_launch("rollout_kernel_tc launch", d.d_track ? track_kernels[d.shape.activation][deep]
+    return serl_launch("rollout_kernel_tc launch", inc ? inc_kernels[d.shape.activation][per_actor][deep]
+                                                   : d.d_track ? track_kernels[d.shape.activation][deep]
                                                    : (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) ? per_actor_kernels[d.shape.activation][gust][deep]
                                                                                              : kernels[d.shape.activation][gust][deep],
                        (unsigned)grid, 2 * TC_THREADS, smem, s, ar, tk);

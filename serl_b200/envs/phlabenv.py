@@ -43,7 +43,10 @@ class CitationEnv:
         self.n_actions = 3
         self.obs_idx = [0, 1, 2, 4]
         m = mode.lower()
-        if m == '' or m == 'nominal' or 'h2000-v90' in m:
+        # incremental control (:174-175): any mode containing 'incremental' flies the nominal build, the first test of the
+        # reference's chain (:99-103), so 'gust-incremental' has no gust and 'noise-incremental' no sensor noise
+        self.incremental = 'incremental' in m
+        if m == '' or m == 'nominal' or 'h2000-v90' in m or self.incremental:
             m = 'nominal'
         alias = {'high-q': 'h2000-v150', 'low-q': 'h10000-v90', 'cg-aft': 'cg', 'cg-shift': 'cg-timed'}
         m = alias.get(m, m)
@@ -64,10 +67,11 @@ class CitationEnv:
         self.x = self.obs = self.last_obs = self.V0 = self.last_u = None
         self.ref = self.ref_values = None
         self.theta_trim = 0.22
-        self.bound = np.deg2rad(10)
+        self.bound = np.deg2rad(25) if self.incremental else np.deg2rad(10)     # a rate [rad/s] in incremental control (:205-208)
         self.max_theta = np.deg2rad(60.)
         self.max_phi = np.deg2rad(75.)
-        self.n_obs = len(self.obs_idx) + self.n_actions
+        # incremental control: + the actuator state last_u (:214-220)
+        self.n_obs = len(self.obs_idx) + (2 if self.incremental else 1) * self.n_actions
         self.error = np.zeros((self.n_actions))
         self.error_scaler = (6 / np.pi * np.array([1., 1., 4.]))[:self.n_actions]
         self.max_bound = np.ones(self.error.shape)
@@ -190,6 +194,8 @@ class CitationEnv:
         self.init_ref(**kwargs)
         self.obs = np.hstack((self.error.flatten(), self.x[self.obs_idx]))     # stale error, as in the reference (:422)
         self.last_obs = self.obs[:]
+        if self.incremental:
+            self.obs = np.hstack((self.obs, self.last_u))
         return self.obs
 
     def calc_reference_value(self):
@@ -211,14 +217,22 @@ class CitationEnv:
             return True, -1 / self.dt * (self.t_max - self.t) * 2
         return False, 0.
 
+    def incremental_control(self, action):
+        """u = last_u + rate * dt in float64, unclipped (:377-380)"""
+        return self.last_u + action * self.dt
+
     def step(self, action):
         self.last_obs = self.obs
         u = self.scale_action(action)
+        if self.incremental:
+            u = self.incremental_control(u)
         self.x = self._native_step(u)
         reward = self.get_reward()
         cost = self.get_cost()
         self.obs = np.hstack((self.error.flatten(), self.x[self.obs_idx]))
         self.last_u = u
+        if self.incremental:
+            self.obs = np.hstack((self.obs, self.last_u))
         is_done, penalty = self.check_bounds()
         reward += penalty
         self.t += self.dt

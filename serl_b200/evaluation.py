@@ -52,6 +52,8 @@ def condition_env(condition, t_max=T_MAX):
     evaluation mode"""
     from .envs import config
     env = config.select_env(condition if '_' in condition else 'PHlab_attitude_' + condition)
+    if env.incremental:
+        raise ValueError('evaluation: the evaluation suite flies absolute control only, not incremental control (%s)' % condition)
     env.set_eval_mode(t_max)
     return env
 
@@ -180,6 +182,8 @@ def evaluate_population(genomes, shape, conditions, user_refs_lst, num_trails=1,
     state instead, as when base/evaluate.py runs once per condition and reseeds (examples/evaluate.py).  When
     the [N, envs, horizon, 3] fp32 deflection record exceeds `actions_cap` bytes, the actors are flown in chunks of equal
     launches (same results)."""
+    if shape.state_dim == rollout.INCREMENTAL_STATE_DIM:
+        raise ValueError('evaluate_population: the evaluation suite flies absolute control only, not incremental control')
     dev = device or torch.device('cuda', torch.cuda.current_device())
     refs = user_refs_lst[:num_trails + 1]
     T, C = len(refs), len(conditions)

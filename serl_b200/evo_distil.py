@@ -44,11 +44,12 @@ def cloning_loss(child_action, p1_action, p2_action, p1_q, p2_q):
 
 def distil_children(genomes, first, second, buffers, shape, activation, critic, generator=None, epochs=EPOCHS, batch=BATCH):
     """genomes [pop, P]; first / second: parent indices (first = the fitter, mod_neuro_evo.py:509-510) of the C children;
-    buffers: list of C tensors [M_c, >=7] (each child's mixed state buffer).  Returns child genomes [C, P]."""
+    buffers: list of C tensors [M_c, >=S] (each child's mixed state buffer); shape = (S, A, h, L).  Returns child genomes [C, P]."""
     dev = genomes.device
     C = len(first)
+    S = int(shape[0])
     M = min(int(b.shape[0]) for b in buffers)
-    states_all = torch.stack([b[:M, :7] for b in buffers]).to(torch.float32)             # [C, M, 7]
+    states_all = torch.stack([b[:M, :S] for b in buffers]).to(torch.float32)             # [C, M, S]
     i1 = torch.as_tensor(first, dtype=torch.int64, device=dev)
     i2 = torch.as_tensor(second, dtype=torch.int64, device=dev)
     G1, G2 = genomes[i1].detach(), genomes[i2].detach()
@@ -61,11 +62,11 @@ def distil_children(genomes, first, second, buffers, shape, activation, critic, 
     try:
         for _ in range(epochs * iters):
             pick = torch.rand((C, M), device=dev, generator=generator).argsort(dim=1)[:, :bs]      # without replacement
-            st = torch.gather(states_all, 1, pick.unsqueeze(-1).expand(C, bs, 7))
+            st = torch.gather(states_all, 1, pick.unsqueeze(-1).expand(C, bs, S))
             with torch.no_grad():
                 a1 = evo_prox.actor_forward_batched(G1, st, shape, activation)
                 a2 = evo_prox.actor_forward_batched(G2, st, shape, activation)
-                flat = st.reshape(C * bs, 7)
+                flat = st.reshape(C * bs, S)
                 q1a, q1b = critic(flat, a1.reshape(C * bs, -1))
                 q2a, q2b = critic(flat, a2.reshape(C * bs, -1))
                 p1_q = torch.min(q1a, q1b).reshape(C, bs)

@@ -104,6 +104,8 @@ class OperatorRunner:
     for each magnitude in turn."""
 
     def __init__(self, args, condition='nominal', num_trails=0, device=None):
+        if getattr(args, 'state_dim', None) == rollout.INCREMENTAL_STATE_DIM:
+            raise ValueError('OperatorRunner: the operator study flies absolute control only, not incremental control')
         self.args = args
         self.num_trails = int(num_trails)
         self.device = device or torch.device('cuda', torch.cuda.current_device())

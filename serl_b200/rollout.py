@@ -14,8 +14,28 @@ from ._native import FAULTS, MODE_GUST, MODE_GUST_UP, PLANT_VARIANTS, REPLAY_COL
 HORIZON = 2001          # envs/phlabenv.py:82,181,392: t_max = 20 s, dt = 0.01, done checked before t += dt
 # trace record columns (SERL_TRACE_COLS): state before the step, commanded deflection, reward, action fed to the env, error
 TRACE_X, TRACE_U, TRACE_R, TRACE_A, TRACE_ERR = slice(0, 12), slice(12, 15), 15, slice(16, 19), slice(19, 22)
-# replay row (SERL_REPLAY_COLS): the transition obs 7 | action 3 | next_obs 7 | reward | done, then the cost flag
-TRANSITION_COLS = REPLAY_COST = 19
+# the observation of incremental control (envs/phlabenv.py:214-220): the 7 of the absolute mode + last_u.  A shape with this
+# state_dim flies with SERL_ROLLOUT_INCREMENTAL
+INCREMENTAL_STATE_DIM = 10
+
+
+# The replay row of an observation of S entries (SERL_REPLAY_COLS_OF): obs S | action 3 | next_obs S | reward | done | cost.
+# Every buffer stores the transition, the row without its last column (the cost flag).
+def replay_dims(state_dim=7):
+    """widths of the fields of a replay row: obs, action, next_obs, reward, done, cost"""
+    return (state_dim, 3, state_dim, 1, 1, 1)
+
+
+def replay_cols(state_dim=7):
+    return sum(replay_dims(state_dim))
+
+
+def transition_cols(state_dim=7):
+    """columns of a stored transition, which is also the column of a replay row's cost flag"""
+    return replay_cols(state_dim) - 1
+
+
+TRANSITION_COLS = REPLAY_COST = transition_cols(7)       # SERL_REPLAY_COLS - 1
 # time-triggered builds: parameter row the plant switches to when its clock reaches 20 s (envs/phlabenv.py:159-163)
 POST_VARIANT = {'cg_timed': 'cg_timed_post'}
 # env mode string (envs/phlabenv.py:99-172) -> (plant variant, command fault)
@@ -95,6 +115,8 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     (sum |e_theta|, sum |e_phi|, sum |e_beta|, sum e_beta; serl_rollout_desc.d_track), the nMAE of a trajectory without a trace.
     cost=True (with track=True): result.cost [pop, n_envs] int32 holds each trajectory's safety cost, the number of its executed
     steps whose cost flag (the replay rows' last column) is set (serl_rollout_desc.d_cost).
+    shape.state_dim = INCREMENTAL_STATE_DIM flies incremental control (SERL_ROLLOUT_INCREMENTAL: rate commands integrated into the
+    deflection, obs + last_u, replay rows of replay_cols(10) columns; on K1 and K1-TC, without track, cost, gust or sensor_noise).
     widths=[w0, w1, ..., w_{n-1}] (2 to 9 widths): width-list actors on the tensor-core kernel K1-TC (csrc/rollout_tc.cu); `shape`
     then only supplies the activation.  widths=None flies the uniform actor `shape` on K1, or on K1-TC with [h] * (L + 1) when its
     genome does not fit K1's kernels (tc_widths)."""
@@ -104,7 +126,7 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
         widths = tc_widths(shape)
     pop, P = weights.shape
     assert weights.dtype == torch.float32 and weights.is_contiguous()
-    assert P == (num_params_wide(widths) if widths else num_params(shape)), (P, widths)
+    assert P == (num_params_wide(widths, shape.state_dim) if widths else num_params(shape)), (P, widths)
     per_actor = env_mode.dim() == 2
     n_envs = env_mode.shape[-1]
     block = (pop, n_envs) if per_actor else (n_envs,)
@@ -124,7 +146,7 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
         r.trace = None
         r.smoothness = None
         r.actions = torch.empty((pop, n_envs, horizon, 3), dtype=torch.float32, device=dev) if actions else None
-        r.replay = torch.empty((pop, horizon, REPLAY_COLS), dtype=torch.float32, device=dev) if replay_env is not None else None
+        r.replay = torch.empty((pop, horizon, replay_cols(shape.state_dim)), dtype=torch.float32, device=dev) if replay_env is not None else None
         r.status = torch.zeros((1,), dtype=torch.int32, device=dev) if status else None
         r.track = torch.empty((pop, n_envs, TRACK_COLS), dtype=torch.float64, device=dev) if track else None
         r.cost = torch.empty((pop, n_envs), dtype=torch.int32, device=dev) if cost else None
@@ -153,7 +175,8 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
         assert sensor_noise.shape == (pop, n_envs, horizon + 1, 7) and sensor_noise.dtype == torch.float32 and sensor_noise.is_contiguous()
         d.d_sensor_noise = p(sensor_noise)
     d.flags = ((_native.ROLLOUT_GUST if gust else 0) | (_native.ROLLOUT_STAGGER if stagger else 0)      # gust: mode_code(...) & MODE_GUST
-               | (_native.ROLLOUT_PER_ACTOR_REFS if per_actor else 0))
+               | (_native.ROLLOUT_PER_ACTOR_REFS if per_actor else 0)
+               | (_native.ROLLOUT_INCREMENTAL if shape.state_dim == INCREMENTAL_STATE_DIM else 0))
     if widths:
         warr = np.asarray(widths, dtype=np.int32)       # host array, alive until the call returns
         d.widths, d.n_widths = warr.ctypes.data, len(widths)
@@ -170,8 +193,11 @@ def tc_widths(shape):
     return out[:n].tolist() if n else None
 
 
-def num_params_wide(widths):
-    return int(_native.lib().serl_actor_num_params_wide(np.asarray(widths, dtype=np.int32).ctypes, len(widths)))
+def num_params_wide(widths, state_dim=7):
+    """parameters of a width-list actor; serl_actor_num_params_wide counts a 7-entry observation, incremental control's
+    layer 0 has 3 * w0 weights more"""
+    n = int(_native.lib().serl_actor_num_params_wide(np.asarray(widths, dtype=np.int32).ctypes, len(widths)))
+    return n + (state_dim - 7) * int(widths[0])
 
 
 def actor_forward_wide(genome, widths, activation, obs):

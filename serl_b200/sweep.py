@@ -36,7 +36,7 @@ import torch
 from . import evaluation, td3_fused
 from .core import agent as agent_mod
 from ._native import NativeError
-from .rollout import actor_shape
+from .rollout import INCREMENTAL_STATE_DIM, actor_shape
 
 
 class RNGState:
@@ -107,6 +107,8 @@ class Sweep:
         if torch.distributed.is_available() and torch.distributed.is_initialized() and torch.distributed.get_world_size() > 1:
             raise NotImplementedError('Sweep: runs on one GPU; a torch.distributed world larger than 1 is not supported')
         for i, (p, _) in enumerate(runs):
+            if p.state_dim == INCREMENTAL_STATE_DIM:
+                raise ValueError('Sweep: run %d flies incremental control (state_dim 10), which fused_td3 (K7) does not train' % i)
             if not getattr(p, 'fused_td3', False):
                 raise ValueError('Sweep: run %d does not set fused_td3 (the sweep trains every RL half in one K7 launch)' % i)
             if mixed_shapes:

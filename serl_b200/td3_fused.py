@@ -12,8 +12,7 @@ import torch
 
 from . import _native
 from .core import td3
-from .core.replay_memory import TRANSITION_COLS
-from .rollout import actor_shape
+from .rollout import INCREMENTAL_STATE_DIM, TRANSITION_COLS, actor_shape
 
 # steps per launch: keeps every launch well under a second at the largest population
 LAUNCH_STEPS = 8192
@@ -41,6 +40,9 @@ def state_floats(shape):
 
 class FusedTD3(td3.TD3):
     def __init__(self, args, cluster_size=0, seed=None):
+        if args.state_dim == INCREMENTAL_STATE_DIM:
+            raise ValueError('fused_td3: K7 trains the actor of absolute control (state_dim 7); incremental control (state_dim 10) '
+                             'trains with the torch TD3 (fused_td3=False)')
         super().__init__(args)
         if torch.device(args.device).type != 'cuda':
             raise _native.NativeError('FusedTD3 needs a CUDA device (no CPU fallback)')
