@@ -186,6 +186,11 @@ __device__ __forceinline__ double plant_cos_fast(double x) { double s, c; plant_
 #undef PLANT_FN
 #define PLANT_FN static __device__ __forceinline__
 #define PLANT_RHS_COMMON_NAME plant_rhs_common
+// Breakpoint searches: the counted form here (tables through a generic pointer: the bucketed form's two dependent table
+// reads cost more than its compares save); the bucketed one (tools/lift/bucket.py) in the shared-space instance below when
+// the including kernel stages the byte tables (PLANT_SMEM_BUCKETS)
+#undef PLANT_SEARCH
+#define PLANT_SEARCH(bucketed, counted) (counted)
 #include PLANT_GEN(plant_rhs_common.h)     // ONE function for every plant variant + per-variant parameter rows
 // Second instance of the same generated text for kernels that stage the tables (+ parameter rows) at the START of their
 // dynamic shared memory: tables and parameter rows are read as plant_smem_tab[...] — the compiler sees the shared address
@@ -212,7 +217,16 @@ __device__ __forceinline__ int plant_smem_index(const real* p)          // eleme
 #define PLANT_PV_TABLE static __device__ const real plant_pv_second_instance_unused[SERL_PLANT_COUNT][PLANT_NPV]
 #undef PLANT_RHS_COMMON_NAME
 #define PLANT_RHS_COMMON_NAME plant_rhs_common_smem
+#if defined(PLANT_SMEM_BUCKETS) && defined(PLANT_BUCKET_BYTES)
+// the byte tables of the bucketed searches follow the parameter rows (plant_stage_buckets)
+#undef PLANT_SEARCH
+#define PLANT_SEARCH(bucketed, counted) (bucketed)
+#define PLANT_BKT(name) (reinterpret_cast<const unsigned char*>(plant_smem_tab + PT_TOTAL + SERL_PLANT_COUNT * PLANT_NPV) + PB_OFF_##name)
+#endif
 #include PLANT_GEN(plant_rhs_common.h)
+#undef PLANT_SEARCH
+#define PLANT_SEARCH(bucketed, counted) (counted)
+#undef PLANT_BKT
 #undef PLANT_RHS_COMMON_NAME
 #undef PLANT_TAB
 #undef PLANT_PV
@@ -434,7 +448,20 @@ struct RolloutArgs {
 // plant tables + per-variant parameter rows (reals), and that count rounded up to an even one: the block K1 stages at the
 // start of its dynamic shared memory, in front of the genome slots
 constexpr int PLANT_TABN = PT_TOTAL + SERL_PLANT_COUNT * PLANT_NPV;
-constexpr int PLANT_TABN2 = (PLANT_TABN + 1) & ~1;
+#if defined(PLANT_SMEM_BUCKETS) && defined(PLANT_BUCKET_BYTES)
+constexpr int PLANT_BKT_WORDS = (PLANT_BUCKET_BYTES + 7) / 8;       // byte tables of the bucketed searches, in doubles
+#else
+constexpr int PLANT_BKT_WORDS = 0;
+#endif
+// a kernel that stages the tables: tables | parameter rows | byte tables of the bucketed searches (PLANT_SMEM_BUCKETS)
+constexpr int PLANT_TABN2 = (PLANT_TABN + PLANT_BKT_WORDS + 1) & ~1;
+__device__ __forceinline__ void plant_stage_buckets(real* tab_s, int tid, int nthreads)
+{
+#if defined(PLANT_SMEM_BUCKETS) && defined(PLANT_BUCKET_BYTES)
+    unsigned char* b = reinterpret_cast<unsigned char*>(tab_s + PLANT_TABN);
+    for (int i = tid; i < PLANT_BUCKET_BYTES; i += nthreads) b[i] = plant_bucket_blob[i];
+#endif
+}
 
 // Tracking-error accumulators of the evaluation suite (serl_rollout_desc.d_track): the kernels take them as a launch
 // argument of their own, next to the argument block, so that adding them moved no field of the training instantiations.

@@ -42,6 +42,30 @@ PLANT_FN int plant_index(const real* x, int n, real u)
     }
 }
 
+/* bucketed breakpoint search (tools/lift/bucket.py), the counted search #{1 <= j <= n-2 : x[j] < y} in O(1): the uniform
+ * cell floor(fma(y, s, o)), clamped to [0, nb - 1] (NaN -> 0), holds at most the one breakpoint x[n0 + 1], and its byte in
+ * bkt (PLANT_BKT: plant_bucket_blob, staged next to the tables) is n0.  The generator emits it only where it has proved the
+ * result equal to the counted search for every double and NaN.  A search with negative breakpoints (tie rule `x[j] <= u`
+ * for those) passes y = plant_tie_up(u): b <= u  <=>  b < (the next double above u) for u < 0. */
+#ifdef __CUDACC__
+PLANT_FN int plant_cell(double v, int nb) { return min(max(__double2int_rd(v), 0), nb - 1); }       /* NaN converts to 0 */
+PLANT_FN double plant_tie_up(double u) { return u < 0.0 ? __longlong_as_double(__double_as_longlong(u) - 1) : u; }
+#else
+PLANT_FN int plant_cell(double v, int nb) { return v >= 1.0 ? (v < (double)(nb - 1) ? (int)v : nb - 1) : 0; }
+PLANT_FN double plant_tie_up(double u)
+{
+    union { double d; long long i; } b;
+    b.d = u;
+    b.i -= 1;
+    return u < 0.0 ? b.d : u;
+}
+#endif
+PLANT_FN int plant_bucket(double y, double s, double o, int nb, const unsigned char* bkt, const real* x)
+{
+    const int n0 = bkt[plant_cell(fma(y, s, o), nb)];
+    return n0 + (x[n0 + 1] < y);
+}
+
 /* interval of the table3 S-function: the first breakpoint not below u, minus one, clamped to [0, n-2].  Breakpoints are
  * strictly increasing, so "scan while x[i] < u" stops after exactly count(x[i] < u) steps: written as that count, the search
  * has no data-dependent loop (n is a literal at every call, the sum unrolls into compare + add). */

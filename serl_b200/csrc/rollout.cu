@@ -20,6 +20,7 @@
 //   rollout_kernel_simple   every thread runs the whole MLP for its env (any h that fits); cross-check / fallback shape.
 #include <type_traits>
 
+#define PLANT_SMEM_BUCKETS          // K1 stages the bucketed searches' byte tables with the plant tables (plant_env.cuh)
 #include "plant_env.cuh"
 
 // ---- simple actor: every thread evaluates the whole MLP for its own observation -------------------------
@@ -437,7 +438,7 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
     if (TABS) plant_tab_check(smem_raw);
     real* tab_s = reinterpret_cast<real*>(smem_raw);
     // PLANT_TABN2 (plant_env.cuh) spelt out: naming it here reorders a few instructions of the gust instantiations
-    constexpr int TABN = PT_TOTAL + SERL_PLANT_COUNT * PLANT_NPV;      // tables + per-variant parameter rows
+    constexpr int TABN = PT_TOTAL + SERL_PLANT_COUNT * PLANT_NPV + PLANT_BKT_WORDS;      // tables + parameter rows + bytes
     constexpr int TABN2 = (TABN + 1) & ~1;
     static_assert(TABN2 == PLANT_TABN2, "shared-memory layout of the plant tables");
     float* wbase = reinterpret_cast<float*>(tab_s + (TABS ? TABN2 : 0));
@@ -451,6 +452,7 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
     if (TABS) {
         for (int i = tid; i < PT_TOTAL; i += blockDim.x) tab_s[i] = plant_tables_blob[i];
         for (int i = tid; i < SERL_PLANT_COUNT * PLANT_NPV; i += blockDim.x) tab_s[PT_TOTAL + i] = (&plant_pv[0][0])[i];
+        plant_stage_buckets(tab_s, tid, blockDim.x);
     }
     if (tid == 0) {
         for (int i = 0; i < ar.apc; ++i) mbar_init(&gbar[i], 1);

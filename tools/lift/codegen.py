@@ -7,10 +7,12 @@ Output = two text blobs:
 Passes: dead-code elimination from the live derivative outputs; lookup specialisation (a 2-D lookup whose
 first argument is a constant collapses to a 1-D lookup over a pre-blended column; slope tables are
 pre-divided in double with the reference's operation order so results stay bit-identical); sharing of
-the breakpoint search between lookups on the same (axis, input).
+the breakpoint search between lookups on the same (axis, input); in the double-precision device build, long searches
+become certified bucketed searches (bucket.py).
 """
 import math
 
+import bucket
 import symtrace as S
 
 
@@ -62,13 +64,17 @@ class ConstPool:
 
 
 class Emitter:
-    def __init__(self, tracer, real='real', pool=None, fast=False):
+    def __init__(self, tracer, real='real', pool=None, fast=False, bucket=False):
         # fast (device build only): divisions by table spacings become multiplications by pre-inverted tables and
         # sin/cos of the same angle are computed by one sincos; results move by <= 1 ulp per affected operation
         self.fast = fast
+        # bucket (double-precision device build only): long breakpoint searches become certified O(1) bucketed searches
+        # (bucket.py); the index is the counted one bit for bit
+        self.bucket = bucket
         self.pool = pool
         self.tr = tracer
         self.tabs = {}        # name -> list of floats
+        self.bkts = {}        # name -> bucket bytes of a bucketed search (bucket.py)
         self.tabname = {}     # key -> name
         self.lines = []
         self.real = real
@@ -121,7 +127,20 @@ class Emitter:
             # u < 0: x[i] <= u < x[i+1]) folded per breakpoint: a negative breakpoint compares with <=.
             xs = self.tabs[axis]
             terms = ['(%s %s %s)' % (self.lit(xs[j]), '<=' if xs[j] < 0 else '<', self.ref(unode)) for j in range(1, n - 1)]
-            self.lines.append('const int %s = %s;' % (iv, ' + '.join(terms) if terms else '0'))
+            counted = ' + '.join(terms) if terms else '0'
+            plan = bucket.plan(xs) if self.bucket else None
+            if plan is not None:
+                # the same index from one uniform cell: its byte (PLANT_BKT) is the count at the cell's left end and
+                # the cell holds at most the one breakpoint xs[n0 + 1]; negative breakpoints' `<=` becomes `<` against
+                # the next double above a negative input.  PLANT_SEARCH(bucketed, counted): the includer picks one
+                # (the bucketed form needs the byte tables next to the staged tables)
+                bk = plan.name()
+                self.bkts[bk] = list(plan.bkt)
+                y = ('plant_tie_up(%s)' if plan.tie else '%s') % self.ref(unode)
+                self.lines.append('const int %s = PLANT_SEARCH(plant_bucket(%s, %s, %s, %d, PLANT_BKT(%s), PLANT_TAB(%s)), %s);'
+                                  % (iv, y, self.lit(plan.s), self.lit(plan.o), plan.nb, bk, axis, counted))
+            else:
+                self.lines.append('const int %s = %s;' % (iv, counted))
             self.lines.append('const %s %s = %s - PLANT_TAB(%s)[%s];' % (self.real, dv, self.ref(unode), axis, iv))
             self.idx[k] = (iv, dv)
         return self.idx[k]
