@@ -153,14 +153,28 @@ int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shap
  *                has 10 * w0 layer-0 weights: serl_actor_num_params_wide(widths) + 3 * w0 floats per actor.
  *                The env modes are device data the host does not read: the reference flies incremental control on the
  *                nominal build only (any mode containing 'incremental' selects h2000-v90, no fault, no gust, no noise)
+ *                SERL_ROLLOUT_SYMMETRIC: symmetric (pitch-only) control (envs/phlabenv.py:84-90, 226-231, 304-313; the env
+ *                PHlab_symmetric_<mode>).  shape.state_dim must be 2 and shape.action_dim 1 with the flag, and a 2 / 1 shape
+ *                needs the flag.  The one action is the elevator, scaled to +-10 deg like the attitude mode's; the plant and
+ *                the fault shim take [de, 0, 0].  obs = [e_theta, q]; reward = -|clip(6/pi e_theta, -1, 1)|, termination and
+ *                penalty as in the attitude mode (they still test phi).  The theta reference's offset is the constant trim
+ *                0.22 deg instead of rad2deg(theta0); the phi channel of d_ref_levels is not read; the training episode's
+ *                smooth width is t_max // 6.7 = 2 s, which the caller passes (t_max > 0).  d_action_noise is
+ *                [pop, n_envs, horizon, 1].  Replay rows have SERL_REPLAY_COLS_SA(2, 1) = 8 columns: 0-1 obs, 2 action,
+ *                3-4 next_obs, 5 reward, 6 done, 7 cost.  The trace's u columns and d_actions stay 3 wide and hold the padded
+ *                deflection [de, 0, 0].  Not with SERL_ROLLOUT_INCREMENTAL, d_track, d_cost, SERL_ROLLOUT_GUST or
+ *                d_sensor_noise: SERL_ERR_ARG before any CUDA call.  With widths (K1-TC) the genome has 2 * w0 layer-0
+ *                weights and one output: serl_actor_num_params_wide(widths) - 5 * w0 - 2 * (w_last + 1) floats per actor
  * t_max <= 0 selects the training defaults (20 s, smooth width 3 s). */
 #define SERL_TRACK_COLS 4
 #define SERL_REPLAY_COLS 20                       /* = SERL_REPLAY_COLS_OF(7) */
 #define SERL_REPLAY_COLS_OF(S) (2 * (S) + 6)      /* obs S | action 3 | next_obs S | reward | done | cost */
+#define SERL_REPLAY_COLS_SA(S, A) (2 * (S) + (A) + 3)     /* obs S | action A | next_obs S | reward | done | cost */
 #define SERL_ROLLOUT_GUST 1
 #define SERL_ROLLOUT_STAGGER 2
 #define SERL_ROLLOUT_PER_ACTOR_REFS 4
 #define SERL_ROLLOUT_INCREMENTAL 8
+#define SERL_ROLLOUT_SYMMETRIC 16
 enum { SERL_STATUS_NONFINITE = 1,     /* a trajectory's state / return became NaN or infinite */
        SERL_STATUS_GUST_FLAG = 2 };   /* an env has SERL_MODE_GUST but the launch was not made with SERL_ROLLOUT_GUST */
 typedef struct {

@@ -25,6 +25,7 @@ ROLLOUT_GUST = 1
 ROLLOUT_STAGGER = 2
 ROLLOUT_PER_ACTOR_REFS = 4
 ROLLOUT_INCREMENTAL = 8
+ROLLOUT_SYMMETRIC = 16
 STATUS_NONFINITE = 1
 STATUS_GUST_FLAG = 2
 # include/serl_td3.h (K7, the fused TD3 learner)

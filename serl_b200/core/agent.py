@@ -75,6 +75,13 @@ class Agent:
         if bool(getattr(environment, 'incremental', False)) != (args.state_dim == rollout.INCREMENTAL_STATE_DIM):
             raise ValueError('Agent: args.state_dim = %s does not match the env: the observation of incremental control has 10 entries, '
                              'that of absolute control 7' % args.state_dim)
+        n_actions = int(getattr(environment, 'n_actions', 3))
+        if args.action_dim != n_actions:
+            raise ValueError('Agent: args.action_dim = %s does not match the env, which takes %d actions (symmetric control: the elevator '
+                             'alone, attitude control: 3)' % (args.action_dim, n_actions))
+        if bool(getattr(environment, 'symmetric', False)) and args.state_dim != rollout.SYMMETRIC_STATE_DIM:
+            raise ValueError('Agent: args.state_dim = %s does not match the env: the observation of symmetric control has 2 entries'
+                             % args.state_dim)
         if not torch.cuda.is_available():
             from .._native import NativeError
             raise NativeError('serl_b200.Agent needs a CUDA device: the rollout / evolution engine has no CPU fallback')
@@ -86,7 +93,7 @@ class Agent:
         else:
             self.rl_agent = td3.TD3(args)
         self.replay_buffer = replay_memory.DeviceReplayMemory(args.buffer_size, self.device, seed=int(getattr(args, 'seed', 7)),
-                                                              state_dim=args.state_dim)
+                                                              state_dim=args.state_dim, action_dim=args.action_dim)
         self.noise_process = mod_utils.GaussianNoise(args.action_dim, sd=args.noise_sd)
         if len(self.pop):
             self.evolver = utils_ne.SSNE(self.args, self.rl_agent.critic, self.evaluate)
@@ -138,7 +145,8 @@ class Agent:
 
     def _eval_kw(self):
         env = self.env
-        kw = {} if env.t_max == 20 else {'t_max': float(env.t_max), 'smooth_width': refsig.widths(env.t_max)[1]}
+        sym = rollout.is_symmetric(self.shape)
+        kw = {} if env.t_max == 20 else {'t_max': float(env.t_max), 'smooth_width': refsig.widths(env.t_max, sym)[1]}
         return dict(kw, gust=rollout.mode_gust(env.mode_code))
 
     def _fly(self, agent, n, is_action_noise=False, store_transition=False, trace=False, stream=None, copy_genome=False, draws=None) -> _Flight:
@@ -151,12 +159,13 @@ class Agent:
         horizon = self._horizon()
         noise_host = None
         if is_action_noise:
-            # one np.random.randn(3) per executed step (agent.py:90-93): draw a full horizon, rewind the global stream to
+            # one np.random.randn(action_dim) per executed step (agent.py:90-93): draw a full horizon, rewind the global stream to
             # "exactly the steps that ran" once the episode length is known (collect)
             assert n == 1
+            A = self.shape.action_dim
             f.noise_state = np.random.get_state()
-            z = np.random.randn(horizon, 3)
-            noise_host = np.clip(self.args.noise_sd * z, -self.args.noise_clip, self.args.noise_clip).astype(np.float32).reshape(1, 1, -1, 3)
+            z = np.random.randn(horizon, A)
+            noise_host = np.clip(self.args.noise_sd * z, -self.args.noise_clip, self.args.noise_clip).astype(np.float32).reshape(1, 1, -1, A)
         f.stream = stream
         ctx = torch.cuda.stream(stream) if stream is not None else _null()
         pre = self._genome_of(agent).clone() if copy_genome else None        # copied on the main stream, before later edits
@@ -184,7 +193,7 @@ class Agent:
         rows = rows[:n]
         self.replay_buffer.add_rows(rows)
         agent.buffer.add_rows(rows)
-        crit = rows[rows[:, rollout.transition_cols(self.shape.state_dim)] > 0.5]
+        crit = rows[rows[:, rollout.transition_cols(self.shape.state_dim, self.shape.action_dim)] > 0.5]
         if crit.shape[0]:
             agent.critical_buffer.add_rows(crit)
         self.num_frames += n
@@ -208,28 +217,33 @@ class Agent:
                 hist = {e: f.r.actions[0, e, :int(steps[e])].cpu().numpy().astype(np.float64) for e in range(f.n)}
         if f.noise_state is not None:
             np.random.set_state(f.noise_state)
-            np.random.randn(int(steps[0]), 3)
+            np.random.randn(int(steps[0]), self.shape.action_dim)
         if store_transition:
             if f.stream is not None:
                 f.r.replay.record_stream(torch.cuda.current_stream(self.device))     # read below by kernels of this stream
             self._store_rows(agent, f.r.replay[0], int(steps[0]))
         env = self.env
-        theta_trim = np.rad2deg(rollout.initial_state(rollout.mode_variant(env.mode_code))[7])
+        sym = rollout.is_symmetric(self.shape)
+        # symmetric control keeps the env's constant trim (envs/phlabenv.py:194, 313)
+        theta_trim = env.theta_trim if sym else np.rad2deg(rollout.initial_state(rollout.mode_variant(env.mode_code))[7])
         from ..envs.phlabenv import _RefSignal
-        sw = refsig.widths(env.t_max)[1]
+        sw = refsig.widths(env.t_max, sym)[1]
+        A = self.shape.action_dim        # the deflection record is [de, 0, 0] in symmetric control; env.last_u has 1 entry
         eps = []
         for e in range(f.n):
             n = int(steps[e])
             refs = [_RefSignal(f.levels[e][0], f.starts[e][0], theta_trim, sw, env.t_max), _RefSignal(f.levels[e][1], f.starts[e][1], 0.0, sw), lambda t: 0.0]
+            if sym:      # the theta reference alone, as the env's ref (envs/phlabenv.py:313)
+                refs = refs[:1]
             fitness = float(returns[e]) + (float(sm[e]) if self.args.smooth_fitness else 0.0)
             state_lst, actions, rewards = [], None, None
             if f.r.trace is not None and (want_history or f.n == 1):
                 tr = hist[e]
                 rewards = [float(x) for x in tr[:, rollout.TRACE_R]]
-                actions = tr[:, rollout.TRACE_U].copy()
+                actions = tr[:, rollout.TRACE_U][:, :A].copy()
                 state_lst = [] if store_transition else [tr[k, rollout.TRACE_X].copy() for k in range(n)]
             else:
-                actions = hist[e] if want_history else np.zeros((0, 3))
+                actions = hist[e][:, :A] if want_history else np.zeros((0, A))
                 rewards = _ReturnOnly(float(returns[e]))
             eps.append(Episode(fitness=fitness, smoothness=float(sm[e]), length=self._final_time(n), state_history=state_lst,
                                ref_signals=refs, actions=actions, reward_lst=rewards))
@@ -392,7 +406,7 @@ class Agent:
         self._last_result = r
         if store:
             # the stored transitions of EVERY actor reach EVERY rank (identical shared / per-actor buffers on all ranks)
-            cols = rollout.replay_cols(self.shape.state_dim)
+            cols = rollout.replay_cols(self.shape.state_dim, self.shape.action_dim)
             rows = r.replay if r is not None else torch.zeros((0, horizon, cols), dtype=torch.float32, device=self.device)
             rows_all = engine.gather_rows(rows.reshape(rows.shape[0], -1), pop, world, rank).reshape(pop, horizon, cols)
             steps_all = rec_all[:, 3].to(torch.int64)
@@ -400,7 +414,7 @@ class Agent:
             self.replay_buffer.add_rows(rows_all[sel])
             actors = torch.arange(pop, device=self.device)
             self.pop.buffers.append(actors, rows_all, sel)
-            self.pop.critical_buffers.append(actors, rows_all, sel & (rows_all[..., rollout.transition_cols(self.shape.state_dim)] > 0.5))
+            self.pop.critical_buffers.append(actors, rows_all, sel & (rows_all[..., rollout.transition_cols(self.shape.state_dim, self.shape.action_dim)] > 0.5))
         rec_host = rec_all.cpu().numpy()
         if r is not None:
             r.check()

@@ -76,10 +76,10 @@ class ReplayMemory:
         return tuple(torch.from_numpy(self._store[f][pick]).to(self.device) for f in Transition._fields)
 
 
-def _split(rows, state_dim):
-    """the Transition fields (obs, action, next_obs, reward, done) of stored transitions [n, transition_cols(state_dim)]"""
+def _split(rows, state_dim, action_dim=3):
+    """the Transition fields (obs, action, next_obs, reward, done) of stored transitions [n, transition_cols(state_dim, action_dim)]"""
     out, off = [], 0
-    for d in replay_dims(state_dim)[:5]:
+    for d in replay_dims(state_dim, action_dim)[:5]:
         out.append(rows[:, off:off + d])
         off += d
     return tuple(out)
@@ -87,14 +87,14 @@ def _split(rows, state_dim):
 
 class DeviceReplayMemory:
     """Ring buffer on the GPU with ReplayMemory's interface.  Rows are K1 replay rows (include/serl_b200.h
-    SERL_REPLAY_COLS_OF(state_dim): obs | action 3 | next_obs | reward | done | cost; rollout.replay_dims) without the cost
+    SERL_REPLAY_COLS_SA(state_dim, action_dim): obs | action | next_obs | reward | done | cost; rollout.replay_dims) without the cost
     flag; sampling uses a device generator, so the stdlib `random` stream the SSNE planner consumes does not depend on the
     buffer (every rank holds identical buffers and identical generators -> identical batches)."""
 
-    def __init__(self, capacity, device, seed=0, state_dim=7):
+    def __init__(self, capacity, device, seed=0, state_dim=7, action_dim=3):
         self.capacity, self.device = int(capacity), torch.device(device)
-        self.state_dim = int(state_dim)
-        self.cols = transition_cols(self.state_dim)
+        self.state_dim, self.action_dim = int(state_dim), int(action_dim)
+        self.cols = transition_cols(self.state_dim, self.action_dim)
         self.data = None
         self._count, self.position = 0, 0
         self.gen = None
@@ -153,7 +153,7 @@ class DeviceReplayMemory:
 
     def get_latest(self, latest):
         rows = self._chronological_rows()[-int(latest):]
-        return [Transition(*_split(rows[i:i + 1], self.state_dim)) for i in range(rows.shape[0])]
+        return [Transition(*_split(rows[i:i + 1], self.state_dim, self.action_dim)) for i in range(rows.shape[0])]
 
     def add_content_of(self, other):
         rows = other._chronological_rows() if hasattr(other, '_chronological_rows') else None
@@ -168,18 +168,19 @@ class DeviceReplayMemory:
         self._alloc()
         n = len(self)
         pick = torch.randperm(n, device=self.device, generator=self.gen)[:int(batch_size)]
-        return _split(self.data[pick], self.state_dim)
+        return _split(self.data[pick], self.state_dim, self.action_dim)
 
 
 class PopulationBuffers:
     """The per-actor replay buffers of the whole population (GeneticAgent.buffer / .critical_buffer,
     base/core/genetic_agent.py:14-16) as ONE device tensor [pop, capacity, cols] with per-actor ring positions, filled
-    for all actors of a generation by one vectorised scatter (cols: the transition of an observation of state_dim entries)."""
+    for all actors of a generation by one vectorised scatter (cols: the transition of an observation of state_dim entries and
+    action_dim actions)."""
 
-    def __init__(self, pop, capacity, device, state_dim=7):
+    def __init__(self, pop, capacity, device, state_dim=7, action_dim=3):
         self.pop, self.capacity, self.device = int(pop), int(capacity), torch.device(device)
-        self.state_dim = int(state_dim)
-        self.cols = transition_cols(self.state_dim)
+        self.state_dim, self.action_dim = int(state_dim), int(action_dim)
+        self.cols = transition_cols(self.state_dim, self.action_dim)
         self.data = None
         self.pos = torch.zeros(self.pop, dtype=torch.int64, device=self.device)
         self.count = torch.zeros(self.pop, dtype=torch.int64, device=self.device)
@@ -264,10 +265,10 @@ class ActorBuffer:
 
     def get_latest(self, latest):
         rows = self._chronological_rows()[-int(latest):]
-        return [Transition(*_split(rows[i:i + 1], self.owner.state_dim)) for i in range(rows.shape[0])]
+        return [Transition(*_split(rows[i:i + 1], self.owner.state_dim, self.owner.action_dim)) for i in range(rows.shape[0])]
 
     def sample(self, batch_size):
         self.owner._alloc()
         rows = self._chronological_rows()
         pick = torch.randperm(rows.shape[0], device=rows.device, generator=self.owner.gen)[:int(batch_size)]
-        return _split(rows[pick], self.owner.state_dim)
+        return _split(rows[pick], self.owner.state_dim, self.owner.action_dim)

@@ -43,7 +43,8 @@ class TD3:
     def __init__(self, args):
         self.args = args
         if torch.device(args.device).type == 'cuda':
-            mem = lambda capacity, device: replay_memory.DeviceReplayMemory(capacity, device, state_dim=args.state_dim)
+            mem = lambda capacity, device: replay_memory.DeviceReplayMemory(capacity, device, state_dim=args.state_dim,
+                                                                               action_dim=args.action_dim)
         else:
             mem = replay_memory.ReplayMemory
         self.buffer = mem(args.individual_bs, args.device)

@@ -414,7 +414,7 @@ struct Handoff {
     double* X;      // [NX][n]
     double* t;      // [n]
     double* ret;    // [n]
-    float* obs;     // [7][n]; incremental launches (INC): [10][n], followed by last_u [3][n] f64
+    float* obs;     // [7][n]; incremental launches (INC): [10][n], followed by last_u [3][n] f64; symmetric (SYM): [2][n]
     int* k;         // [n]  executed steps | done << 30
     int* flag;      // [n / 32] one word per warp, 1 when the record is complete
     long long n;
@@ -423,7 +423,7 @@ struct Handoff {
 struct RolloutArgs {
     const float* weights; int P; serl_actor_shape sh;
     const double* ref_levels; const double* ref_starts; const int* env_mode; int n_envs; int horizon;
-    const float* action_noise;      // optional [pop, n_envs, horizon, 3]: clipped exploration noise (agent.py:90-93)
+    const float* action_noise;      // optional [pop, n_envs, horizon, 3 (1 with symmetric control)]: clipped exploration noise (agent.py:90-93)
     double* returns; int* steps; double* trace;   // trace optional [pop, n_envs, horizon, SERL_TRACE_COLS]
     float* actions;                 // optional [pop, n_envs, horizon, 3] fp32: commanded deflection last_u (smoothness metric)
     int pop;
@@ -538,14 +538,20 @@ __device__ __forceinline__ void env_bind(Env& e, const RolloutArgs& a, int env, 
     if (!GUST && e.gust && a.status) atomicOr(a.status, SERL_STATUS_GUST_FLAG);
 }
 
-// observation entries of a kernel instantiation: 7, or 10 with incremental control (INC).  A namespace-scope constant because
-// a local constexpr declaration in a kernel body moved the instruction schedule of the instantiations without INC
-template <bool INC> constexpr int OBS_DIM = INC ? 10 : 7;
+// observation entries of a kernel instantiation: 7, 10 with incremental control (INC), 2 with symmetric control (SYM).  A
+// namespace-scope constant because a local constexpr declaration in a kernel body moved the instruction schedule of the
+// instantiations without INC
+template <bool INC, bool SYM = false> constexpr int OBS_DIM = SYM ? 2 : INC ? 10 : 7;
+// actor outputs: 3, or the elevator alone with symmetric control
+template <bool SYM> constexpr int ACT_DIM = SYM ? 1 : 3;
+// symmetric control's theta reference offset: the env's constant trim, never replaced by rad2deg(theta0) (phlabenv.py:194, 313)
+constexpr double SYM_THETA_TRIM = 0.22;
 
 // a lane without an env: done from the start, with a zero state and observation (it still takes part in the actor)
 // INC: incremental control (SERL_ROLLOUT_INCREMENTAL): the observation has 10 entries and the env carries last_u[3], the
 // deflection the rates were integrated into (kept by the kernel next to Env, which the other instantiations share unchanged)
-template <bool INC = false>
+// SYM: symmetric control (SERL_ROLLOUT_SYMMETRIC): a 2-entry observation
+template <bool INC = false, bool SYM = false>
 __device__ __forceinline__ void env_idle(Env& e, const RolloutArgs& a, const real* pv_base, float* obs, double* last_u = nullptr)
 {
     e.done = true; e.k = 0; e.ret = 0.0; e.t = 0.0; e.fault = 0; e.gust = 0; e.pv = pv_base; e.pv_post = nullptr; e.theta_trim = 0.0;
@@ -553,7 +559,7 @@ __device__ __forceinline__ void env_idle(Env& e, const RolloutArgs& a, const rea
 #pragma unroll
     for (int i = 0; i < NX; ++i) e.X[i] = 0.0;
 #pragma unroll
-    for (int i = 0; i < 7; ++i) obs[i] = 0.f;
+    for (int i = 0; i < (SYM ? 2 : 7); ++i) obs[i] = 0.f;
     if constexpr (INC)
 #pragma unroll
         for (int i = 0; i < 3; ++i) { obs[7 + i] = 0.f; last_u[i] = 0.0; }
@@ -603,7 +609,8 @@ __device__ __forceinline__ void sensor_noise(const RolloutArgs& a, size_t traj, 
 // carries one copy of the step code.
 // TRACK: zero the tracking-error sums; the controlled state before step 0 is reset()'s output env.x.
 // INC: last_u = 0 and obs[7..9] = last_u (phlabenv.py:425-426)
-template <bool STAB = false, bool GUST = false, bool TRACK = false, bool INC = false>
+// SYM: obs = [0, q] (phlabenv.py:422 with obs_idx = [1])
+template <bool STAB = false, bool GUST = false, bool TRACK = false, bool INC = false, bool SYM = false>
 static __device__ __forceinline__ void env_reset(Env& e, const RolloutArgs& a, int env, float* obs, size_t traj = 0,
                                                  double* last_u = nullptr)
 {
@@ -620,8 +627,12 @@ static __device__ __forceinline__ void env_reset(Env& e, const RolloutArgs& a, i
         e.trk[SERL_TRACK_COLS] = x0[7]; e.trk[SERL_TRACK_COLS + 1] = x0[6]; e.trk[SERL_TRACK_COLS + 2] = x0[5];
         e.trk[TRACK_COST] = 0.0; e.trk[TRACK_V0] = ic[3];
     }
-    obs[0] = obs[1] = obs[2] = 0.f;
-    obs[3] = (float)x0[0]; obs[4] = (float)x0[1]; obs[5] = (float)x0[2]; obs[6] = (float)x0[4];
+    if constexpr (SYM) {
+        obs[0] = 0.f; obs[1] = (float)x0[1];
+    } else {
+        obs[0] = obs[1] = obs[2] = 0.f;
+        obs[3] = (float)x0[0]; obs[4] = (float)x0[1]; obs[5] = (float)x0[2]; obs[6] = (float)x0[4];
+    }
     if constexpr (INC)
 #pragma unroll
         for (int i = 0; i < 3; ++i) { obs[7 + i] = 0.f; last_u[i] = 0.0; }
@@ -639,7 +650,10 @@ static __device__ __forceinline__ void env_reset(Env& e, const RolloutArgs& a, i
 // INC: incremental control (phlabenv.py:443-466): the scaled action is a rate (bound 25 deg/s, :205-206), integrated as
 // u = last_u + rate * dt in fp64 in the reference's operation order (:377-380; no contraction to fma), u drives the fault
 // shim and the plant, last_u = u, obs[7..9] = (float)u; replay rows of SERL_REPLAY_COLS_OF(10) columns
-template <bool STAB = false, bool GUST = false, bool TRACK = false, bool PER_ACTOR = false, bool INC = false>
+// SYM: symmetric control (phlabenv.py:84-90, 226-231, 304-313, 362-367): `a` holds the elevator alone, the plant takes
+// [de, 0, 0] (pad_action), the error is theta's against a reference offset by the constant trim, reward = -|clip(k e_theta)|
+// (a sum of one term over error.shape[0] = 1), obs = [e_theta, q]; replay rows of SERL_REPLAY_COLS_SA(2, 1) columns
+template <bool STAB = false, bool GUST = false, bool TRACK = false, bool PER_ACTOR = false, bool INC = false, bool SYM = false>
 static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, size_t traj, int actor, bool replay, const float* a, float* obs,
                                                 double* last_u = nullptr)
 {
@@ -650,9 +664,9 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
     double U[3], cmd[3], act_d[3];
     if (ar.action_noise) {
         // action = clip(action + clipped_noise, -1, 1) in float64, then scale_action in float64 (agent.py:90-96)
-        const float* nz = ar.action_noise + (traj * ar.horizon + e.k) * 3;
+        const float* nz = ar.action_noise + (traj * ar.horizon + e.k) * ACT_DIM<SYM>;
 #pragma unroll
-        for (int i = 0; i < 3; ++i) {
+        for (int i = 0; i < ACT_DIM<SYM>; ++i) {
             act_d[i] = fmin(fmax((double)a[i] + (double)nz[i], -1.0), 1.0);
             if constexpr (INC) U[i] = __dadd_rn(-bound, __dmul_rn(0.5 * __dadd_rn(act_d[i], 1.0), bound - (-bound)));
             else U[i] = -bound + 0.5 * (act_d[i] + 1.0) * (bound - (-bound));
@@ -660,7 +674,7 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
     } else {
         // scale_action: low + 0.5*(a + 1.0)*(high - low) with a float32: (a + 1.0) and the halving round in fp32 (:72-73)
 #pragma unroll
-        for (int i = 0; i < 3; ++i) {
+        for (int i = 0; i < ACT_DIM<SYM>; ++i) {
             act_d[i] = (double)a[i];
             const float t1 = __fadd_rn(a[i], 1.0f);
             const float t2 = __fmul_rn(0.5f, t1);
@@ -671,6 +685,7 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
     if constexpr (INC)
 #pragma unroll
         for (int i = 0; i < 3; ++i) U[i] = __dadd_rn(last_u[i], __dmul_rn(U[i], 0.01));
+    if constexpr (SYM) { U[1] = U[2] = 0.0; act_d[1] = act_d[2] = 0.0; }      // pad_action (:373-379)
     // a NaN action would be squashed to a bound by the plant's input saturation (as in the reference binary): report it
     if (ar.status && !isfinite(act_d[0] + act_d[1] + act_d[2])) atomicOr(ar.status, SERL_STATUS_NONFINITE);
     apply_fault(e.fault, U, cmd);
@@ -682,9 +697,9 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
 
     const double t = e.t;
     // + signals.Const(0., t_max, theta_trim) (phlabenv.py:344): the trim offset exists on [0, t_max] only
-    const double r_th = ref_deg(e.ref_lv, e.ref_st, t, t <= ar.t_max ? e.theta_trim : 0.0, ar.smooth_w) * DEG2RAD;
-    const double r_ph = ref_deg(e.ref_lv + SERL_REF_BLOCKS, e.ref_st + SERL_REF_BLOCKS, t, 0.0, ar.smooth_w) * DEG2RAD;
-    const double e0 = r_th - xo[7], e1 = r_ph - xo[6], e2 = 0.0 - xo[5];
+    const double r_th = ref_deg(e.ref_lv, e.ref_st, t, t <= ar.t_max ? (SYM ? SYM_THETA_TRIM : e.theta_trim) : 0.0, ar.smooth_w) * DEG2RAD;
+    const double r_ph = SYM ? 0.0 : ref_deg(e.ref_lv + SERL_REF_BLOCKS, e.ref_st + SERL_REF_BLOCKS, t, 0.0, ar.smooth_w) * DEG2RAD;
+    const double e0 = r_th - xo[7], e1 = SYM ? 0.0 : r_ph - xo[6], e2 = SYM ? 0.0 : 0.0 - xo[5];
     if constexpr (TRACK) {
         const double et = r_th - e.trk[SERL_TRACK_COLS], ep = r_ph - e.trk[SERL_TRACK_COLS + 1], eb = 0.0 - e.trk[SERL_TRACK_COLS + 2];
         e.trk[0] += fabs(et); e.trk[1] += fabs(ep); e.trk[2] += fabs(eb); e.trk[3] += eb;
@@ -694,7 +709,7 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
     const double c0 = fabs(fmin(fmax(k_err * e0, -1.0), 1.0));
     const double c1 = fabs(fmin(fmax(k_err * e1, -1.0), 1.0));
     const double c2 = fabs(fmin(fmax(k_err4 * e2, -1.0), 1.0));
-    double reward = -((c0 + c1) + c2) / 3.0;
+    double reward = SYM ? -c0 : -((c0 + c1) + c2) / 3.0;
     const bool done = (t >= ar.t_max) || (fabs(xo[7]) > max_theta) || (fabs(xo[6]) > max_phi) || (xo[9] < 50.0);
     if (done) reward += (-1.0 / 0.01) * (ar.t_max - t) * 2.0;  // check_bounds penalty (:391-399)
     e.ret += reward;
@@ -717,13 +732,20 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
         // the transition Agent.evaluate stores (agent.py:101-112) + the cost flag of get_cost (phlabenv.py:369-375,
         // including its degrees-vs-radians comparison on the bank angle).  The same test as step_cost, spelt out: calling
         // it here changes the code of the instantiations without TRACK
-        constexpr int S = INC ? 10 : 7;
-        float* rp = ar.replay + ((size_t)actor * ar.horizon + e.k) * SERL_REPLAY_COLS_OF(S);
+        constexpr int S = INC ? 10 : SYM ? 2 : 7;
+        float* rp = ar.replay + ((size_t)actor * ar.horizon + e.k) * SERL_REPLAY_COLS_SA(S, ACT_DIM<SYM>);
 #pragma unroll
         for (int i = 0; i < S; ++i) rp[i] = obs[i];
-        rp[S] = (float)act_d[0]; rp[S + 1] = (float)act_d[1]; rp[S + 2] = (float)act_d[2];
-        float* rn = rp + S + 3;
-        rn[0] = o0; rn[1] = o1; rn[2] = o2; rn[3] = o3; rn[4] = o4; rn[5] = o5; rn[6] = o6;
+        float* rn;
+        if constexpr (SYM) {
+            rp[S] = (float)act_d[0];
+            rn = rp + S + 1;
+            rn[0] = o0; rn[1] = o4;
+        } else {
+            rp[S] = (float)act_d[0]; rp[S + 1] = (float)act_d[1]; rp[S + 2] = (float)act_d[2];
+            rn = rp + S + 3;
+            rn[0] = o0; rn[1] = o1; rn[2] = o2; rn[3] = o3; rn[4] = o4; rn[5] = o5; rn[6] = o6;
+        }
         if constexpr (INC) { rn[7] = (float)U[0]; rn[8] = (float)U[1]; rn[9] = (float)U[2]; }
         rn[S] = (float)reward;
         rn[S + 1] = done ? 1.f : 0.f;
@@ -732,7 +754,11 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
         const bool cost = (fabs(xo[4]) * RAD2DEG > 11.0) || (fabs(xo[6]) * RAD2DEG > 0.75 * max_phi) || (xo[3] < v0 / 3.0);
         rn[S + 2] = cost ? 1.f : 0.f;
     }
-    obs[0] = o0; obs[1] = o1; obs[2] = o2; obs[3] = o3; obs[4] = o4; obs[5] = o5; obs[6] = o6;
+    if constexpr (SYM) {
+        obs[0] = o0; obs[1] = o4;
+    } else {
+        obs[0] = o0; obs[1] = o1; obs[2] = o2; obs[3] = o3; obs[4] = o4; obs[5] = o5; obs[6] = o6;
+    }
     if constexpr (INC)
 #pragma unroll
         for (int i = 0; i < 3; ++i) { last_u[i] = U[i]; obs[7 + i] = (float)U[i]; }

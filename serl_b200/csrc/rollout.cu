@@ -112,7 +112,7 @@ __host__ __device__ constexpr int actor_xbuf_floats(int H, int S) { return (H / 
 // pair a block of 2H floats in which lane og's 2·T8 weights (row k's T8, then row k+1's) are its N4 float4 (at
 // 16-byte chunk i: all eight lanes' chunk i side by side, so that an LDS.128 of the warp touches 128 contiguous bytes)
 // and, for odd T8, one float2 after the chunks.  An odd last row (the observation layer: R = 7) is a plain row; the
-// incremental-control observation (R = 10) is five pairs.
+// incremental-control observation (R = 10) is five pairs, the symmetric-control one (R = 2) one pair.
 __host__ __device__ constexpr int pair_layout_index(int k, int n, int R, int H)
 {
     const int T8 = H / 8, N4 = T8 / 2 * 4;                 // floats of a lane's pair weights in float4 chunks
@@ -257,17 +257,16 @@ __device__ __forceinline__ void quarter_totals(F f, int og, float (&tot)[2])
 __device__ __forceinline__ int quarter_src_lane(int g, int c) { return g * 8 + 1 + ((c >> 2) & 1) * 2 + ((c >> 1) & 1) * 4; }
 
 // observation in, action out: by value (registers) rather than through pointers, which put them in local memory
-template <int S> struct ActorObs { float v[S]; };     // S = 7, or 10 with incremental control (+ last_u)
-struct ActorAct { float v[3]; };
+template <int S> struct ActorObs { float v[S]; };     // S = 7, 10 with incremental control (+ last_u), 2 with symmetric control
+template <int A = 3> struct ActorAct { float v[A]; };  // A = 3, or 1 with symmetric control (the elevator)
 
 // xb: this warp's exchange buffer, actor_xbuf_floats(H) floats in shared memory (actor_xbuf_floats(H, 10) for S = 10),
 // 16-byte aligned.  The observation layer sums its S inputs with fma from 0 in index order, then adds the bias (the
-// kernel-order specification)
-template <int H, int ACT, int S = 7>
-__device__ __noinline__ ActorAct actor_forward_warp(const float* __restrict__ w, int L, int lane, float* xb, ActorObs<S> obs)
+// kernel-order specification).  A: outputs, summed and squashed one by one in the same order
+template <int H, int ACT, int S = 7, int A = 3>
+__device__ __noinline__ ActorAct<A> actor_forward_warp(const float* __restrict__ w, int L, int lane, float* xb, ActorObs<S> obs)
 {
     constexpr int TM = H / 4, T8 = H / 8;
-    constexpr int A = 3;
     static_assert(S == 10 || TM >= S, "the observation rows fit the exchange buffer");
     const int og = lane & 7, g = lane >> 3, n0 = og * T8;
     const float* Wt0 = w;
@@ -340,7 +339,7 @@ __device__ __noinline__ ActorAct actor_forward_warp(const float* __restrict__ w,
         }
     }
     // output layer: quarter-block dot products over the group, combined like the LayerNorm sums; lane og keeps env 8g+og.
-    // The three tanh go through two pair calls.
+    // The three tanh go through two pair calls, a single action through one.
     float y[A];
 #pragma unroll
     for (int j = 0; j < A; ++j) {
@@ -352,27 +351,31 @@ __device__ __noinline__ ActorAct actor_forward_warp(const float* __restrict__ w,
         const float t0 = __shfl_sync(0xffffffffu, t[0], src), t1 = __shfl_sync(0xffffffffu, t[1], src);
         y[j] = __fadd_rn(og & 1 ? t1 : t0, bo[j]);
     }
-    static_assert(A == 3, "two tanh pairs");
-    const float2 t01 = am_tanh2(make_float2(y[0], y[1])), t2 = am_tanh2(make_float2(y[2], y[2]));
-    ActorAct action;
-    action.v[0] = t01.x; action.v[1] = t01.y; action.v[2] = t2.x;
+    static_assert(A == 3 || A == 1, "two tanh pairs, or one");
+    ActorAct<A> action;
+    if constexpr (A == 1) {
+        action.v[0] = am_tanh2(make_float2(y[0], y[0])).x;
+    } else {
+        const float2 t01 = am_tanh2(make_float2(y[0], y[1])), t2 = am_tanh2(make_float2(y[2], y[2]));
+        action.v[0] = t01.x; action.v[1] = t01.y; action.v[2] = t2.x;
+    }
     return action;
 }
 
 // one instantiation per activation: the choice is compiled into the 4 x h/4 activation calls of every layer
-template <int H, int S>
+template <int H, int S, int A>
 __device__ __forceinline__ void actor_forward(int act, const float* __restrict__ w, int L, int lane, float* xb, const float (&obs)[S],
-                                              float (&a)[3])
+                                              float (&a)[A])
 {
     ActorObs<S> o;
 #pragma unroll
     for (int k = 0; k < S; ++k) o.v[k] = obs[k];
-    ActorAct r;
-    if (act == SERL_ACT_TANH) r = actor_forward_warp<H, SERL_ACT_TANH, S>(w, L, lane, xb, o);
-    else if (act == SERL_ACT_ELU) r = actor_forward_warp<H, SERL_ACT_ELU, S>(w, L, lane, xb, o);
-    else r = actor_forward_warp<H, SERL_ACT_LEAKY_RELU, S>(w, L, lane, xb, o);
+    ActorAct<A> r;
+    if (act == SERL_ACT_TANH) r = actor_forward_warp<H, SERL_ACT_TANH, S, A>(w, L, lane, xb, o);
+    else if (act == SERL_ACT_ELU) r = actor_forward_warp<H, SERL_ACT_ELU, S, A>(w, L, lane, xb, o);
+    else r = actor_forward_warp<H, SERL_ACT_LEAKY_RELU, S, A>(w, L, lane, xb, o);
 #pragma unroll
-    for (int j = 0; j < 3; ++j) a[j] = r.v[j];
+    for (int j = 0; j < A; ++j) a[j] = r.v[j];
 }
 
 
@@ -429,7 +432,8 @@ __global__ void genome_layout_kernel(const float* __restrict__ w, float* __restr
 // (instantiated without TRACK, with both GUST values)
 // INC: incremental control (SERL_ROLLOUT_INCREMENTAL; instantiated without GUST and TRACK): a 10-entry observation and the
 // env's last_u, both carried in the hand-over records too (OBS_DIM: plant_env.cuh).
-template <int H, bool TABS, bool GUST, bool TRACK = false, bool PER_ACTOR = false, bool INC = false>
+// SYM: symmetric control (SERL_ROLLOUT_SYMMETRIC; instantiated without GUST and TRACK): a 2-entry observation, one action
+template <int H, bool TABS, bool GUST, bool TRACK = false, bool PER_ACTOR = false, bool INC = false, bool SYM = false>
 __global__ void __launch_bounds__(MAX_CTA_THREADS, 1)
 rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
 {
@@ -496,7 +500,7 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
     Env e;
     e.tab = tab;
     e.done = true; e.k = 0;
-    float obs[OBS_DIM<INC>], a[3];
+    float obs[OBS_DIM<INC, SYM>], a[ACT_DIM<SYM>];
     double last_u[3];                                  // INC only
     double* const ho_u = INC ? reinterpret_cast<double*>(ar.ho.obs + (size_t)OBS_DIM<INC> * ar.ho.n) : nullptr;
     bool in_seg = false, pending = false, to_h = false, valid = false, replay = false;
@@ -524,7 +528,7 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
                         for (int i = 0; i < NX; ++i) __stcg(ar.ho.X + (size_t)i * ar.ho.n + hx, e.X[i]);
                         __stcg(ar.ho.t + hx, e.t); __stcg(ar.ho.ret + hx, e.ret);
 #pragma unroll
-                        for (int i = 0; i < OBS_DIM<INC>; ++i) __stcg(ar.ho.obs + (size_t)i * ar.ho.n + hx, obs[i]);
+                        for (int i = 0; i < OBS_DIM<INC, SYM>; ++i) __stcg(ar.ho.obs + (size_t)i * ar.ho.n + hx, obs[i]);
                         if constexpr (INC)
 #pragma unroll
                             for (int i = 0; i < 3; ++i) __stcg(ho_u + (size_t)i * ar.ho.n + hx, last_u[i]);
@@ -603,7 +607,7 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
                         for (int i = 0; i < NX; ++i) e.X[i] = __ldcg(ar.ho.X + (size_t)i * ar.ho.n + hx);
                         e.t = __ldcg(ar.ho.t + hx); e.ret = __ldcg(ar.ho.ret + hx);
 #pragma unroll
-                        for (int i = 0; i < OBS_DIM<INC>; ++i) obs[i] = __ldcg(ar.ho.obs + (size_t)i * ar.ho.n + hx);
+                        for (int i = 0; i < OBS_DIM<INC, SYM>; ++i) obs[i] = __ldcg(ar.ho.obs + (size_t)i * ar.ho.n + hx);
                         if constexpr (INC)
 #pragma unroll
                             for (int i = 0; i < 3; ++i) last_u[i] = __ldcg(ho_u + (size_t)i * ar.ho.n + hx);
@@ -613,10 +617,10 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
 #pragma unroll
                             for (int i = 0; i < TRACK_CARRY; ++i) e.trk[i] = __ldcg(tk.ho + (size_t)i * ar.ho.n + hx);
                     } else {
-                        env_reset<TABS, GUST, TRACK, INC>(e, ar, row, obs, traj, last_u);
+                        env_reset<TABS, GUST, TRACK, INC, SYM>(e, ar, row, obs, traj, last_u);
                     }
                 } else {
-                    env_idle<INC>(e, ar, pv_base, obs, last_u);
+                    env_idle<INC, SYM>(e, ar, pv_base, obs, last_u);
                 }
                 replay = valid && ar.replay != nullptr && env == ar.replay_env;
                 in_seg = true;
@@ -627,15 +631,15 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
         if (!__syncthreads_or(in_seg || pending || stage < 3)) break;
         const bool mine = in_seg && !e.done && e.k < ke;
         if (actor_half && __any_sync(0xffffffffu, mine)) actor_forward<H>(actfn, w, L, lane, xb, obs, a);
-        if ((!stagger || !actor_half) && mine) env_step<TABS, GUST, TRACK, PER_ACTOR, INC>(e, ar, traj, actor, replay, a, obs, last_u);
+        if ((!stagger || !actor_half) && mine) env_step<TABS, GUST, TRACK, PER_ACTOR, INC, SYM>(e, ar, traj, actor, replay, a, obs, last_u);
         actor_half ^= stagger;
     }
 }
 
 // ---- cross-check kernel: every thread evaluates the whole MLP for its own env (any hidden size that fits) ------
 // PER_ACTOR as in rollout_kernel_persist
-// INC as in rollout_kernel_persist (instantiated without TRACK)
-template <bool TRACK = false, bool PER_ACTOR = false, bool INC = false>
+// INC, SYM as in rollout_kernel_persist (instantiated without TRACK)
+template <bool TRACK = false, bool PER_ACTOR = false, bool INC = false, bool SYM = false>
 __global__ void __launch_bounds__(128)
 rollout_kernel_simple(RolloutArgs ar, TrackArgs tk)
 {
@@ -653,24 +657,24 @@ rollout_kernel_simple(RolloutArgs ar, TrackArgs tk)
     const int env = ar.env_order ? ar.env_order[eslot] : eslot;
     Env e;
     e.tab = plant_tables_blob;
-    float obs[INC ? 10 : 7], a[3];
+    float obs[SYM ? 2 : INC ? 10 : 7], a[3];
     double last_u[3];                                  // INC only
     const int row = PER_ACTOR ? actor * ar.n_envs + env : env;
     env_bind<true>(e, ar, row, &plant_pv[0][0], (size_t)actor * ar.n_envs + env);
-    env_reset<false, true, TRACK, INC>(e, ar, row, obs, (size_t)actor * ar.n_envs + env, last_u);
+    env_reset<false, true, TRACK, INC, SYM>(e, ar, row, obs, (size_t)actor * ar.n_envs + env, last_u);
     const size_t traj = (size_t)actor * ar.n_envs + env;
     const bool replay = ar.replay != nullptr && env == ar.replay_env;
     while (!e.done) {
         actor_forward_simple(w, ar.sh, bufA, bufB, tid, 128, obs, a);
-        env_step<false, true, TRACK, PER_ACTOR, INC>(e, ar, traj, actor, replay, a, obs, last_u);   // (the gust schedule costs nothing that matters here)
+        env_step<false, true, TRACK, PER_ACTOR, INC, SYM>(e, ar, traj, actor, replay, a, obs, last_u);   // (the gust schedule costs nothing that matters here)
     }
     traj_store(e, ar, traj);
     if constexpr (TRACK) track_store(e, tk, traj);
 }
 
 // ---- Actor.forward for a batch of observations (same device functions as the rollout) --------------------------
-// S: observation entries (7, or 10 with incremental control)
-template <int H, int S = 7>
+// S: observation entries (7, 10 with incremental control, 2 with symmetric control); A: actions (3, or 1 with symmetric control)
+template <int H, int S = 7, int A = 3>
 __global__ void __launch_bounds__(128)
 actor_forward_kernel(const float* __restrict__ genome, int P, serl_actor_shape sh, const float* __restrict__ obs_in, int n,
                      float* __restrict__ act_out)
@@ -684,14 +688,18 @@ actor_forward_kernel(const float* __restrict__ genome, int P, serl_actor_shape s
     const int base = (blockIdx.x * 128 + (tid & ~31));
     if (base >= n) return;
     const int i = base + lane;
-    float obs[S], a[3];
+    float obs[S], a[A];
 #pragma unroll
     for (int k = 0; k < S; ++k) obs[k] = i < n ? obs_in[(size_t)i * S + k] : 0.f;
     actor_forward<H>(sh.activation, w, sh.num_layers, lane, xb, obs, a);
-    if (i < n) { act_out[(size_t)i * 3] = a[0]; act_out[(size_t)i * 3 + 1] = a[1]; act_out[(size_t)i * 3 + 2] = a[2]; }
+    if constexpr (A == 1) {
+        if (i < n) act_out[i] = a[0];
+    } else {
+        if (i < n) { act_out[(size_t)i * 3] = a[0]; act_out[(size_t)i * 3 + 1] = a[1]; act_out[(size_t)i * 3 + 2] = a[2]; }
+    }
 }
 
-template <int S = 7>
+template <int S = 7, int A = 3>
 __global__ void __launch_bounds__(128)
 actor_forward_kernel_simple(const float* __restrict__ genome, int P, serl_actor_shape sh, const float* __restrict__ obs_in, int n,
                             float* __restrict__ act_out)
@@ -705,10 +713,11 @@ actor_forward_kernel_simple(const float* __restrict__ genome, int P, serl_actor_
     __syncthreads();
     const int i = blockIdx.x * 128 + tid;
     if (i >= n) return;
-    float obs[S], a[3];
+    float obs[S], a[A];
     for (int k = 0; k < S; ++k) obs[k] = obs_in[(size_t)i * S + k];
     actor_forward_simple(w, sh, bufA, bufB, tid, 128, obs, a);
-    act_out[(size_t)i * 3] = a[0]; act_out[(size_t)i * 3 + 1] = a[1]; act_out[(size_t)i * 3 + 2] = a[2];
+    if constexpr (A == 1) act_out[i] = a[0];
+    else { act_out[(size_t)i * 3] = a[0]; act_out[(size_t)i * 3 + 1] = a[1]; act_out[(size_t)i * 3 + 2] = a[2]; }
 }
 // fitness[a] = mean over envs of returns[a, :]  (base/core/agent.py:245, np.mean over the evaluation axis)
 __global__ void fitness_mean_kernel(const double* __restrict__ returns, int pop, int n_envs, double* __restrict__ fitness)
@@ -791,11 +800,17 @@ static bool force_simple()
     return v;
 }
 
-// the uniform actors of the PH-LAB attitude task the kernels of this file implement (state_dim 10: incremental control)
+// the observation / action widths of the PH-LAB tasks: attitude control 7 -> 3, incremental 10 -> 3, symmetric 2 -> 1
+static bool task_dims(const serl_actor_shape& sh)
+{
+    return ((sh.state_dim == 7 || sh.state_dim == 10) && sh.action_dim == 3) || (sh.state_dim == 2 && sh.action_dim == 1);
+}
+static bool is_symmetric(const serl_actor_shape& sh) { return sh.state_dim == 2 && sh.action_dim == 1; }
+
+// the uniform actors of the PH-LAB tasks the kernels of this file implement
 static bool actor_shape_ok(const serl_actor_shape& sh)
 {
-    return (sh.state_dim == 7 || sh.state_dim == 10) && sh.action_dim == 3 && sh.hidden >= 2 && sh.hidden <= 256 && sh.num_layers >= 0 &&
-           sh.activation >= 0 && sh.activation <= 2;
+    return task_dims(sh) && sh.hidden >= 2 && sh.hidden <= 256 && sh.num_layers >= 0 && sh.activation >= 0 && sh.activation <= 2;
 }
 
 // CTA shape of the persistent kernel: `apc` genome slots x `wps` warps.  A slot's warps fly wps*32 envs of one actor;
@@ -825,7 +840,8 @@ static void choose_shape(int pop, int n_envs, int apc_max, int sms, int* apc_out
 }
 
 template <int H, bool TABS>
-static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust, bool stagger, bool per_actor, bool inc, cudaStream_t s)
+static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust, bool stagger, bool per_actor, bool inc, bool sym,
+                          cudaStream_t s)
 {
     const int sms = ar.sm_limit > 0 && ar.sm_limit < serl_device_sms() ? ar.sm_limit : serl_device_sms();
     int apc, wps;
@@ -844,8 +860,9 @@ static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust,
     // scratch: genomes in the shared-memory layout + hand-over records of the time-split schedule (stream-ordered)
     const size_t wt_bytes = (size_t)ar.pop * ar.P4 * 4;
     const long long hn = ar.n_tasks > ar.n_slots ? ar.n_slots * wps * 32 : 0;
-    // a record's observation: 7 floats, or 10 floats and last_u (3 f64) with incremental control (Handoff.obs)
-    const size_t ho_obs = inc ? 10 * 4 + 3 * 8 : 7 * 4;
+    // a record's observation: 7 floats, 10 floats and last_u (3 f64) with incremental control, 2 floats with symmetric
+    // control (Handoff.obs)
+    const size_t ho_obs = inc ? 10 * 4 + 3 * 8 : sym ? 2 * 4 : 7 * 4;
     const size_t ho_bytes = (size_t)hn * (NX * 8 + 8 + 8 + ho_obs + 4) + (size_t)(hn / 32) * 4 + (tk.out ? (size_t)hn * TRACK_CARRY * 8 + 8 : 0);
     void* scratch = nullptr;
     cudaError_t e = serl_scratch(SERL_SCRATCH_K1, s, wt_bytes + ho_bytes + 512, &scratch);
@@ -875,6 +892,8 @@ static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust,
                         (size_t)apc * wps * (inc ? actor_xbuf_floats(H, 10) : actor_xbuf_floats(H)) * 4;
     void (*const kernel)(RolloutArgs, TrackArgs) =
         inc         ? (per_actor ? rollout_kernel_persist<H, TABS, false, false, true, true> : rollout_kernel_persist<H, TABS, false, false, false, true>)
+        : sym       ? (per_actor ? rollout_kernel_persist<H, TABS, false, false, true, false, true>
+                                 : rollout_kernel_persist<H, TABS, false, false, false, false, true>)
         : tk.out    ? rollout_kernel_persist<H, TABS, true, true>
         : per_actor ? (gust ? rollout_kernel_persist<H, TABS, true, false, true> : rollout_kernel_persist<H, TABS, false, false, true>)
         : gust      ? rollout_kernel_persist<H, TABS, true> : rollout_kernel_persist<H, TABS, false>;
@@ -930,8 +949,7 @@ extern "C" int32_t serl_actor_tc_widths(const serl_actor_shape* shape, int32_t* 
 {
     if (!shape) return serl_fail(SERL_ERR_ARG, "serl_actor_tc_widths: null shape");
     const serl_actor_shape& sh = *shape;
-    const bool task = (sh.state_dim == 7 || sh.state_dim == 10) && sh.action_dim == 3 && sh.hidden >= 2 && sh.num_layers >= 1 && sh.activation >= 0 &&
-                      sh.activation <= 2;
+    const bool task = task_dims(sh) && sh.hidden >= 2 && sh.num_layers >= 1 && sh.activation >= 0 && sh.activation <= 2;
     if (!task || (actor_shape_ok(sh) && k1_fits(sh))) return 0;
     const int n = sh.num_layers + 1;
     if (!widths_out || cap < n) return serl_fail(SERL_ERR_ARG, "serl_actor_tc_widths: widths_out holds fewer than num_layers + 1 widths");
@@ -944,11 +962,12 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
 {
     const TrackArgs tk = {d.d_track, nullptr, d.d_cost};
     if (!actor_shape_ok(d.shape))
-        return serl_fail(SERL_ERR_ARG, "serl_rollout: unsupported actor shape (state_dim = 7 or 10, action_dim = 3, 2 <= hidden <= 256)");
+        return serl_fail(SERL_ERR_ARG, "serl_rollout: unsupported actor shape (state_dim = 7 or 10 with action_dim = 3, or 2 with 1; 2 <= hidden <= 256)");
     if (d.pop > 65535) return serl_fail(SERL_ERR_ARG, "serl_rollout: pop must be <= 65535 per call");       // grid.y of the simple kernel
     if (d.horizon >= (1 << 30)) return serl_fail(SERL_ERR_ARG, "serl_rollout: horizon too long");        // Handoff.k: steps | done << 30
     const int H = d.shape.hidden;
     const bool per_actor = (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) != 0, inc = (d.flags & SERL_ROLLOUT_INCREMENTAL) != 0;
+    const bool sym = (d.flags & SERL_ROLLOUT_SYMMETRIC) != 0;
     ar.weights = d.d_weights; ar.P = (int)serl_actor_num_params(&d.shape); ar.sh = d.shape;
     ar.P4 = (ar.P + 3) & ~3;
     if (!k1_warp(d.shape)) {
@@ -956,6 +975,7 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
         const size_t smem = (size_t)ar.P4 * 4 + 2ull * H * 128 * 4;
         return serl_launch("rollout_kernel launch",
                            inc         ? (per_actor ? rollout_kernel_simple<false, true, true> : rollout_kernel_simple<false, false, true>)
+                           : sym       ? (per_actor ? rollout_kernel_simple<false, true, false, true> : rollout_kernel_simple<false, false, false, true>)
                            : d.d_track ? rollout_kernel_simple<true> : per_actor ? rollout_kernel_simple<false, true> : rollout_kernel_simple<false>,
                            dim3((d.n_envs + 127) / 128, d.pop), 128, smem, s, ar, tk);
     }
@@ -971,10 +991,10 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
     warp_hidden(H, [&](auto h) {
         constexpr int HH = decltype(h)::value;
         if constexpr (HH == 128)          // the one size instantiated with the tables in global memory too
-            rc = tabs ? launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, per_actor, inc, s)
-                      : launch_persist<HH, false>(ar, tk, apc_max, gust, stagger, per_actor, inc, s);
+            rc = tabs ? launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, per_actor, inc, sym, s)
+                      : launch_persist<HH, false>(ar, tk, apc_max, gust, stagger, per_actor, inc, sym, s);
         else
-            rc = launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, per_actor, inc, s);
+            rc = launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, per_actor, inc, sym, s);
     });
     return rc;
 }
@@ -1007,6 +1027,18 @@ static int check_desc(const serl_rollout_desc& d)
         if (d.d_sensor_noise) return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) does not take d_sensor_noise");
     } else if (d.n_widths == 0 && d.shape.state_dim == 10) {
         return serl_fail(SERL_ERR_ARG, "serl_rollout: state_dim = 10 is the observation of incremental control: it needs SERL_ROLLOUT_INCREMENTAL");
+    }
+    // symmetric control: a 2-entry observation and one action, on the training instantiations of K1 and K1-TC only
+    if (d.flags & SERL_ROLLOUT_SYMMETRIC) {
+        if (d.shape.state_dim != 2 || d.shape.action_dim != 1)
+            return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) needs state_dim = 2 and action_dim = 1");
+        if (d.flags & SERL_ROLLOUT_INCREMENTAL)
+            return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) does not take SERL_ROLLOUT_INCREMENTAL");
+        if (d.d_track || d.d_cost) return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) does not take d_track / d_cost");
+        if (d.flags & SERL_ROLLOUT_GUST) return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) does not take SERL_ROLLOUT_GUST");
+        if (d.d_sensor_noise) return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) does not take d_sensor_noise");
+    } else if (d.n_widths == 0 && is_symmetric(d.shape)) {
+        return serl_fail(SERL_ERR_ARG, "serl_rollout: state_dim = 2, action_dim = 1 is the actor of symmetric control: it needs SERL_ROLLOUT_SYMMETRIC");
     }
     return SERL_OK;
 }
@@ -1088,18 +1120,20 @@ extern "C" int serl_actor_forward(const float* d_genome, const serl_actor_shape*
     cudaStream_t s = (cudaStream_t)stream;
     const int P = (int)serl_actor_num_params(shape), H = shape->hidden;
     const bool inc = shape->state_dim == 10;        // the observation of incremental control
+    const bool sym = is_symmetric(*shape);
     const int grid = (n + 127) / 128;
     const size_t smem = (size_t)((P + 3) & ~3) * 4;
     int rc = SERL_OK;
     const size_t warp_smem = smem + 4ull * (inc ? actor_xbuf_floats(H, 10) : actor_xbuf_floats(H)) * 4;      // genome + 4 warps' buffers
     const auto warp_launch = [&](auto h) {
-        rc = serl_launch("actor_forward_kernel", inc ? actor_forward_kernel<decltype(h)::value, 10> : actor_forward_kernel<decltype(h)::value>,
+        rc = serl_launch("actor_forward_kernel", inc ? actor_forward_kernel<decltype(h)::value, 10>
+                                                 : sym ? actor_forward_kernel<decltype(h)::value, 2, 1> : actor_forward_kernel<decltype(h)::value>,
                          grid, 128, warp_smem, s, d_genome, P, *shape, d_obs, n, d_actions);
     };
     // the warp kernel when it holds the genome, else the one-thread-per-env kernel (no static shared memory in either)
     if (!force_simple() && warp_smem <= SERL_SMEM_OPTIN && warp_hidden(H, warp_launch)) return rc;
     const size_t sm2 = smem + 2ull * H * 128 * 4;
     if (sm2 > SERL_SMEM_OPTIN) return serl_fail(SERL_ERR_UNSUPPORTED, "serl_actor_forward: genome + activations exceed shared memory");
-    return serl_launch("actor_forward_kernel", inc ? actor_forward_kernel_simple<10> : actor_forward_kernel_simple<>, grid, 128, sm2, s, d_genome,
-                       P, *shape, d_obs, n, d_actions);
+    return serl_launch("actor_forward_kernel", inc ? actor_forward_kernel_simple<10> : sym ? actor_forward_kernel_simple<2, 1> : actor_forward_kernel_simple<>,
+                       grid, 128, sm2, s, d_genome, P, *shape, d_obs, n, d_actions);
 }

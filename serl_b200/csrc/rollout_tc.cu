@@ -63,7 +63,7 @@ struct TcArgs {
     int stages;                    // K-slabs of one forward pass of 64 rows (all layers)
     int tile_floats;               // per-actor tile block
     int abuf_stride;               // row stride of the inter-layer activation buffer (floats)
-    int gWo;                       // genome: Wo[3][w_last] bo[3]
+    int gWo;                       // genome: Wo[3][w_last] bo[3] (symmetric control: Wo[1][w_last] bo[1])
     TcLayer ly[TC_MAXL];
 };
 
@@ -73,16 +73,20 @@ __device__ __forceinline__ float rn_tf32(float x)       // round to nearest TF32
 }
 
 // Row width of W0p in the small block and of the group's observations in shared memory: 8 floats for the 7-entry
-// observation, 12 for the 10 of incremental control (SERL_ROLLOUT_INCREMENTAL: + last_u); float4-aligned either way
-__host__ __device__ constexpr int tc_row(int S) { return S == 7 ? 8 : 12; }
+// observation, 12 for the 10 of incremental control (SERL_ROLLOUT_INCREMENTAL: + last_u), 4 for the 2 of symmetric control
+// (SERL_ROLLOUT_SYMMETRIC: 2 weights + bias + 0); float4-aligned in every case
+__host__ __device__ constexpr int tc_row(int S) { return S == 7 ? 8 : S == 2 ? 4 : 12; }
 
 // small block layout (floats): W0p[w0pad][8] (7 weights + bias; S = 10: [w0pad][12], 10 weights + bias + 0) | per layer l: b[npad] gamma[npad] beta[npad] |
 // Wo[3][npad of the last layer] | bo[4].  With two widths [w1, w2] this is W0p[w1][8] | b1 | gamma | beta | Wo | bo.
+// A genome with one output (symmetric control) fills Wo's row 0 and bo[0]; rows 1-2 and bo[1..3] are zero neurons, so the
+// output block's actions 1-2 are tanh(0) = 0 and nobody reads them.
 // Tile block: per layer l, n_stages K-slabs of stage_floats (pre-split TF32 hi / lo, canonical K-major core matrices).
 
 // K0-TC: genome (parameters() order: W0[w0,S] b0[w0], per layer W_l[w_l,w_{l-1}] b gamma beta, Wo[3,w_last] bo[3]) -> small
 // block + tile block.  Rows and columns past a layer's real width are zero neurons: zero weights, bias, gamma and beta.
-template <int S = 7>
+// A: the genome's outputs (3, or 1 with symmetric control); the small block's output rows past A are zero.
+template <int S = 7, int A = 3>
 __global__ void tc_layout_kernel(const float* __restrict__ w, int pop, int P, const __grid_constant__ TcArgs ar, float* __restrict__ small,
                                  float* __restrict__ tiles)
 {
@@ -110,10 +114,10 @@ __global__ void tc_layout_kernel(const float* __restrict__ w, int pop, int P, co
             v = n < L.w ? ga[L.gW + L.w * L.win + which * L.w + n] : 0.f;
         } else if (i < wo + 3 * last.npad) {
             const int r = i - wo, j = r / last.npad, n = r - j * last.npad;
-            v = n < last.w ? ga[ar.gWo + j * last.w + n] : 0.f;
+            v = n < last.w && (A == 3 || j < A) ? ga[ar.gWo + j * last.w + n] : 0.f;
         } else if (i < ar.small_floats) {
             const int r = i - wo - 3 * last.npad;
-            v = r < 3 ? ga[ar.gWo + 3 * last.w + r] : 0.f;
+            v = r < A ? ga[ar.gWo + A * last.w + r] : 0.f;
         } else {
             const int t = i - ar.small_floats;
             int l = 0;
@@ -211,6 +215,10 @@ __device__ __forceinline__ float tc_layer0(const float* wr, const float (&ob)[S]
         a = __fmaf_rn(wa.x, ob[0], a); a = __fmaf_rn(wa.y, ob[1], a); a = __fmaf_rn(wa.z, ob[2], a);
         a = __fmaf_rn(wa.w, ob[3], a); a = __fmaf_rn(wb.x, ob[4], a); a = __fmaf_rn(wb.y, ob[5], a);
         a = __fmaf_rn(wb.z, ob[6], a);
+        return a;
+    } else if constexpr (S == 2) {
+        float a = wa.z;                                              // bias (wb is not read)
+        a = __fmaf_rn(wa.x, ob[0], a); a = __fmaf_rn(wa.y, ob[1], a);
         return a;
     } else {
         const float4 wc = *reinterpret_cast<const float4*>(wr + 8);
@@ -643,8 +651,9 @@ __device__ __forceinline__ void tc_load_small(TcCtx& c, const TcArgs& ar, int ac
 // sums `tk` (serl_rollout_desc.d_track; instantiated with GUST only).  PER_ACTOR: env `env` of actor `actor` binds row
 // actor * n_envs + env of env_mode / ref_levels / ref_starts (SERL_ROLLOUT_PER_ACTOR_REFS; instantiated without TRACK).
 // INC: incremental control (SERL_ROLLOUT_INCREMENTAL; instantiated without GUST and TRACK): a 10-entry observation, layer 0
-// with 10 inputs, and the env's last_u
-template <int ACT, bool GUST, bool DEEP, bool TRACK = false, bool PER_ACTOR = false, bool INC = false>
+// with 10 inputs, and the env's last_u.  SYM: symmetric control (SERL_ROLLOUT_SYMMETRIC; instantiated without GUST and
+// TRACK): a 2-entry observation, layer 0 with 2 inputs, and action 0 of the output block as the elevator
+template <int ACT, bool GUST, bool DEEP, bool TRACK = false, bool PER_ACTOR = false, bool INC = false, bool SYM = false>
 __global__ void __launch_bounds__(2 * TC_THREADS, 1)
 rollout_kernel_tc(const __grid_constant__ TcArgs ar, TrackArgs tk)
 {
@@ -653,7 +662,7 @@ rollout_kernel_tc(const __grid_constant__ TcArgs ar, TrackArgs tk)
     __shared__ uint32_t shared_state[2];
     TcCtx c;
     plant_tab_check(smem_raw);
-    tc_setup<DEEP, OBS_DIM<INC>>(c, ar, smem_raw, bars, shared_state);
+    tc_setup<DEEP, OBS_DIM<INC, SYM>>(c, ar, smem_raw, bars, shared_state);
     const RolloutArgs& r = ar.r;
     const real* tab = reinterpret_cast<const real*>(smem_raw);
     const real* pv_base = tab + PT_TOTAL;
@@ -668,21 +677,21 @@ rollout_kernel_tc(const __grid_constant__ TcArgs ar, TrackArgs tk)
         const int env = valid ? (r.env_order ? r.env_order[eslot] : eslot) : 0;
         Env e;
         e.tab = tab;
-        float obs[OBS_DIM<INC>], a[3];
+        float obs[OBS_DIM<INC, SYM>], a[3];
         double last_u[3];                              // INC only
         if (valid) {
             const int row = PER_ACTOR ? actor * r.n_envs + env : env;
             env_bind<GUST>(e, r, row, pv_base, (size_t)actor * r.n_envs + env);
-            env_reset<true, GUST, TRACK, INC>(e, r, row, obs, (size_t)actor * r.n_envs + env, last_u);
+            env_reset<true, GUST, TRACK, INC, SYM>(e, r, row, obs, (size_t)actor * r.n_envs + env, last_u);
         } else {
-            env_idle<INC>(e, r, pv_base, obs, last_u);
+            env_idle<INC, SYM>(e, r, pv_base, obs, last_u);
         }
         const size_t traj = (size_t)actor * r.n_envs + env;
         const bool replay = valid && r.replay != nullptr && env == r.replay_env;
         while (group_any(c.grp, !e.done)) {
-            if constexpr (DEEP) tc_actor_forward_deep<ACT, OBS_DIM<INC>>(c, ar, tiles_actor, obs, a);
-            else tc_actor_forward<ACT, OBS_DIM<INC>>(c, ar, tiles_actor, obs, a);
-            if (!e.done) env_step<true, GUST, TRACK, PER_ACTOR, INC>(e, r, traj, actor, replay, a, obs, last_u);
+            if constexpr (DEEP) tc_actor_forward_deep<ACT, OBS_DIM<INC, SYM>>(c, ar, tiles_actor, obs, a);
+            else tc_actor_forward<ACT, OBS_DIM<INC, SYM>>(c, ar, tiles_actor, obs, a);
+            if (!e.done) env_step<true, GUST, TRACK, PER_ACTOR, INC, SYM>(e, r, traj, actor, replay, a, obs, last_u);
         }
         if (valid) traj_store(e, r, traj);
         if constexpr (TRACK) if (valid) track_store(e, tk, traj);
@@ -723,9 +732,9 @@ extern "C" int64_t serl_actor_num_params_wide(const int32_t* widths, int32_t n_w
 
 // Checks the widths and sizes the layer table, the kernel layout and the shared memory (all before any CUDA call), then
 // brings the genomes into the kernel layout (K0-TC) in the stream's scratch buffer.
-// S: observation entries (7, or 10 with incremental control)
+// S: observation entries (7, 10 with incremental control, 2 with symmetric control); A: actions (3, or 1 with symmetric control)
 static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t* widths, int n_widths, cudaStream_t s, size_t* smem_out,
-                      int S = 7)
+                      int S = 7, int A = 3)
 {
     if (!widths || n_widths < 2 || n_widths > TC_MAXL + 1)
         return serl_fail(SERL_ERR_UNSUPPORTED, "wide actors: the tensor-core path takes 2 to 9 widths [w0, w1, ..., w_{n-1}]");
@@ -766,7 +775,7 @@ static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t
     if (*smem_out > SERL_SMEM_OPTIN - 256)
         return serl_fail(SERL_ERR_UNSUPPORTED, deep ? "wide actors: tables + rings + activation buffer exceed the shared memory of an SM"
                                                     : "wide actors: tables + parameters + rings exceed the shared memory of an SM");
-    const int P = (int)serl_actor_num_params_wide(widths, n_widths) + (S - 7) * widths[0];
+    const int P = (int)serl_actor_num_params_wide(widths, n_widths) + (S - 7) * widths[0] + (A - 3) * (widths[n_widths - 1] + 1);
     const size_t small_bytes = (size_t)pop * ar.small_floats * 4;
     const size_t tile_bytes = (size_t)pop * ar.tile_floats * 4;
     void* scratch = nullptr;
@@ -777,8 +786,8 @@ static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t
     ar.small = small; ar.tiles = tiles;
     const long long total = (long long)pop * ((long long)ar.small_floats + ar.tile_floats);
     const int grid = (int)((total + 255) / 256 < 8192 ? (total + 255) / 256 : 8192);
-    return serl_launch("tc_layout_kernel", S == 7 ? tc_layout_kernel<7> : tc_layout_kernel<10>, grid, 256, 0, s, d_weights, pop, P, ar,
-                       small, tiles);
+    return serl_launch("tc_layout_kernel", S == 7 ? tc_layout_kernel<7> : S == 2 ? tc_layout_kernel<2, 1> : tc_layout_kernel<10>, grid, 256, 0,
+                       s, d_weights, pop, P, ar, small, tiles);
 }
 
 // K1-TC launch (serl_rollout_run has checked the descriptor and built the env / output arguments `r`)
@@ -788,8 +797,8 @@ int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, cudaStream
     memset(&ar, 0, sizeof(ar));
     ar.r = r;
     size_t smem = 0;
-    const bool inc = (d.flags & SERL_ROLLOUT_INCREMENTAL) != 0;
-    const int rc = tc_prepare(ar, d.d_weights, d.pop, d.widths, d.n_widths, s, &smem, inc ? 10 : 7);
+    const bool inc = (d.flags & SERL_ROLLOUT_INCREMENTAL) != 0, sym = (d.flags & SERL_ROLLOUT_SYMMETRIC) != 0;
+    const int rc = tc_prepare(ar, d.d_weights, d.pop, d.widths, d.n_widths, s, &smem, inc ? 10 : sym ? 2 : 7, sym ? 1 : 3);
     if (rc != SERL_OK) return rc;
     ar.n_chunks = (d.n_envs + TC_THREADS - 1) / TC_THREADS;
     ar.n_tasks = (long long)d.pop * ar.n_chunks;
@@ -821,11 +830,21 @@ int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, cudaStream
          {rollout_kernel_tc<SERL_ACT_ELU, false, false, false, true, true>, rollout_kernel_tc<SERL_ACT_ELU, false, true, false, true, true>}},
         {{rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, false, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, false, true>},
          {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, true, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, true, true>}}};
+    static void (*const sym_kernels[3][2][2])(TcArgs, TrackArgs) = {   // [SERL_ACT_*][per actor][deep]
+        {{rollout_kernel_tc<SERL_ACT_TANH, false, false, false, false, false, true>, rollout_kernel_tc<SERL_ACT_TANH, false, true, false, false, false, true>},
+         {rollout_kernel_tc<SERL_ACT_TANH, false, false, false, true, false, true>, rollout_kernel_tc<SERL_ACT_TANH, false, true, false, true, false, true>}},
+        {{rollout_kernel_tc<SERL_ACT_ELU, false, false, false, false, false, true>, rollout_kernel_tc<SERL_ACT_ELU, false, true, false, false, false, true>},
+         {rollout_kernel_tc<SERL_ACT_ELU, false, false, false, true, false, true>, rollout_kernel_tc<SERL_ACT_ELU, false, true, false, true, false, true>}},
+        {{rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, false, false, true>,
+          rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, false, false, true>},
+         {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, true, false, true>,
+          rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, true, false, true>}}};
     const TrackArgs tk = {d.d_track, nullptr, d.d_cost};
     const bool gust = (d.flags & SERL_ROLLOUT_GUST) != 0, deep = ar.n_layers > 1;
     const bool per_actor = (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) != 0;
     // one CTA = the two groups of TC_THREADS threads
     return serl_launch("rollout_kernel_tc launch", inc ? inc_kernels[d.shape.activation][per_actor][deep]
+                                                   : sym ? sym_kernels[d.shape.activation][per_actor][deep]
                                                    : d.d_track ? track_kernels[d.shape.activation][deep]
                                                    : (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) ? per_actor_kernels[d.shape.activation][gust][deep]
                                                                                              : kernels[d.shape.activation][gust][deep],

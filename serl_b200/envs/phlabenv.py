@@ -37,12 +37,23 @@ class CitationEnv:
     dt = 0.01
 
     def __init__(self, configuration: str = None, mode: str = 'nominal'):
-        configuration = configuration or 'attitude'
-        if 'attitude' not in configuration.lower():
-            raise ValueError("the B200 rollout engine implements the 'attitude' configuration (3 actions, obs = 3 errors + p,q,r,alpha)")
-        self.n_actions = 3
-        self.obs_idx = [0, 1, 2, 4]
+        configuration = (configuration or 'attitude').lower()
         m = mode.lower()
+        # the configuration token (:84-97): 'symmetric' (checked first, as the reference does) flies the elevator alone on
+        # obs = [e_theta, q]; 'attitude' the three surfaces
+        self.symmetric = 'symmetric' in configuration
+        if self.symmetric:
+            if 'incremental' in m:
+                raise ValueError("the B200 rollout engine does not fly symmetric control with incremental control "
+                                 "('symmetric' with mode %r: 3 observations)" % mode)
+            self.n_actions = 1
+            self.obs_idx = [1]
+        elif 'attitude' in configuration:
+            self.n_actions = 3
+            self.obs_idx = [0, 1, 2, 4]
+        else:
+            raise ValueError("the B200 rollout engine does not fly full-state control (configuration %r: 13 observations); it "
+                             "implements the 'attitude' and 'symmetric' configurations" % configuration)
         # incremental control (:174-175): any mode containing 'incremental' flies the nominal build, the first test of the
         # reference's chain (:99-103), so 'gust-incremental' has no gust and 'noise-incremental' no sensor noise
         self.incremental = 'incremental' in m
@@ -73,7 +84,7 @@ class CitationEnv:
         # incremental control: + the actuator state last_u (:214-220)
         self.n_obs = len(self.obs_idx) + (2 if self.incremental else 1) * self.n_actions
         self.error = np.zeros((self.n_actions))
-        self.error_scaler = (6 / np.pi * np.array([1., 1., 4.]))[:self.n_actions]
+        self.error_scaler = 6 / np.pi * np.array([1.]) if self.n_actions == 1 else (6 / np.pi * np.array([1., 1., 4.]))[:self.n_actions]
         self.max_bound = np.ones(self.error.shape)
         self.levels = self.starts = None
         self._X = None
@@ -128,17 +139,22 @@ class CitationEnv:
         """consume the global np.random stream like init_ref (:303-345) and return (levels[2,6], starts[2,6])."""
         levels = np.zeros((2, refsig.N_BLOCKS))
         starts = np.zeros((2, refsig.N_BLOCKS))
-        for c in range(2):
+        for c in range(1 if self.symmetric else 2):         # symmetric control draws the theta reference alone (:304-313)
             grid = np.linspace(-refsig.AMPL[c], refsig.AMPL[c], refsig.N_LEVELS)
             lv = grid[np.random.randint(0, refsig.N_LEVELS, size=refsig.N_BLOCKS)]
             lv[0] = 0.0
-            block_w, _, jitter = refsig.widths(self.t_max)
+            block_w, _, jitter = refsig.widths(self.t_max, self.symmetric)
             st = block_w * np.arange(refsig.N_BLOCKS) + np.random.uniform(-jitter, jitter, size=refsig.N_BLOCKS)
             st[0] = 0.0
             levels[c], starts[c] = lv, st
         return levels, starts
 
     def init_ref(self, **kwargs):
+        if self.symmetric:      # the theta reference alone, offset by the constant trim 0.22 deg (:304-313)
+            self.levels, self.starts = self.draw_reference()
+            self.user_smooth_width = None
+            self.ref = [_RefSignal(self.levels[0], self.starts[0], self.theta_trim, refsig.widths(self.t_max, True)[1], self.t_max)]
+            return
         self.theta_trim = np.rad2deg(self.x[7])
         sw = refsig.widths(self.t_max)[1]
         self.user_smooth_width = None
@@ -203,7 +219,7 @@ class CitationEnv:
 
     def get_reward(self):
         self.calc_reference_value()
-        self.error[:self.n_actions] = self.ref_values - np.asarray([self.theta, self.phi, self.beta])
+        self.error[:self.n_actions] = self.ref_values - np.asarray([self.theta, self.phi, self.beta])[:self.n_actions]
         reward_vec = np.abs(np.clip(self.error_scaler * self.error, -self.max_bound, self.max_bound))
         return -reward_vec.sum() / self.error.shape[0]
 

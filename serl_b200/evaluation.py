@@ -54,6 +54,8 @@ def condition_env(condition, t_max=T_MAX):
     env = config.select_env(condition if '_' in condition else 'PHlab_attitude_' + condition)
     if env.incremental:
         raise ValueError('evaluation: the evaluation suite flies absolute control only, not incremental control (%s)' % condition)
+    if env.symmetric:
+        raise ValueError('evaluation: the evaluation suite flies attitude control only, not symmetric control (%s)' % condition)
     env.set_eval_mode(t_max)
     return env
 
@@ -184,6 +186,8 @@ def evaluate_population(genomes, shape, conditions, user_refs_lst, num_trails=1,
     launches (same results)."""
     if shape.state_dim == rollout.INCREMENTAL_STATE_DIM:
         raise ValueError('evaluate_population: the evaluation suite flies absolute control only, not incremental control')
+    if rollout.is_symmetric(shape):
+        raise ValueError('evaluate_population: the evaluation suite flies attitude control only, not symmetric control')
     dev = device or torch.device('cuda', torch.cuda.current_device())
     refs = user_refs_lst[:num_trails + 1]
     T, C = len(refs), len(conditions)

@@ -106,6 +106,8 @@ class OperatorRunner:
     def __init__(self, args, condition='nominal', num_trails=0, device=None):
         if getattr(args, 'state_dim', None) == rollout.INCREMENTAL_STATE_DIM:
             raise ValueError('OperatorRunner: the operator study flies absolute control only, not incremental control')
+        if (getattr(args, 'state_dim', None), getattr(args, 'action_dim', None)) == (rollout.SYMMETRIC_STATE_DIM, rollout.SYMMETRIC_ACTION_DIM):
+            raise ValueError('OperatorRunner: the operator study flies attitude control only, not symmetric control')
         self.args = args
         self.num_trails = int(num_trails)
         self.device = device or torch.device('cuda', torch.cuda.current_device())

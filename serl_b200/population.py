@@ -25,8 +25,9 @@ class PopulationList(list):
             a.actor.bind(self.genomes[i])
             a.index = i
         # GeneticAgent.buffer / .critical_buffer of every actor: two device tensors, allocated on first use
-        self.buffers = replay_memory.PopulationBuffers(args.pop_size, args.individual_bs, self.device, args.state_dim)
-        self.critical_buffers = replay_memory.PopulationBuffers(args.pop_size, args.individual_bs, self.device, args.state_dim)
+        self.buffers = replay_memory.PopulationBuffers(args.pop_size, args.individual_bs, self.device, args.state_dim, args.action_dim)
+        self.critical_buffers = replay_memory.PopulationBuffers(args.pop_size, args.individual_bs, self.device, args.state_dim,
+                                                                args.action_dim)
         for i, a in enumerate(agents):
             a.buffer = replay_memory.ActorBuffer(self.buffers, i)
             a.critical_buffer = replay_memory.ActorBuffer(self.critical_buffers, i)

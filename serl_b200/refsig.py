@@ -18,19 +18,24 @@ N_LEVELS = 10
 AMPL = (30.0, 20.0)   # theta, phi [deg]
 
 
-def widths(t_max=20):
-    """(block width, smooth width, timing jitter) of init_ref (envs/phlabenv.py:321-335) for an episode of t_max seconds."""
+def widths(t_max=20, symmetric=False):
+    """(block width, smooth width, timing jitter) of init_ref (envs/phlabenv.py:321-335) for an episode of t_max seconds.
+    symmetric=True: the theta-only reference of symmetric control (:304-313), smooth width t_max // 6.7 (2 s at 20 s, 11 s at
+    80 s) and jitter t_max // 500, a floor division that is 0 for any episode shorter than 500 s."""
+    if symmetric:
+        return float(t_max // 5), float(t_max // 6.7), float(t_max // 500)
     return float(t_max // 5), float(t_max // 6), t_max / 500.
 
 
-def make_ref_params(n_envs, seed_base=7_000_000, t_max=20):
-    """levels[n_envs, 2, N_BLOCKS] (deg, without the theta trim offset), starts[n_envs, 2, N_BLOCKS] (s)."""
-    block_w, _, jitter = widths(t_max)
+def make_ref_params(n_envs, seed_base=7_000_000, t_max=20, symmetric=False):
+    """levels[n_envs, 2, N_BLOCKS] (deg, without the theta trim offset), starts[n_envs, 2, N_BLOCKS] (s).
+    symmetric=True draws the theta channel alone (symmetric control's parameters); the phi channel stays zero."""
+    block_w, _, jitter = widths(t_max, symmetric)
     levels = np.zeros((n_envs, 2, N_BLOCKS))
     starts = np.zeros((n_envs, 2, N_BLOCKS))
     for e in range(n_envs):
         rs = np.random.RandomState(seed_base + e)
-        for c in range(2):
+        for c in range(1 if symmetric else 2):
             grid = np.linspace(-AMPL[c], AMPL[c], N_LEVELS)
             lv = grid[rs.randint(0, N_LEVELS, size=N_BLOCKS)]
             lv[0] = 0.0

@@ -8,7 +8,7 @@ import functools
 import numpy as np
 import torch
 
-from . import _native
+from . import _native, refsig
 from ._native import FAULTS, MODE_GUST, MODE_GUST_UP, PLANT_VARIANTS, REPLAY_COLS, TRACE_COLS, TRACK_COLS
 
 HORIZON = 2001          # envs/phlabenv.py:82,181,392: t_max = 20 s, dt = 0.01, done checked before t += dt
@@ -17,22 +17,29 @@ TRACE_X, TRACE_U, TRACE_R, TRACE_A, TRACE_ERR = slice(0, 12), slice(12, 15), 15,
 # the observation of incremental control (envs/phlabenv.py:214-220): the 7 of the absolute mode + last_u.  A shape with this
 # state_dim flies with SERL_ROLLOUT_INCREMENTAL
 INCREMENTAL_STATE_DIM = 10
+# the actor of symmetric control (envs/phlabenv.py:86-89): obs = [e_theta, q] -> the elevator.  A shape with these widths flies
+# with SERL_ROLLOUT_SYMMETRIC
+SYMMETRIC_STATE_DIM, SYMMETRIC_ACTION_DIM = 2, 1
 
 
-# The replay row of an observation of S entries (SERL_REPLAY_COLS_OF): obs S | action 3 | next_obs S | reward | done | cost.
-# Every buffer stores the transition, the row without its last column (the cost flag).
-def replay_dims(state_dim=7):
+def is_symmetric(shape):
+    return shape.state_dim == SYMMETRIC_STATE_DIM and shape.action_dim == SYMMETRIC_ACTION_DIM
+
+
+# The replay row of an observation of S entries and A actions (SERL_REPLAY_COLS_SA): obs S | action A | next_obs S | reward |
+# done | cost.  Every buffer stores the transition, the row without its last column (the cost flag).
+def replay_dims(state_dim=7, action_dim=3):
     """widths of the fields of a replay row: obs, action, next_obs, reward, done, cost"""
-    return (state_dim, 3, state_dim, 1, 1, 1)
+    return (state_dim, action_dim, state_dim, 1, 1, 1)
 
 
-def replay_cols(state_dim=7):
-    return sum(replay_dims(state_dim))
+def replay_cols(state_dim=7, action_dim=3):
+    return sum(replay_dims(state_dim, action_dim))
 
 
-def transition_cols(state_dim=7):
+def transition_cols(state_dim=7, action_dim=3):
     """columns of a stored transition, which is also the column of a replay row's cost flag"""
-    return replay_cols(state_dim) - 1
+    return replay_cols(state_dim, action_dim) - 1
 
 
 TRANSITION_COLS = REPLAY_COST = transition_cols(7)       # SERL_REPLAY_COLS - 1
@@ -117,6 +124,9 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     steps whose cost flag (the replay rows' last column) is set (serl_rollout_desc.d_cost).
     shape.state_dim = INCREMENTAL_STATE_DIM flies incremental control (SERL_ROLLOUT_INCREMENTAL: rate commands integrated into the
     deflection, obs + last_u, replay rows of replay_cols(10) columns; on K1 and K1-TC, without track, cost, gust or sensor_noise).
+    A 2 -> 1 shape (is_symmetric) flies symmetric control (SERL_ROLLOUT_SYMMETRIC: the elevator alone, obs = [e_theta, q], the theta
+    reference of refsig.make_ref_params(symmetric=True) with its smooth width, action_noise [pop, n_envs, horizon, 1], replay rows
+    of replay_cols(2, 1) columns; on K1 and K1-TC, without track, cost, gust or sensor_noise).
     widths=[w0, w1, ..., w_{n-1}] (2 to 9 widths): width-list actors on the tensor-core kernel K1-TC (csrc/rollout_tc.cu); `shape`
     then only supplies the activation.  widths=None flies the uniform actor `shape` on K1, or on K1-TC with [h] * (L + 1) when its
     genome does not fit K1's kernels (tc_widths)."""
@@ -126,7 +136,8 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
         widths = tc_widths(shape)
     pop, P = weights.shape
     assert weights.dtype == torch.float32 and weights.is_contiguous()
-    assert P == (num_params_wide(widths, shape.state_dim) if widths else num_params(shape)), (P, widths)
+    assert P == (num_params_wide(widths, shape.state_dim, shape.action_dim) if widths else num_params(shape)), (P, widths)
+    sym = is_symmetric(shape)
     per_actor = env_mode.dim() == 2
     n_envs = env_mode.shape[-1]
     block = (pop, n_envs) if per_actor else (n_envs,)
@@ -134,7 +145,7 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     assert ref_levels.shape == block + (2, 6) and ref_levels.dtype == torch.float64 and ref_levels.is_contiguous()
     assert ref_starts.shape == block + (2, 6) and ref_starts.dtype == torch.float64 and ref_starts.is_contiguous()
     if action_noise is not None:
-        assert action_noise.shape == (pop, n_envs, horizon, 3) and action_noise.dtype == torch.float32 and action_noise.is_contiguous()
+        assert action_noise.shape == (pop, n_envs, horizon, shape.action_dim if sym else 3) and action_noise.dtype == torch.float32 and action_noise.is_contiguous()
     if env_order is not None:
         assert env_order.shape == (n_envs,) and env_order.dtype == torch.int32 and env_order.is_cuda
     dev = weights.device
@@ -146,7 +157,7 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
         r.trace = None
         r.smoothness = None
         r.actions = torch.empty((pop, n_envs, horizon, 3), dtype=torch.float32, device=dev) if actions else None
-        r.replay = torch.empty((pop, horizon, replay_cols(shape.state_dim)), dtype=torch.float32, device=dev) if replay_env is not None else None
+        r.replay = torch.empty((pop, horizon, replay_cols(shape.state_dim, shape.action_dim)), dtype=torch.float32, device=dev) if replay_env is not None else None
         r.status = torch.zeros((1,), dtype=torch.int32, device=dev) if status else None
         r.track = torch.empty((pop, n_envs, TRACK_COLS), dtype=torch.float64, device=dev) if track else None
         r.cost = torch.empty((pop, n_envs), dtype=torch.int32, device=dev) if cost else None
@@ -162,7 +173,9 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     d.d_returns, d.d_steps, d.d_fitness, d.d_trace, d.d_actions = p(r.returns), p(r.steps), p(r.fitness), p(r.trace), p(getattr(r, 'actions', None))
     if t_max is not None:      # evaluation mode (envs/phlabenv.py:295-301): longer episodes, wider reference transitions
         d.t_max = float(t_max)
-        d.smooth_width = float(smooth_width if smooth_width is not None else float(t_max // 6))
+        d.smooth_width = float(smooth_width if smooth_width is not None else refsig.widths(t_max, sym)[1])
+    elif sym:                  # symmetric control's training episode: 20 s with 2 s transitions (t_max // 6.7)
+        d.t_max, d.smooth_width = 20.0, float(smooth_width if smooth_width is not None else refsig.widths(20, True)[1])
     d.d_env_order = p(env_order)
     d.d_replay, d.replay_env = p(getattr(r, 'replay', None)), int(replay_env if replay_env is not None else 0)
     d.d_status = p(getattr(r, 'status', None))
@@ -176,7 +189,8 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
         d.d_sensor_noise = p(sensor_noise)
     d.flags = ((_native.ROLLOUT_GUST if gust else 0) | (_native.ROLLOUT_STAGGER if stagger else 0)      # gust: mode_code(...) & MODE_GUST
                | (_native.ROLLOUT_PER_ACTOR_REFS if per_actor else 0)
-               | (_native.ROLLOUT_INCREMENTAL if shape.state_dim == INCREMENTAL_STATE_DIM else 0))
+               | (_native.ROLLOUT_INCREMENTAL if shape.state_dim == INCREMENTAL_STATE_DIM else 0)
+               | (_native.ROLLOUT_SYMMETRIC if sym else 0))
     if widths:
         warr = np.asarray(widths, dtype=np.int32)       # host array, alive until the call returns
         d.widths, d.n_widths = warr.ctypes.data, len(widths)
@@ -193,11 +207,11 @@ def tc_widths(shape):
     return out[:n].tolist() if n else None
 
 
-def num_params_wide(widths, state_dim=7):
-    """parameters of a width-list actor; serl_actor_num_params_wide counts a 7-entry observation, incremental control's
-    layer 0 has 3 * w0 weights more"""
+def num_params_wide(widths, state_dim=7, action_dim=3):
+    """parameters of a width-list actor; serl_actor_num_params_wide counts a 7-entry observation and 3 actions: incremental
+    control's layer 0 has 3 * w0 weights more, symmetric control's 5 * w0 fewer and its output layer 2 * (w_last + 1) fewer"""
     n = int(_native.lib().serl_actor_num_params_wide(np.asarray(widths, dtype=np.int32).ctypes, len(widths)))
-    return n + (state_dim - 7) * int(widths[0])
+    return n + (state_dim - 7) * int(widths[0]) + (action_dim - 3) * (int(widths[-1]) + 1)
 
 
 def actor_forward_wide(genome, widths, activation, obs):

@@ -36,7 +36,7 @@ import torch
 from . import evaluation, td3_fused
 from .core import agent as agent_mod
 from ._native import NativeError
-from .rollout import INCREMENTAL_STATE_DIM, actor_shape
+from .rollout import INCREMENTAL_STATE_DIM, SYMMETRIC_ACTION_DIM, SYMMETRIC_STATE_DIM, actor_shape
 
 
 class RNGState:
@@ -109,6 +109,8 @@ class Sweep:
         for i, (p, _) in enumerate(runs):
             if p.state_dim == INCREMENTAL_STATE_DIM:
                 raise ValueError('Sweep: run %d flies incremental control (state_dim 10), which fused_td3 (K7) does not train' % i)
+            if (p.state_dim, p.action_dim) == (SYMMETRIC_STATE_DIM, SYMMETRIC_ACTION_DIM):
+                raise ValueError('Sweep: run %d flies symmetric control (state_dim 2, action_dim 1), which fused_td3 (K7) does not train' % i)
             if not getattr(p, 'fused_td3', False):
                 raise ValueError('Sweep: run %d does not set fused_td3 (the sweep trains every RL half in one K7 launch)' % i)
             if mixed_shapes:

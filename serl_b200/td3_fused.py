@@ -12,7 +12,7 @@ import torch
 
 from . import _native
 from .core import td3
-from .rollout import INCREMENTAL_STATE_DIM, TRANSITION_COLS, actor_shape
+from .rollout import INCREMENTAL_STATE_DIM, SYMMETRIC_ACTION_DIM, SYMMETRIC_STATE_DIM, TRANSITION_COLS, actor_shape
 
 # steps per launch: keeps every launch well under a second at the largest population
 LAUNCH_STEPS = 8192
@@ -43,6 +43,9 @@ class FusedTD3(td3.TD3):
         if args.state_dim == INCREMENTAL_STATE_DIM:
             raise ValueError('fused_td3: K7 trains the actor of absolute control (state_dim 7); incremental control (state_dim 10) '
                              'trains with the torch TD3 (fused_td3=False)')
+        if (args.state_dim, args.action_dim) == (SYMMETRIC_STATE_DIM, SYMMETRIC_ACTION_DIM):
+            raise ValueError('fused_td3: K7 trains the actor of attitude control (3 actions); symmetric control (state_dim 2, '
+                             'action_dim 1) trains with the torch TD3 (fused_td3=False)')
         super().__init__(args)
         if torch.device(args.device).type != 'cuda':
             raise _native.NativeError('FusedTD3 needs a CUDA device (no CPU fallback)')
