@@ -5,8 +5,11 @@
     python examples/evaluate.py -agent_name <run dir> -env be,jr -eval_rl
 
 `-agent_name` is a run directory holding files/config.yaml and the checkpoints Agent.save_agent writes (files/evo_nets.pkl,
-files/rl_net.pkl).  `-env` takes one condition ('nominal', 'be', ..., or 'PHlab_attitude_<condition>'), a comma list, or
-'all' (serl_b200.evaluation.CONDITIONS).  -eval_pop flies the whole population on every condition in one rollout launch per
+files/rl_net.pkl).  `-env` takes one condition ('nominal', 'be', ..., or a full env name 'PHlab_<configuration>_<mode>'), a
+comma list of one configuration, 'all' (serl_b200.evaluation.CONDITIONS) or 'PHlab_<configuration>_all'.  The actor's
+state_dim / action_dim come from the env, as in base/evaluate.py: 'PHlab_attitude_incremental' evaluates an incremental-control
+run (10 -> 3), 'PHlab_symmetric_<mode>' a symmetric-control run (2 -> 1), whose references are evaluation.symmetric_refs
+seeded from -seed.  Output folders are named after the mode token (figures/incremental/, figures/be/).  -eval_pop flies the whole population on every condition in one rollout launch per
 sensor-noise group (evaluation.evaluate_population); -eval_actor and -eval_rl fly one actor per condition
 (evaluation.validate_agent).  base/evaluate.py evaluates one condition per run and seeds every run alike, so every
 condition here flies the same references and draws its sensor noise from the same generator state.  -save_stats writes
@@ -27,7 +30,8 @@ from serl_b200 import evaluation, rollout              # noqa: E402
 from serl_b200.parameters import Parameters           # noqa: E402
 
 parser = argparse.ArgumentParser()
-parser.add_argument('-env', type=str, default='nominal', help="a condition, a comma list of conditions, or 'all'")
+parser.add_argument('-env', type=str, default='nominal',
+                    help="a condition, a full env name PHlab_<configuration>_<mode>, PHlab_<configuration>_all, a comma list, or 'all'")
 parser.add_argument('-seed', type=int, default=7)
 parser.add_argument('-agent_name', type=str, required=True, help='run directory (files/config.yaml, files/*.pkl)')
 parser.add_argument('-eval_pop', default=False, action='store_true')
@@ -41,9 +45,13 @@ parser.add_argument('-num_trails', default=1, type=int)
 
 
 def conditions(text):
-    if text == 'all':
-        return list(evaluation.CONDITIONS)
-    return [c.split('_')[-1] if c.lower().startswith('phlab_') else c for c in text.split(',') if c]
+    try:
+        return evaluation.env_conditions(text)
+    except ValueError as e:
+        raise SystemExit(str(e))
+
+
+folder, env_dims = evaluation.condition_folder, evaluation.env_dims
 
 
 def seed_all(seed):
@@ -59,10 +67,10 @@ def actor_shape(params):
 
 def fly_one(genome, shape, cond, refs, cla, label, state):
     np.random.set_state(state)          # this condition's sensor noise, as a run of base/evaluate.py on it alone draws it
-    data, stats = evaluation.validate_agent(genome, shape, evaluation.condition_env(cond), refs, cla.num_trails)
+    data, stats = evaluation.validate_agent(genome, shape, evaluation.condition_env(cond, shape=shape), refs, cla.num_trails)
     print(f'{cond} {label}: nMAE: {stats.nmae:0.1f}% with STD: {stats.nmae_sd:0.1f}   Smoothness: {stats.sm:0.0f} with STD: {stats.sm_sd:0.1f}')
     if cla.save_trajectory:
-        evaluation.write_trajectory(cla.agent_name, cond, data)
+        evaluation.write_trajectory(cla.agent_name, folder(cond), data)
     return stats
 
 
@@ -71,9 +79,13 @@ def main(argv=None):
     conds = conditions(cla.env)
     seed_all(cla.seed)
     params = evaluation.run_config(cla.agent_name, Parameters(cla))
-    params.state_dim, params.action_dim = 7, 3
+    params.state_dim, params.action_dim = env_dims(conds[0])
     shape = actor_shape(params)
     refs = evaluation.eval_refs(cla.num_trails)
+    if evaluation.control_mode(params.state_dim, params.action_dim) == 'symmetric':
+        # the symmetric env draws its own theta reference per episode; eval_refs above still advances np.random as
+        # base/evaluate.py's gen_refs calls do
+        refs = evaluation.symmetric_refs(cla.num_trails, cla.seed)
     state = np.random.get_state()        # where each condition's sensor-noise draws start
     if cla.eval_actor or cla.eval_pop:
         pop = evaluation.load_pop(cla.agent_name, params)
@@ -94,15 +106,15 @@ def main(argv=None):
             print(f'{c}: average nMAE: {avg.nmae:0.1f} with SD: {avg.nmae_sd:0.1f}   average smoothness: {avg.sm:0.1f} with SD: {avg.sm_sd:0.1f}')
             if cla.save_trajectory:      # the champion's traces: one more (traced) launch
                 np.random.set_state(state)
-                env = evaluation.condition_env(c)
+                env = evaluation.condition_env(c, shape=shape)
                 if env.sensor_noise:     # skip the draws of the actors before the champion: the suite's trajectories again
                     evaluation.sensor_noise_draws(idx * (cla.num_trails + 1), int(round(env.t_max / env.dt)) + 1)
                 data, _ = evaluation.validate_agent(pop[idx], shape, env, refs, cla.num_trails)
-                evaluation.write_trajectory(cla.agent_name, c, data)
+                evaluation.write_trajectory(cla.agent_name, folder(c), data)
             if cla.save_stats:
                 ci = res.conditions.index(c)
-                evaluation.write_final_performance(cla.agent_name, c, res.sm[:, ci], res.nmae[:, ci])
-                evaluation.append_stats_toml(cla.agent_name, c, idx, res.stats(idx, c), avg)
+                evaluation.write_final_performance(cla.agent_name, folder(c), res.sm[:, ci], res.nmae[:, ci])
+                evaluation.append_stats_toml(cla.agent_name, folder(c), idx, res.stats(idx, c), avg)
         return res
     elif cla.eval_rl:
         rl = evaluation.load_rl_agent(cla.agent_name, params)
@@ -110,7 +122,7 @@ def main(argv=None):
         for c in conds:
             out[c] = fly_one(rl[0], shape, c, refs, cla, 'RL actor', state)
             if cla.save_stats:
-                evaluation.append_rl_stats_toml(cla.agent_name, c, out[c])
+                evaluation.append_rl_stats_toml(cla.agent_name, folder(c), out[c])
         return out
     else:
         raise SystemExit('choose one of -eval_pop, -eval_actor, -eval_rl')

@@ -6,7 +6,9 @@
 For every actor of the run's population: the parent flies num_trails + 1 evaluation episodes of 20 s and stores their
 transitions, then one normal, one proximal and one safe child fly the same references; the relative change of each
 child's return and safety cost against its parent is printed per operator (serl_b200.operators).  `-env` takes one
-condition, a comma list or 'all'; every condition runs the study on its own, seeded as a run of the reference script on
+condition, a full env name, a comma list of one configuration, 'all' or 'PHlab_<configuration>_all'
+(evaluation.env_conditions; 'PHlab_attitude_incremental' studies an incremental-control run, 'PHlab_symmetric_<mode>' a
+symmetric one, except on 'gust' and 'test'); every condition runs the study on its own, seeded as a run of the reference script on
 that condition alone.  `-mags m1,m2,...` repeats the study at several mutation magnitudes (default: the run's
 mutation_mag).  -save_stats writes <run>/mutation_stats.toml (stats_cost, then stats_reward, the reference's layout; with
 several conditions or magnitudes, the last ones run).
@@ -25,7 +27,8 @@ from serl_b200 import evaluation, operators            # noqa: E402
 from serl_b200.parameters import Parameters           # noqa: E402
 
 parser = argparse.ArgumentParser()
-parser.add_argument('-env', type=str, default='nominal', help="a condition, a comma list of conditions, or 'all'")
+parser.add_argument('-env', type=str, default='nominal',
+                    help="a condition, a full env name PHlab_<configuration>_<mode>, PHlab_<configuration>_all, a comma list, or 'all'")
 parser.add_argument('-seed', type=int, default=7)
 parser.add_argument('-agent_name', type=str, required=True, help='run directory (files/config.yaml, files/evo_nets.pkl)')
 parser.add_argument('-save_stats', default=False, action='store_true')
@@ -35,9 +38,10 @@ parser.add_argument('-mags', type=str, default=None, help='comma list of mutatio
 
 
 def conditions(text):
-    if text == 'all':
-        return list(evaluation.CONDITIONS)
-    return [c.split('_')[-1] if c.lower().startswith('phlab_') else c for c in text.split(',') if c]
+    try:
+        return evaluation.env_conditions(text)
+    except ValueError as e:
+        raise SystemExit(str(e))
 
 
 def seed_all(seed):
@@ -51,12 +55,14 @@ def main(argv=None):
     cla = parser.parse_args(argv)
     mags = [float(m) for m in cla.mags.split(',')] if cla.mags else None
     params = evaluation.run_config(cla.agent_name, Parameters(cla))
-    params.state_dim, params.action_dim = 7, 3
+    conds = conditions(cla.env)
+    params.state_dim, params.action_dim = evaluation.env_dims(conds[0])       # from the env, as the reference sets them
+    sym = evaluation.control_mode(params.state_dim, params.action_dim) == 'symmetric'
     pop = evaluation.load_pop(cla.agent_name, params)
     out = {}
-    for c in conditions(cla.env):
+    for c in conds:
         seed_all(cla.seed)
-        refs = operators.study_refs(cla.num_trails)
+        refs = operators.study_refs(cla.num_trails, symmetric=sym, seed=cla.seed)
         runner = operators.OperatorRunner(params, c, num_trails=cla.num_trails)
         res = runner.test_mutation(pop, refs, mags)
         out[c] = res

@@ -165,6 +165,18 @@ int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shap
  *                deflection [de, 0, 0].  Not with SERL_ROLLOUT_INCREMENTAL, d_track, d_cost, SERL_ROLLOUT_GUST or
  *                d_sensor_noise: SERL_ERR_ARG before any CUDA call.  With widths (K1-TC) the genome has 2 * w0 layer-0
  *                weights and one output: serl_actor_num_params_wide(widths) - 5 * w0 - 2 * (w_last + 1) floats per actor
+ *                SERL_ROLLOUT_SUITE: the launch belongs to the evaluation suite or the operator study of incremental or
+ *                symmetric control.  Valid only together with exactly one of SERL_ROLLOUT_INCREMENTAL /
+ *                SERL_ROLLOUT_SYMMETRIC (SERL_ERR_ARG otherwise); without it every refusal of both modes above holds.  It
+ *                lifts these refusals:
+ *                  with SERL_ROLLOUT_INCREMENTAL: d_track and d_cost are allowed (SERL_ROLLOUT_GUST and d_sensor_noise stay
+ *                  refused: every incremental mode flies the nominal build);
+ *                  with SERL_ROLLOUT_SYMMETRIC: d_track and d_cost are allowed, SERL_ROLLOUT_GUST with d_track only (the
+ *                  tracking instantiations carry the gust schedule), d_sensor_noise with or without d_track.
+ *                The tracking sums of incremental control are the attitude ones, with the integrated deflection u in the
+ *                trace and d_actions.  With symmetric control d_track holds sum |e_theta|, 0, 0, sum e_theta, e_theta =
+ *                ref_theta(t_k) (with the 0.22 deg trim) - theta of the state env.x holds when step k starts; the d_cost
+ *                tally is the attitude one (it still tests alpha, phi and V)
  * t_max <= 0 selects the training defaults (20 s, smooth width 3 s). */
 #define SERL_TRACK_COLS 4
 #define SERL_REPLAY_COLS 20                       /* = SERL_REPLAY_COLS_OF(7) */
@@ -175,6 +187,7 @@ int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shap
 #define SERL_ROLLOUT_PER_ACTOR_REFS 4
 #define SERL_ROLLOUT_INCREMENTAL 8
 #define SERL_ROLLOUT_SYMMETRIC 16
+#define SERL_ROLLOUT_SUITE 32
 enum { SERL_STATUS_NONFINITE = 1,     /* a trajectory's state / return became NaN or infinite */
        SERL_STATUS_GUST_FLAG = 2 };   /* an env has SERL_MODE_GUST but the launch was not made with SERL_ROLLOUT_GUST */
 typedef struct {

@@ -26,6 +26,7 @@ ROLLOUT_STAGGER = 2
 ROLLOUT_PER_ACTOR_REFS = 4
 ROLLOUT_INCREMENTAL = 8
 ROLLOUT_SYMMETRIC = 16
+ROLLOUT_SUITE = 32
 STATUS_NONFINITE = 1
 STATUS_GUST_FLAG = 2
 # include/serl_td3.h (K7, the fused TD3 learner)

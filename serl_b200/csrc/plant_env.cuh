@@ -645,7 +645,8 @@ static __device__ __forceinline__ void env_reset(Env& e, const RolloutArgs& a, i
 // one CitationEnv.step (phlabenv.py:430-482) + the bookkeeping of Agent.evaluate (agent.py:85-118)
 // TRACK: + the tracking error of base/evaluate.py:71-100, e = ref(t) - x_ctrl with x_ctrl = env.x[[7, 6, 5]] when the step
 // starts (the native step output of the previous step, or of reset()'s step: in the sensor-noise builds it carries the
-// noise, as the reference's env.x does), accumulated in step order in fp64
+// noise, as the reference's env.x does), accumulated in step order in fp64.  With SYM the controlled state is theta alone
+// (get_controlled_state of the symmetric env): sum |e_theta|, 0, 0, sum e_theta, e_theta against the trimmed reference
 // PER_ACTOR: env_mode holds one row per (actor, env); the replay row's V0 comes from the actor's own replay_env row
 // INC: incremental control (phlabenv.py:443-466): the scaled action is a rate (bound 25 deg/s, :205-206), integrated as
 // u = last_u + rate * dt in fp64 in the reference's operation order (:377-380; no contraction to fma), u drives the fault
@@ -702,7 +703,11 @@ static __device__ __forceinline__ void env_step(Env& e, const RolloutArgs& ar, s
     const double e0 = r_th - xo[7], e1 = SYM ? 0.0 : r_ph - xo[6], e2 = SYM ? 0.0 : 0.0 - xo[5];
     if constexpr (TRACK) {
         const double et = r_th - e.trk[SERL_TRACK_COLS], ep = r_ph - e.trk[SERL_TRACK_COLS + 1], eb = 0.0 - e.trk[SERL_TRACK_COLS + 2];
-        e.trk[0] += fabs(et); e.trk[1] += fabs(ep); e.trk[2] += fabs(eb); e.trk[3] += eb;
+        if constexpr (SYM) {      // a 1-column controlled state: sum |e_theta|, 0, 0, sum e_theta (evaluation.nmae_from_track)
+            e.trk[0] += fabs(et); e.trk[3] += et;
+        } else {
+            e.trk[0] += fabs(et); e.trk[1] += fabs(ep); e.trk[2] += fabs(eb); e.trk[3] += eb;
+        }
         e.trk[SERL_TRACK_COLS] = xo[7]; e.trk[SERL_TRACK_COLS + 1] = xo[6]; e.trk[SERL_TRACK_COLS + 2] = xo[5];
         if (step_cost(xo, e.trk[TRACK_V0])) e.trk[TRACK_COST] += 1.0;     // the replay row's cost flag, for every env
     }

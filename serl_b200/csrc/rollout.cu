@@ -430,9 +430,11 @@ __global__ void genome_layout_kernel(const float* __restrict__ w, float* __restr
 // PER_ACTOR: every actor flies its own env block (SERL_ROLLOUT_PER_ACTOR_REFS): env `env` of actor `actor` binds row
 // actor * n_envs + env of env_mode / ref_levels / ref_starts, also when a slot resumes it from a hand-over record
 // (instantiated without TRACK, with both GUST values)
-// INC: incremental control (SERL_ROLLOUT_INCREMENTAL; instantiated without GUST and TRACK): a 10-entry observation and the
-// env's last_u, both carried in the hand-over records too (OBS_DIM: plant_env.cuh).
-// SYM: symmetric control (SERL_ROLLOUT_SYMMETRIC; instantiated without GUST and TRACK): a 2-entry observation, one action
+// INC: incremental control (SERL_ROLLOUT_INCREMENTAL; instantiated without GUST and TRACK, and with both for the evaluation
+// suite, SERL_ROLLOUT_SUITE): a 10-entry observation and the env's last_u, both carried in the hand-over records too
+// (OBS_DIM: plant_env.cuh), next to the tracking sums of a TRACK instantiation.
+// SYM: symmetric control (SERL_ROLLOUT_SYMMETRIC; instantiated without GUST and TRACK, and with both for the evaluation
+// suite): a 2-entry observation, one action
 template <int H, bool TABS, bool GUST, bool TRACK = false, bool PER_ACTOR = false, bool INC = false, bool SYM = false>
 __global__ void __launch_bounds__(MAX_CTA_THREADS, 1)
 rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
@@ -638,7 +640,7 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
 
 // ---- cross-check kernel: every thread evaluates the whole MLP for its own env (any hidden size that fits) ------
 // PER_ACTOR as in rollout_kernel_persist
-// INC, SYM as in rollout_kernel_persist (instantiated without TRACK)
+// INC, SYM as in rollout_kernel_persist (instantiated without TRACK, and with it for the evaluation suite)
 template <bool TRACK = false, bool PER_ACTOR = false, bool INC = false, bool SYM = false>
 __global__ void __launch_bounds__(128)
 rollout_kernel_simple(RolloutArgs ar, TrackArgs tk)
@@ -861,7 +863,8 @@ static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust,
     const size_t wt_bytes = (size_t)ar.pop * ar.P4 * 4;
     const long long hn = ar.n_tasks > ar.n_slots ? ar.n_slots * wps * 32 : 0;
     // a record's observation: 7 floats, 10 floats and last_u (3 f64) with incremental control, 2 floats with symmetric
-    // control (Handoff.obs)
+    // control (Handoff.obs).  A tracking record (tk.ho) follows the flags, after all of these: an incremental-control
+    // tracking launch carries both
     const size_t ho_obs = inc ? 10 * 4 + 3 * 8 : sym ? 2 * 4 : 7 * 4;
     const size_t ho_bytes = (size_t)hn * (NX * 8 + 8 + 8 + ho_obs + 4) + (size_t)(hn / 32) * 4 + (tk.out ? (size_t)hn * TRACK_CARRY * 8 + 8 : 0);
     void* scratch = nullptr;
@@ -891,7 +894,9 @@ static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust,
     const size_t smem = (TABS ? (size_t)PLANT_TABN2 * sizeof(real) : 0) + (size_t)apc * ar.P4 * 4 +
                         (size_t)apc * wps * (inc ? actor_xbuf_floats(H, 10) : actor_xbuf_floats(H)) * 4;
     void (*const kernel)(RolloutArgs, TrackArgs) =
-        inc         ? (per_actor ? rollout_kernel_persist<H, TABS, false, false, true, true> : rollout_kernel_persist<H, TABS, false, false, false, true>)
+        inc && tk.out ? rollout_kernel_persist<H, TABS, true, true, false, true>          // the suite's tracking launches
+        : sym && tk.out ? rollout_kernel_persist<H, TABS, true, true, false, false, true>
+        : inc       ? (per_actor ? rollout_kernel_persist<H, TABS, false, false, true, true> : rollout_kernel_persist<H, TABS, false, false, false, true>)
         : sym       ? (per_actor ? rollout_kernel_persist<H, TABS, false, false, true, false, true>
                                  : rollout_kernel_persist<H, TABS, false, false, false, false, true>)
         : tk.out    ? rollout_kernel_persist<H, TABS, true, true>
@@ -974,7 +979,9 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
         if (!k1_fits(d.shape)) return serl_fail(SERL_ERR_UNSUPPORTED, "serl_rollout: genome + activations exceed 227 KB of shared memory");
         const size_t smem = (size_t)ar.P4 * 4 + 2ull * H * 128 * 4;
         return serl_launch("rollout_kernel launch",
-                           inc         ? (per_actor ? rollout_kernel_simple<false, true, true> : rollout_kernel_simple<false, false, true>)
+                           inc && d.d_track ? rollout_kernel_simple<true, false, true>
+                           : sym && d.d_track ? rollout_kernel_simple<true, false, false, true>
+                           : inc       ? (per_actor ? rollout_kernel_simple<false, true, true> : rollout_kernel_simple<false, false, true>)
                            : sym       ? (per_actor ? rollout_kernel_simple<false, true, false, true> : rollout_kernel_simple<false, false, false, true>)
                            : d.d_track ? rollout_kernel_simple<true> : per_actor ? rollout_kernel_simple<false, true> : rollout_kernel_simple<false>,
                            dim3((d.n_envs + 127) / 128, d.pop), 128, smem, s, ar, tk);
@@ -1019,24 +1026,36 @@ static int check_desc(const serl_rollout_desc& d)
         if (d.d_track) return serl_fail(SERL_ERR_ARG, "serl_rollout: SERL_ROLLOUT_PER_ACTOR_REFS does not take d_track");
         if ((int64_t)d.pop * d.n_envs > INT32_MAX) return serl_fail(SERL_ERR_ARG, "serl_rollout: pop * n_envs must fit int32 with per-actor refs");
     }
-    // incremental control: a 10-entry observation, on the training instantiations of K1 and K1-TC only
+    // the evaluation suite / operator study of incremental or symmetric control: a launch of exactly one of the two modes
+    const bool suite = (d.flags & SERL_ROLLOUT_SUITE) != 0;
+    if (suite && ((d.flags & SERL_ROLLOUT_INCREMENTAL) != 0) == ((d.flags & SERL_ROLLOUT_SYMMETRIC) != 0))
+        return serl_fail(SERL_ERR_ARG, "serl_rollout: SERL_ROLLOUT_SUITE needs exactly one of SERL_ROLLOUT_INCREMENTAL / SERL_ROLLOUT_SYMMETRIC");
+    // incremental control: a 10-entry observation, on the training instantiations of K1 and K1-TC (and their tracking
+    // instantiations in suite launches)
     if (d.flags & SERL_ROLLOUT_INCREMENTAL) {
         if (d.shape.state_dim != 10) return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) needs state_dim = 10");
-        if (d.d_track || d.d_cost) return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) does not take d_track / d_cost");
+        if (!suite && (d.d_track || d.d_cost))
+            return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) does not take d_track / d_cost");
         if (d.flags & SERL_ROLLOUT_GUST) return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) does not take SERL_ROLLOUT_GUST");
         if (d.d_sensor_noise) return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) does not take d_sensor_noise");
     } else if (d.n_widths == 0 && d.shape.state_dim == 10) {
         return serl_fail(SERL_ERR_ARG, "serl_rollout: state_dim = 10 is the observation of incremental control: it needs SERL_ROLLOUT_INCREMENTAL");
     }
-    // symmetric control: a 2-entry observation and one action, on the training instantiations of K1 and K1-TC only
+    // symmetric control: a 2-entry observation and one action, on the training instantiations of K1 and K1-TC (and, in suite
+    // launches, their tracking instantiations, which carry the gust schedule, and the sensor-noise shim of every instantiation)
     if (d.flags & SERL_ROLLOUT_SYMMETRIC) {
         if (d.shape.state_dim != 2 || d.shape.action_dim != 1)
             return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) needs state_dim = 2 and action_dim = 1");
         if (d.flags & SERL_ROLLOUT_INCREMENTAL)
             return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) does not take SERL_ROLLOUT_INCREMENTAL");
-        if (d.d_track || d.d_cost) return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) does not take d_track / d_cost");
-        if (d.flags & SERL_ROLLOUT_GUST) return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) does not take SERL_ROLLOUT_GUST");
-        if (d.d_sensor_noise) return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) does not take d_sensor_noise");
+        if (!suite && (d.d_track || d.d_cost))
+            return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) does not take d_track / d_cost");
+        if (!suite && (d.flags & SERL_ROLLOUT_GUST))
+            return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) does not take SERL_ROLLOUT_GUST");
+        if ((d.flags & SERL_ROLLOUT_GUST) && !d.d_track)
+            return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC | SERL_ROLLOUT_SUITE) takes SERL_ROLLOUT_GUST with d_track only");
+        if (!suite && d.d_sensor_noise)
+            return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) does not take d_sensor_noise");
     } else if (d.n_widths == 0 && is_symmetric(d.shape)) {
         return serl_fail(SERL_ERR_ARG, "serl_rollout: state_dim = 2, action_dim = 1 is the actor of symmetric control: it needs SERL_ROLLOUT_SYMMETRIC");
     }

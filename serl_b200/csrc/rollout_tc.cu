@@ -650,9 +650,10 @@ __device__ __forceinline__ void tc_load_small(TcCtx& c, const TcArgs& ar, int ac
 // (tc_actor_forward_deep); the two-width instantiations run tc_actor_forward.  TRACK: the launch writes the tracking-error
 // sums `tk` (serl_rollout_desc.d_track; instantiated with GUST only).  PER_ACTOR: env `env` of actor `actor` binds row
 // actor * n_envs + env of env_mode / ref_levels / ref_starts (SERL_ROLLOUT_PER_ACTOR_REFS; instantiated without TRACK).
-// INC: incremental control (SERL_ROLLOUT_INCREMENTAL; instantiated without GUST and TRACK): a 10-entry observation, layer 0
-// with 10 inputs, and the env's last_u.  SYM: symmetric control (SERL_ROLLOUT_SYMMETRIC; instantiated without GUST and
-// TRACK): a 2-entry observation, layer 0 with 2 inputs, and action 0 of the output block as the elevator
+// INC: incremental control (SERL_ROLLOUT_INCREMENTAL; instantiated without GUST and TRACK, and with both for the evaluation
+// suite): a 10-entry observation, layer 0 with 10 inputs, and the env's last_u.  SYM: symmetric control
+// (SERL_ROLLOUT_SYMMETRIC; instantiated without GUST and TRACK, and with both for the evaluation suite): a 2-entry
+// observation, layer 0 with 2 inputs, and action 0 of the output block as the elevator
 template <int ACT, bool GUST, bool DEEP, bool TRACK = false, bool PER_ACTOR = false, bool INC = false, bool SYM = false>
 __global__ void __launch_bounds__(2 * TC_THREADS, 1)
 rollout_kernel_tc(const __grid_constant__ TcArgs ar, TrackArgs tk)
@@ -839,11 +840,26 @@ int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, cudaStream
           rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, false, false, true>},
          {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, true, false, true>,
           rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, true, false, true>}}};
+    // the evaluation suite's tracking launches of incremental / symmetric control (SERL_ROLLOUT_SUITE)
+    static void (*const inc_track_kernels[3][2])(TcArgs, TrackArgs) = {                              // [SERL_ACT_*][deep]
+        {rollout_kernel_tc<SERL_ACT_TANH, true, false, true, false, true>, rollout_kernel_tc<SERL_ACT_TANH, true, true, true, false, true>},
+        {rollout_kernel_tc<SERL_ACT_ELU, true, false, true, false, true>, rollout_kernel_tc<SERL_ACT_ELU, true, true, true, false, true>},
+        {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, false, true, false, true>,
+         rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, true, true, false, true>}};
+    static void (*const sym_track_kernels[3][2])(TcArgs, TrackArgs) = {                              // [SERL_ACT_*][deep]
+        {rollout_kernel_tc<SERL_ACT_TANH, true, false, true, false, false, true>,
+         rollout_kernel_tc<SERL_ACT_TANH, true, true, true, false, false, true>},
+        {rollout_kernel_tc<SERL_ACT_ELU, true, false, true, false, false, true>,
+         rollout_kernel_tc<SERL_ACT_ELU, true, true, true, false, false, true>},
+        {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, false, true, false, false, true>,
+         rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, true, true, false, false, true>}};
     const TrackArgs tk = {d.d_track, nullptr, d.d_cost};
     const bool gust = (d.flags & SERL_ROLLOUT_GUST) != 0, deep = ar.n_layers > 1;
     const bool per_actor = (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) != 0;
     // one CTA = the two groups of TC_THREADS threads
-    return serl_launch("rollout_kernel_tc launch", inc ? inc_kernels[d.shape.activation][per_actor][deep]
+    return serl_launch("rollout_kernel_tc launch", inc && d.d_track ? inc_track_kernels[d.shape.activation][deep]
+                                                   : sym && d.d_track ? sym_track_kernels[d.shape.activation][deep]
+                                                   : inc ? inc_kernels[d.shape.activation][per_actor][deep]
                                                    : sym ? sym_kernels[d.shape.activation][per_actor][deep]
                                                    : d.d_track ? track_kernels[d.shape.activation][deep]
                                                    : (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) ? per_actor_kernels[d.shape.activation][gust][deep]

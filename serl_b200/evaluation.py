@@ -47,17 +47,87 @@ def reset_state(x_ic, z0=None):
     return x
 
 
-def condition_env(condition, t_max=T_MAX):
-    """the CitationEnv of a condition name ('nominal', 'low-q', ..., or a full env name 'PHlab_attitude_<condition>') in
-    evaluation mode"""
+_MODE_TEXT = {'attitude': 'attitude control with absolute commands', 'incremental': 'incremental control',
+              'symmetric': 'symmetric control'}
+
+
+def control_mode(state_dim=7, action_dim=3):
+    """the control mode an actor of these widths flies: 'attitude' (7 -> 3), 'incremental' (10 -> 3) or 'symmetric' (2 -> 1)"""
+    if (state_dim, action_dim) == (rollout.SYMMETRIC_STATE_DIM, rollout.SYMMETRIC_ACTION_DIM):
+        return 'symmetric'
+    return 'incremental' if state_dim == rollout.INCREMENTAL_STATE_DIM else 'attitude'
+
+
+def env_control_mode(env):
+    return 'symmetric' if env.symmetric else 'incremental' if env.incremental else 'attitude'
+
+
+def full_name(condition):
+    """the env name of a condition: a bare name ('nominal', 'be', ..., 'incremental') is the attitude configuration's"""
+    return condition if '_' in condition else 'PHlab_attitude_' + condition
+
+
+def condition_env(condition, t_max=T_MAX, shape=None):
+    """the CitationEnv of a condition name ('nominal', 'low-q', ..., or a full env name 'PHlab_<configuration>_<mode>') in
+    evaluation mode, for an actor of `shape` (None: the attitude 7 -> 3 actor).  The env's control mode must be the actor's:
+    a bare name is an attitude env with absolute commands, 'incremental' (or any mode containing it) one with incremental
+    commands, and 'PHlab_symmetric_<mode>' a symmetric one.  A mismatch raises ValueError naming both modes."""
     from .envs import config
-    env = config.select_env(condition if '_' in condition else 'PHlab_attitude_' + condition)
-    if env.incremental:
-        raise ValueError('evaluation: the evaluation suite flies absolute control only, not incremental control (%s)' % condition)
-    if env.symmetric:
-        raise ValueError('evaluation: the evaluation suite flies attitude control only, not symmetric control (%s)' % condition)
+    env = config.select_env(full_name(condition))
+    mode = 'attitude' if shape is None else control_mode(shape.state_dim, shape.action_dim)
+    have = env_control_mode(env)
+    if have != mode:
+        raise ValueError('evaluation: condition %r is an env of %s, but the actor flies %s' % (condition, _MODE_TEXT[have], _MODE_TEXT[mode]))
     env.set_eval_mode(t_max)
     return env
+
+
+def _configuration(name):
+    """the configuration token of a full env name ('attitude', 'symmetric'), or 'attitude' for a bare condition"""
+    return name.split('_')[1].lower() if '_' in name else 'attitude'
+
+
+def env_conditions(text):
+    """the condition list of an -env argument: 'all', a condition, a full name 'PHlab_<configuration>_<mode>' or a comma
+    list of them.  Attitude names become their bare mode ('PHlab_attitude_be' -> 'be'); other configurations keep their full name.
+    'PHlab_<configuration>_all' is every condition of that configuration.  One list flies one configuration."""
+    out, cfgs = [], set()
+    for c in (c for c in text.split(',') if c):
+        cfg = _configuration(c) if c.lower().startswith('phlab_') else 'attitude'
+        cfgs.add(cfg)
+        mode = c.split('_')[-1] if c.lower().startswith('phlab_') else c
+        if mode == 'all':
+            out += list(CONDITIONS) if cfg == 'attitude' else ['PHlab_%s_%s' % (c.split('_')[1], m) for m in CONDITIONS]
+        else:
+            out.append(mode if cfg == 'attitude' else c)
+    if len(cfgs) > 1:
+        raise ValueError('evaluation: one condition list flies one configuration, not %s' % ', '.join(sorted(cfgs)))
+    return out
+
+
+def condition_folder(cond):
+    """the output folder of a condition under <run>/figures: the mode token, as base/evaluate.py names it"""
+    return cond.split('_')[-1]
+
+
+def env_dims(cond):
+    """(state_dim, action_dim) of the env a condition names: env.observation_space / env.action_space, as base/evaluate.py
+    sets them"""
+    from .envs import config
+    env = config.select_env(full_name(cond))
+    return env.observation_space.shape[0], env.action_space.shape[0]
+
+
+def symmetric_refs(num_trails, seed=7, t_max=T_MAX):
+    """the theta references of symmetric control's evaluation episodes: the reference's env ignores user_refs and draws one
+    RandomizedCosineStepSequence(t_max, ampl_max=30, block_width=t_max // 5, smooth_width=t_max // 6.7, n_levels=40,
+    vary_timings=0) per episode (envs/phlabenv.py:303-313); here num_trails + 1 of them from refsig.make_ref_params(seed_base
+    = seed, symmetric=True), as (theta, phi) pairs whose phi channel is zero and never read.  The kernels add the 0.22 deg
+    trim themselves."""
+    levels, starts = refsig.make_ref_params(num_trails + 1, seed_base=seed, t_max=t_max, symmetric=True)
+    sw = refsig.widths(t_max, True)[1]
+    return [(signals.SmoothedStepSequence(starts[i, 0], levels[i, 0], smooth_width=sw),
+             signals.SmoothedStepSequence(starts[i, 1], levels[i, 1], smooth_width=sw)) for i in range(num_trails + 1)]
 
 
 def gen_refs(t_max, amp_times, ampl_max, num_trails=10):
@@ -86,11 +156,14 @@ def eval_refs(num_trails, t_max=T_MAX):
     return list(zip(theta, phi))
 
 
-def nmae_from_track(track, steps):
-    """calc_nMAE (base/core/utils.py:39-58) of trajectories from their tracking-error sums: track [..., 4], steps [...]"""
+def nmae_from_track(track, steps, symmetric=False):
+    """calc_nMAE (base/core/utils.py:39-58) of trajectories from their tracking-error sums: track [..., 4], steps [...].
+    symmetric=True: the sums of symmetric control (sum |e_theta|, 0, 0, sum e_theta), whose (n, 1) error array calc_nMAE
+    broadcasts: theta's mean error over [20 deg, 20 deg, max(|mean e_theta|, 3.14159 / 180)], the last range ("beta's") taken
+    from theta's own signed mean"""
     track = np.asarray(track, dtype=np.float64)
     n = np.asarray(steps, dtype=np.float64)[..., None]
-    mae = track[..., :3] / n
+    mae = np.broadcast_to(track[..., 0:1] / n, track[..., :3].shape) if symmetric else track[..., :3] / n
     beta_range = np.maximum(np.abs(track[..., 3:4] / n), 3.14159 / 180)
     ranges = np.concatenate((np.broadcast_to(np.deg2rad(20), beta_range.shape), np.broadcast_to(np.deg2rad(20), beta_range.shape),
                              beta_range), axis=-1)
@@ -102,10 +175,22 @@ def _ref_arrays(refs):
     starts = np.stack([np.stack([th.starts, ph.starts]) for th, ph in refs])
     return levels, starts
 
-def validate_agent(genome, shape, env, user_refs_lst, num_trails=1, device=None):
-    """genome: [P] fp32 tensor / array of one actor; env: serl_b200.envs CitationEnv (mode, eval t_max); user_refs_lst: list of
-    (theta_ref, phi_ref) serl_b200.signals.SmoothedStepSequence; trials 0..num_trails are flown (base/evaluate.py:127)."""
+class Flight:
+    """what validate_agent's launch gives per trial, rebuilt as base/evaluate.py's loop records it: errors [k, c] (c = 3, or 1
+    with symmetric control), deflections u_before [k, c], data (the traces of base/evaluate.py), and the launch's own
+    tracking-error sums track [T, 4] (None for attitude control with absolute commands, whose launch has no d_track)"""
+    __slots__ = ('errors', 'u_before', 'data', 'steps', 'returns', 'track')
+
+
+def fly_traced(genome, shape, env, user_refs_lst, num_trails=1, device=None, widths=None):
+    """validate_agent's one traced launch, with the per-trial records (Flight).  Incremental and symmetric control fly it
+    as a tracking launch of the suite (track=True, suite=True): their tracking instantiations are the ones with the gust
+    schedule."""
     dev = device or torch.device('cuda', torch.cuda.current_device())
+    mode = control_mode(shape.state_dim, shape.action_dim)
+    if env_control_mode(env) != mode:
+        raise ValueError('validate_agent: the env flies %s, but the actor flies %s' % (_MODE_TEXT[env_control_mode(env)], _MODE_TEXT[mode]))
+    sym, suite = mode == 'symmetric', mode != 'attitude'
     refs = user_refs_lst[:num_trails + 1]
     n = len(refs)
     horizon = int(round(env.t_max / env.dt)) + 1
@@ -119,26 +204,46 @@ def validate_agent(genome, shape, env, user_refs_lst, num_trails=1, device=None)
         noise = torch.as_tensor(z.reshape(1, n, horizon + 1, 7), device=dev)
     r = rollout.population_rollout(g, shape, torch.as_tensor(levels, device=dev), torch.as_tensor(starts, device=dev), md,
                                    horizon=horizon, trace=True, t_max=float(env.t_max), smooth_width=smooth_w, sensor_noise=noise,
-                                   gust=rollout.mode_gust(env.mode_code))
+                                   gust=rollout.mode_gust(env.mode_code), widths=widths, track=suite, suite=suite)
     torch.cuda.synchronize()
     r.check()
     steps = r.steps[0].cpu().numpy()
     trace = r.trace[0].cpu().numpy()
     x_ic = rollout.initial_state(rollout.mode_variant(env.mode_code))
-    nmaes, sms, data = [], [], None
+    f = Flight()
+    f.errors, f.u_before, f.data = [], [], None
+    f.steps, f.returns = steps, r.returns[0].cpu().numpy()
+    f.track = r.track[0].cpu().numpy() if suite else None
     for i in range(n):
-        k = int(steps[i])
-        tr = trace[i, :k]
-        x_after = tr[:, rollout.TRACE_X]                        # env.x after each step() = state before that plant step
-        ref_values = tr[:, rollout.TRACE_ERR] + x_after[:, [7, 6, 5]]      # ref(t_k) [rad] = error_k + controlled state
-        x0 = reset_state(x_ic, None if z is None else z[i, 0])
-        x_before = np.vstack((x0[None], x_after[:-1]))          # env.x when the loop body starts (evaluate.py:73)
-        u_before = np.vstack((np.zeros((1, 3)), tr[:-1, rollout.TRACE_U]))
-        errors = ref_values - x_before[:, [7, 6, 5]]
-        nmaes.append(calc_nMAE(errors))
-        sms.append(calc_smoothness(u_before, plot_spectra=False))
-        data = np.concatenate((ref_values, u_before, x_before, tr[:, rollout.TRACE_R, None]), axis=1)
-    return data, Stats(float(np.average(nmaes)), float(np.std(nmaes)), float(np.average(sms)), float(np.std(sms)))
+        errors, u_before, f.data = rebuild_trial(trace[i, :int(steps[i])], reset_state(x_ic, None if z is None else z[i, 0]), sym)
+        f.errors.append(errors)
+        f.u_before.append(u_before)
+    return f
+
+
+def rebuild_trial(tr, x0, symmetric=False):
+    """what base/evaluate.py's loop records for one episode, from its trace rows tr [k, TRACE_COLS] and env.x after reset()
+    x0 [12]: errors [k, c] (ref(t) - env.get_controlled_state() when the loop body starts), the deflections env.last_u then
+    [k, c], and data = ref c | u c | x 12 | reward (c = 3, or 1 with symmetric control: theta, the elevator)"""
+    ctrl = [7] if symmetric else [7, 6, 5]       # env.get_controlled_state(): theta, or theta, phi, beta
+    x_after = tr[:, rollout.TRACE_X]                             # env.x after each step() = state before that plant step
+    ref_values = tr[:, rollout.TRACE_ERR][:, :len(ctrl)] + x_after[:, ctrl]      # ref(t_k) [rad] = error_k + controlled state
+    x_before = np.vstack((np.asarray(x0)[None], x_after[:-1]))   # env.x when the loop body starts (evaluate.py:73)
+    u_before = np.vstack((np.zeros((1, len(ctrl))), tr[:-1, rollout.TRACE_U][:, :len(ctrl)]))
+    data = np.concatenate((ref_values, u_before, x_before, tr[:, rollout.TRACE_R, None]), axis=1)
+    return ref_values - x_before[:, ctrl], u_before, data
+
+
+def validate_agent(genome, shape, env, user_refs_lst, num_trails=1, device=None, widths=None):
+    """genome: [P] fp32 tensor / array of one actor; env: serl_b200.envs CitationEnv (mode, eval t_max) of the actor's control
+    mode (condition_env(..., shape=shape)); user_refs_lst: list of (theta_ref, phi_ref) serl_b200.signals.SmoothedStepSequence
+    (symmetric control: symmetric_refs); trials 0..num_trails are flown (base/evaluate.py:127).  widths: a width-list actor on
+    K1-TC, as in rollout.population_rollout.  Returns the traces of the last trial (ref | u | x 12 | reward: 19 columns, 15
+    with symmetric control's ref_theta | de) and Stats."""
+    f = fly_traced(genome, shape, env, user_refs_lst, num_trails, device, widths)
+    nmaes = [calc_nMAE(e) for e in f.errors]
+    sms = [calc_smoothness(u, plot_spectra=False) for u in f.u_before]
+    return f.data, Stats(float(np.average(nmaes)), float(np.std(nmaes)), float(np.average(sms)), float(np.std(sms)))
 
 
 class PopulationEval:
@@ -183,11 +288,13 @@ def evaluate_population(genomes, shape, conditions, user_refs_lst, num_trails=1,
     continued np.random stream; with `noise_state` (an np.random.get_state()) every noisy condition's draws start from that
     state instead, as when base/evaluate.py runs once per condition and reseeds (examples/evaluate.py).  When
     the [N, envs, horizon, 3] fp32 deflection record exceeds `actions_cap` bytes, the actors are flown in chunks of equal
-    launches (same results)."""
-    if shape.state_dim == rollout.INCREMENTAL_STATE_DIM:
-        raise ValueError('evaluate_population: the evaluation suite flies absolute control only, not incremental control')
-    if rollout.is_symmetric(shape):
-        raise ValueError('evaluate_population: the evaluation suite flies attitude control only, not symmetric control')
+    launches (same results).  Incremental (10 -> 3) and symmetric (2 -> 1) actors fly the conditions of their own control
+    mode (condition_env(..., shape)) in tracking launches of the suite (suite=True); symmetric control's references come
+    from symmetric_refs.  The recorded deflection is [de, 0, 0] with symmetric control: K6 of it is the one-column
+    calc_smoothness."""
+    envs = [condition_env(c, shape=shape) for c in conditions]      # the conditions of the actor's control mode
+    mode = control_mode(shape.state_dim, shape.action_dim)
+    sym, suite = mode == 'symmetric', mode != 'attitude'
     dev = device or torch.device('cuda', torch.cuda.current_device())
     refs = user_refs_lst[:num_trails + 1]
     T, C = len(refs), len(conditions)
@@ -197,7 +304,6 @@ def evaluate_population(genomes, shape, conditions, user_refs_lst, num_trails=1,
     g = torch.as_tensor(np.asarray(genomes, dtype=np.float32) if not torch.is_tensor(genomes) else genomes, device=dev)
     g = g.reshape(g.shape[0], -1).contiguous()
     N = g.shape[0]
-    envs = [condition_env(c) for c in conditions]
     t_max = float(envs[0].t_max)
     horizon = int(round(t_max / envs[0].dt)) + 1
     lv1, st1 = _ref_arrays(refs)
@@ -238,7 +344,8 @@ def evaluate_population(genomes, shape, conditions, user_refs_lst, num_trails=1,
             rollout.population_rollout(g[lo:hi], shape, torch.as_tensor(np.tile(lv1, (len(idx), 1, 1)), device=dev),
                                        torch.as_tensor(np.tile(st1, (len(idx), 1, 1)), device=dev), md, horizon=horizon, out=out,
                                        t_max=t_max, smooth_width=smooth_w, env_order=rollout.variant_sorted_order(md), fitness=False,
-                                       widths=widths, sensor_noise=noise, gust=any(rollout.mode_gust(int(c)) for c in codes))
+                                       widths=widths, sensor_noise=noise, gust=any(rollout.mode_gust(int(c)) for c in codes),
+                                       suite=suite)
             runs.append((idx, out))
             row += n * ne
         steps = torch.cat([out.steps.reshape(-1) for _, out in runs])
@@ -250,7 +357,7 @@ def evaluate_population(genomes, shape, conditions, user_refs_lst, num_trails=1,
         for idx, out in runs:
             out.check()
             ne = len(idx) * T
-            nm = nmae_from_track(out.track.cpu().numpy(), out.steps.cpu().numpy())
+            nm = nmae_from_track(out.track.cpu().numpy(), out.steps.cpu().numpy(), symmetric=sym)
             nmae[lo:hi, idx] = nm.reshape(n, len(idx), T)
             sm[lo:hi, idx] = smooth[row:row + n * ne].reshape(n, len(idx), T)
             row += n * ne

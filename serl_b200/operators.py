@@ -29,10 +29,13 @@ T_MAX = 20                   # base/evaluate_operators.py:46: the study's episod
 ParentFlight = namedtuple('ParentFlight', ('returns', 'costs', 'steps', 'buffers', 'critical_buffers'))
 
 
-def study_refs(num_trails, t_max=T_MAX):
+def study_refs(num_trails, t_max=T_MAX, symmetric=False, seed=7):
     """base/evaluate_operators.py:85-104: num_trails random (theta, phi) pairs from gen_refs (smooth width t_max // 10),
-    then the fixed base sequences as trial num_trails — evaluation.eval_refs at t_max = 20 s"""
-    return evaluation.eval_refs(num_trails, t_max)
+    then the fixed base sequences as trial num_trails — evaluation.eval_refs at t_max = 20 s.  symmetric=True: the symmetric
+    env ignores them and draws its own theta references (evaluation.symmetric_refs at t_max = 20 s, seeded from `seed`); the
+    gen_refs draws are still made, so the legacy np.random stream stands where the reference's does"""
+    refs = evaluation.eval_refs(num_trails, t_max)
+    return evaluation.symmetric_refs(num_trails, seed, t_max) if symmetric else refs
 
 
 def mutation_stats(parent_returns, parent_costs, child_returns, child_costs):
@@ -91,7 +94,10 @@ class MutationStudy:
 
 class OperatorRunner:
     """base/core/operator_runner.py OperatorRunner over a [N, P] genome matrix (fp32, parameters() order) of the uniform
-    actor `args` describes (hidden_size, num_layers, activation_actor), on one flight condition ('nominal', 'be', ...).
+    actor `args` describes (hidden_size, num_layers, activation_actor, and state_dim / action_dim: 7 / 3 by default, 10 / 3 for
+    incremental control, 2 / 1 for symmetric control), on one flight condition of the actor's control mode ('nominal', 'be',
+    ..., 'incremental', 'PHlab_symmetric_<mode>'; evaluation.condition_env).  Symmetric control refuses 'gust' and 'test':
+    its parents fly a per-actor replay launch, and symmetric control has no per-actor instantiation with the gust schedule.
 
     Draws.  The legacy np.random stream and the stdlib random stream are consumed as test_mutation consumes them for
     mags = [args.mutation_mag], model by model: the sensor-noise draws of the episodes (noisy conditions; the full
@@ -104,16 +110,19 @@ class OperatorRunner:
     for each magnitude in turn."""
 
     def __init__(self, args, condition='nominal', num_trails=0, device=None):
-        if getattr(args, 'state_dim', None) == rollout.INCREMENTAL_STATE_DIM:
-            raise ValueError('OperatorRunner: the operator study flies absolute control only, not incremental control')
-        if (getattr(args, 'state_dim', None), getattr(args, 'action_dim', None)) == (rollout.SYMMETRIC_STATE_DIM, rollout.SYMMETRIC_ACTION_DIM):
-            raise ValueError('OperatorRunner: the operator study flies attitude control only, not symmetric control')
+        S, A = int(getattr(args, 'state_dim', None) or 7), int(getattr(args, 'action_dim', None) or 3)
+        self.shape = rollout.actor_shape(args.hidden_size, args.num_layers, args.activation_actor, S, A)
+        # the condition must be one of the actor's control mode (a bare name is attitude control with absolute commands)
+        self.env = evaluation.condition_env(condition, T_MAX, shape=self.shape)
+        self.mode = evaluation.control_mode(S, A)
+        if self.mode == 'symmetric' and rollout.mode_gust(self.env.mode_code):
+            raise ValueError('OperatorRunner: symmetric control has no per-actor gust instantiation for the parents\' replay '
+                             'launch (%s)' % condition)
         self.args = args
         self.num_trails = int(num_trails)
         self.device = device or torch.device('cuda', torch.cuda.current_device())
-        self.env = evaluation.condition_env(condition, T_MAX)
-        self.shape = rollout.actor_shape(args.hidden_size, args.num_layers, args.activation_actor)
-        self.shape_tuple = (7, 3, int(args.hidden_size), int(args.num_layers))
+        self.shape_tuple = (S, A, int(args.hidden_size), int(args.num_layers))
+        self.dims = rollout.replay_dims(S, A)           # obs, action, next_obs, reward, done, cost
         self.horizon = int(round(self.env.t_max / self.env.dt)) + 1
         self.gen = None
 
@@ -138,16 +147,17 @@ class OperatorRunner:
         sn = None if noise is None else torch.as_tensor(np.ascontiguousarray(noise.reshape(N * T, 1, h + 1, 7)), device=dev)
         r = rollout.population_rollout(weights, self.shape, levels, starts, md, horizon=h, t_max=float(self.env.t_max),
                                        smooth_width=float(refs[0][0].smooth_width), replay_env=0, fitness=False, sensor_noise=sn,
-                                       gust=rollout.mode_gust(self.env.mode_code))
+                                       gust=rollout.mode_gust(self.env.mode_code), suite=self.mode != 'attitude')
         r.check()
         steps = r.steps.reshape(N, T)
-        rows = r.replay.reshape(N, T, h, rollout.REPLAY_COLS).clone()
-        rows[..., 0:7] = rows[..., 10:17]                                     # state = next_obs (operator_runner.py:52-57)
+        S, A = self.shape_tuple[:2]
+        rows = r.replay.reshape(N, T, h, rollout.replay_cols(S, A)).clone()
+        rows[..., 0:S] = rows[..., S + A:2 * S + A]                           # state = next_obs (operator_runner.py:52-57)
         live = torch.arange(h, device=dev)[None, None, :] < steps[..., None]
-        crit = live & (rows[..., rollout.REPLAY_COST] > 0.5)
+        crit = live & (rows[..., rollout.transition_cols(S, A)] > 0.5)
         costs = crit.sum(-1)
-        buffers = PopulationBuffers(N, self.args.individual_bs, dev)
-        critical = PopulationBuffers(N, self.args.individual_bs, dev)
+        buffers = PopulationBuffers(N, self.args.individual_bs, dev, S, A)
+        critical = PopulationBuffers(N, self.args.individual_bs, dev, S, A)
         actors = torch.arange(N, device=dev)
         for t in range(T):                                                    # trial by trial, as validate_agent fills them
             buffers.append(actors, rows[:, t], live[:, t])
@@ -159,7 +169,7 @@ class OperatorRunner:
         reference's ReplayMemory.memory order)"""
         n = int(min(int(bufs.count[actor]), bufs.capacity))
         idx = random.sample(range(n), min(int(self.args.mutation_batch_size), n))
-        return bufs.data[actor, torch.as_tensor(idx, dtype=torch.int64, device=self.device), :7]
+        return bufs.data[actor, torch.as_tensor(idx, dtype=torch.int64, device=self.device), :self.shape_tuple[0]]
 
     def test_mutation(self, genomes, user_eval_refs, mags=None):
         """OperatorRunner.test_mutation for every model of `genomes` [N, P] and every magnitude of `mags` (None:
@@ -227,7 +237,9 @@ class OperatorRunner:
         sn = None if noise is None else torch.as_tensor(np.ascontiguousarray(noise), device=dev)
         r = rollout.population_rollout(genomes.contiguous(), self.shape, torch.as_tensor(lv, device=dev), torch.as_tensor(st, device=dev),
                                        md, horizon=h, t_max=float(self.env.t_max), smooth_width=float(refs[0][0].smooth_width),
-                                       fitness=False, sensor_noise=sn, gust=rollout.mode_gust(self.env.mode_code), track=True, cost=True)
+                                       fitness=False, sensor_noise=sn, gust=rollout.mode_gust(self.env.mode_code), track=True, cost=True,
+                                       suite=self.mode != 'attitude')
         r.check()
         steps = r.steps.cpu().numpy()
-        return r.returns.cpu().numpy(), r.cost.cpu().numpy(), evaluation.nmae_from_track(r.track.cpu().numpy(), steps)
+        return r.returns.cpu().numpy(), r.cost.cpu().numpy(), evaluation.nmae_from_track(r.track.cpu().numpy(), steps,
+                                                                                         symmetric=self.mode == 'symmetric')

@@ -109,7 +109,8 @@ def variant_sorted_order(env_mode):
 
 def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon=HORIZON, trace=False, out=None, action_noise=None,
                        actions=False, t_max=None, smooth_width=None, env_order=None, replay_env=None, status=True, sm_limit=0,
-                       fitness=True, widths=None, sensor_noise=None, gust=False, stagger=False, track=False, cost=False):
+                       fitness=True, widths=None, sensor_noise=None, gust=False, stagger=False, track=False, cost=False,
+                       suite=False):
     """weights [pop,P] fp32 cuda; ref_levels/ref_starts [n_envs,2,6] f64 cuda; env_mode [n_envs] int32 cuda.
     Per-actor env blocks: ref_levels/ref_starts [pop,n_envs,2,6] and env_mode [pop,n_envs] give every actor its own n_envs
     envs (SERL_ROLLOUT_PER_ACTOR_REFS; the shapes select the layout; not with env_order or track).
@@ -127,6 +128,10 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     A 2 -> 1 shape (is_symmetric) flies symmetric control (SERL_ROLLOUT_SYMMETRIC: the elevator alone, obs = [e_theta, q], the theta
     reference of refsig.make_ref_params(symmetric=True) with its smooth width, action_noise [pop, n_envs, horizon, 1], replay rows
     of replay_cols(2, 1) columns; on K1 and K1-TC, without track, cost, gust or sensor_noise).
+    suite=True (SERL_ROLLOUT_SUITE, with incremental or symmetric control only): a launch of the evaluation suite or the operator
+    study.  It lifts these refusals: incremental control takes track and cost (still not gust or sensor_noise); symmetric control
+    takes track and cost, gust with track, and sensor_noise.  Symmetric control's track holds sum |e_theta|, 0, 0, sum e_theta
+    (evaluation.nmae_from_track(symmetric=True)).  Nothing sets it implicitly.
     widths=[w0, w1, ..., w_{n-1}] (2 to 9 widths): width-list actors on the tensor-core kernel K1-TC (csrc/rollout_tc.cu); `shape`
     then only supplies the activation.  widths=None flies the uniform actor `shape` on K1, or on K1-TC with [h] * (L + 1) when its
     genome does not fit K1's kernels (tc_widths)."""
@@ -190,7 +195,7 @@ def population_rollout(weights, shape, ref_levels, ref_starts, env_mode, horizon
     d.flags = ((_native.ROLLOUT_GUST if gust else 0) | (_native.ROLLOUT_STAGGER if stagger else 0)      # gust: mode_code(...) & MODE_GUST
                | (_native.ROLLOUT_PER_ACTOR_REFS if per_actor else 0)
                | (_native.ROLLOUT_INCREMENTAL if shape.state_dim == INCREMENTAL_STATE_DIM else 0)
-               | (_native.ROLLOUT_SYMMETRIC if sym else 0))
+               | (_native.ROLLOUT_SYMMETRIC if sym else 0) | (_native.ROLLOUT_SUITE if suite else 0))
     if widths:
         warr = np.asarray(widths, dtype=np.int32)       # host array, alive until the call returns
         d.widths, d.n_widths = warr.ctypes.data, len(widths)
