@@ -33,6 +33,7 @@ parser.add_argument('-hidden_size', type=int, default=72)
 parser.add_argument('-independent_refs', default=False, action='store_true',
                     help='every episode of every actor draws its own reference signals, as the reference does (default: the '
                          'actors of a generation share num_envs draws)')
+parser.add_argument('-per', help='Use Prioritised Experience Replay', action='store_true')
 parser.add_argument('-no_prefetch', dest='prefetch_generation', default=True, action='store_false',
                     help='strictly one generation per Agent.train() call (no rollouts of the next generation queued ahead)')
 

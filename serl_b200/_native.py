@@ -3,7 +3,8 @@ fallback: importing succeeds without a GPU (so host logic is testable), but the 
 fails loudly when CUDA is unavailable.  tests/test_capi.py holds the signatures and constants below to the header,
 tests/test_td3_oracle.py those of include/serl_td3.h (TD3_SIGNATURES, TD3Desc, TD3_*), tests/test_deep_actor.py those of
 include/serl_route.h (ROUTE_SIGNATURES), tests/test_td3_group.py those of include/serl_td3_group.h (TD3_GROUP_SIGNATURES,
-TD3_MAX_GROUP), tests/test_td3_mixed.py those of include/serl_td3_mixed.h (TD3_MIXED_SIGNATURES)."""
+TD3_MAX_GROUP), tests/test_td3_mixed.py those of include/serl_td3_mixed.h (TD3_MIXED_SIGNATURES), tests/test_td3_per.py those of
+include/serl_td3_per.h (PER_SIGNATURES, TD3PerDesc, PER_MAX_CAPACITY)."""
 import ctypes
 import os
 
@@ -38,6 +39,8 @@ TD3_CHAMPION_TARGET = 1
 TD3_STATUS_INDEX = 4
 # include/serl_td3_group.h (K7 for a group of learners in one launch)
 TD3_MAX_GROUP = 64
+# include/serl_td3_per.h (prioritized replay: the priority tree and K7 with it)
+PER_MAX_CAPACITY = 1 << 30
 
 
 class ActorShape(ctypes.Structure):
@@ -72,6 +75,13 @@ class TD3Desc(ctypes.Structure):
                 ('cluster_size', ctypes.c_int32), ('d_indices', ctypes.c_void_p), ('d_losses', ctypes.c_void_p),
                 ('d_rec_indices', ctypes.c_void_p), ('d_rec_noise', ctypes.c_void_p), ('d_rec_caps', ctypes.c_void_p),
                 ('d_status', ctypes.c_void_p)]
+
+
+class TD3PerDesc(ctypes.Structure):
+    """serl_td3_per_desc (include/serl_td3_per.h)"""
+    _fields_ = [('d_tree', ctypes.c_void_p), ('capacity', ctypes.c_int32), ('n_valid', ctypes.c_int32),
+                ('alpha', ctypes.c_double), ('beta0', ctypes.c_double), ('beta_frames', ctypes.c_double),
+                ('d_rec_weights', ctypes.c_void_p), ('d_rec_td', ctypes.c_void_p)]
 
 
 _vp, _i32, _i64, _f64, _int, _shape = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_double, ctypes.c_int, ctypes.POINTER(ActorShape)
@@ -113,6 +123,15 @@ TD3_GROUP_SIGNATURES = {
 TD3_MIXED_SIGNATURES = {
     'serl_td3_train_mixed': (_int, [ctypes.POINTER(TD3Desc), _i32, _vp]),
 }
+# include/serl_td3_per.h: the priority tree's entry points and K7 with prioritized replay
+PER_SIGNATURES = {
+    'serl_per_tree_doubles': (_i64, [_i32]),
+    'serl_per_rebuild': (_int, [_vp, _i32, _vp]),
+    'serl_per_insert': (_int, [_vp, _i32, _i32, _i32, _i32, _vp]),
+    'serl_per_update': (_int, [_vp, _i32, _vp, _vp, _i32, _f64, _vp]),
+    'serl_per_sample': (_int, [_vp, _i32, _i32, _i32, ctypes.c_uint64, _i64, _f64, _vp, _vp, _vp]),
+    'serl_td3_train_per': (_int, [ctypes.POINTER(TD3Desc), ctypes.POINTER(TD3PerDesc), _vp]),
+}
 # include/serl_route.h: the kernel of a uniform actor (host only, no stream)
 ROUTE_SIGNATURES = {
     'serl_actor_tc_widths': (_i32, [_shape, _vp, _i32]),
@@ -132,7 +151,7 @@ def lib():
                               '(there is no CPU fallback)' % LIB_PATH)
         L = ctypes.CDLL(LIB_PATH)
         for name, (restype, argtypes) in {**SIGNATURES, **TD3_SIGNATURES, **TD3_GROUP_SIGNATURES, **TD3_MIXED_SIGNATURES,
-                                         **ROUTE_SIGNATURES}.items():
+                                         **PER_SIGNATURES, **ROUTE_SIGNATURES}.items():
             f = getattr(L, name)
             f.restype, f.argtypes = restype, argtypes
         _lib = L

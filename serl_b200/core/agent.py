@@ -92,8 +92,14 @@ class Agent:
             self.rl_agent = FusedTD3(args)
         else:
             self.rl_agent = td3.TD3(args)
-        self.replay_buffer = replay_memory.DeviceReplayMemory(args.buffer_size, self.device, seed=int(getattr(args, 'seed', 7)),
-                                                              state_dim=args.state_dim, action_dim=args.action_dim)
+        if getattr(args, 'per', False):
+            # the reference's agent.py:30-32 (alpha 0.6 and beta_start 0.4 are the buffer's defaults there too)
+            self.replay_buffer = replay_memory.DevicePrioritizedReplayMemory(
+                args.buffer_size, self.device, seed=int(getattr(args, 'seed', 7)), state_dim=args.state_dim,
+                action_dim=args.action_dim, beta_frames=args.num_frames)
+        else:
+            self.replay_buffer = replay_memory.DeviceReplayMemory(args.buffer_size, self.device, seed=int(getattr(args, 'seed', 7)),
+                                                                  state_dim=args.state_dim, action_dim=args.action_dim)
         self.noise_process = mod_utils.GaussianNoise(args.action_dim, sd=args.noise_sd)
         if len(self.pop):
             self.evolver = utils_ne.SSNE(self.args, self.rl_agent.critic, self.evaluate)
@@ -284,7 +290,9 @@ class Agent:
             for _ in range(int(rl_transitions * self.args.frac_frames_train)):
                 self.rl_iteration += 1
                 batch = self.replay_buffer.sample(self.args.batch_size)
-                pgl, TD = self.rl_agent.update_parameters(batch, self.rl_iteration, self.args.use_champion_target)
+                pgl, TD, *delta = self.rl_agent.update_parameters(batch, self.rl_iteration, self.args.use_champion_target)
+                if delta:                       # a prioritized batch: its rows get the step's TD errors
+                    self.replay_buffer.update_priorities(batch[6], delta[0])
                 if pgl is not None:
                     pgs_obj.append(-pgl)
                 if TD is not None:

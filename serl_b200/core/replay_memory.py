@@ -9,6 +9,7 @@ from collections import namedtuple
 import numpy as np
 import torch
 
+from .. import _native
 from ..rollout import replay_dims, transition_cols
 
 Transition = namedtuple('Transition', ('state', 'action', 'next_state', 'reward', 'done'))
@@ -169,6 +170,78 @@ class DeviceReplayMemory:
         n = len(self)
         pick = torch.randperm(n, device=self.device, generator=self.gen)[:int(batch_size)]
         return _split(self.data[pick], self.state_dim, self.action_dim)
+
+
+class DevicePrioritizedReplayMemory(DeviceReplayMemory):
+    """The reference's PrioritizedReplayMemory (base/core/replay_memory.py:103-176) on the GPU: DeviceReplayMemory's rows plus
+    a priority tree over them (include/serl_td3_per.h, csrc/per.cu) in fp64.  A new row gets the largest stored priority
+    (1.0 in an empty buffer); `sample` draws B rows with replacement with P(i) = p_i / sum p and returns them with their
+    importance weights w = (N P(i))^-beta / (N min P)^-beta and the row indices; `update_priorities` sets p = (|delta| +
+    1e-5)^alpha.  beta = min(1, beta_start + frame (1 - beta_start) / beta_frames) at the frame-th sample (frame from 1).
+    The draw of the frame-th sample is K7's draw at global iteration `frame` with Philox key `seed`, so FusedTD3 (which
+    samples this tree inside K7, td3_fused.FusedTD3.run) and the torch loop of Agent.train_rl draw the same rows."""
+
+    def __init__(self, capacity, device, seed=0, state_dim=7, action_dim=3, alpha=0.6, beta_start=0.4, beta_frames=100000):
+        super().__init__(capacity, device, seed, state_dim, action_dim)
+        self.prob_alpha, self.beta_start, self.beta_frames = float(alpha), float(beta_start), float(beta_frames)
+        self.frame = 1
+        self.tree = None
+
+    def beta_by_frame(self, frame_idx):
+        return min(1.0, self.beta_start + frame_idx * (1.0 - self.beta_start) / self.beta_frames)
+
+    def _alloc(self):
+        super()._alloc()
+        if self.tree is None:
+            n = int(_native.lib().serl_per_tree_doubles(self.capacity))
+            if n < 0:
+                raise _native.NativeError('serl_per_tree_doubles: ' + _native.lib().serl_last_error().decode())
+            self.tree = torch.empty(n, dtype=torch.float64, device=self.device)
+            self._clear_tree()
+
+    def _clear_tree(self):
+        t = self.tree.view(-1, 2)
+        t[:, 0] = 0.0                      # no stored row: sum 0, min +inf
+        t[:, 1] = float('inf')
+
+    def reset(self):
+        super().reset()
+        if self.tree is not None:
+            self._clear_tree()
+
+    def add_rows(self, rows):
+        # a bulk add gives every new or overwritten row the max stored before the add: n sequential adds of the reference
+        # would give the same, since writing the max never lowers the max
+        n = int(rows.shape[0])
+        if n == 0:
+            return
+        self._alloc()
+        n_valid, start = len(self), (self.position + max(0, n - self.capacity)) % self.capacity
+        super().add_rows(rows)
+        _native.call('serl_per_insert', self.tree, self.capacity, n_valid, start, min(n, self.capacity), device=self.device)
+
+    def sample(self, batch_size):
+        """(state, action, next_state, reward, done, weights [B, 1] fp32, rows [B] int32)"""
+        self._alloc()
+        B = int(batch_size)
+        rows = torch.empty(B, dtype=torch.int32, device=self.device)
+        weights = torch.empty((B, 1), dtype=torch.float32, device=self.device)
+        _native.call('serl_per_sample', self.tree, self.capacity, len(self), B, self._seed, self.frame,
+                     self.beta_by_frame(self.frame), rows, weights, device=self.device)
+        self.frame += 1
+        return _split(self.data[rows.long()], self.state_dim, self.action_dim) + (weights, rows)
+
+    def update_priorities(self, batch_indices, batch_priorities):
+        """rows batch_indices [B] get (|delta| + 1e-5)^alpha from batch_priorities = delta [B] (batch order: a row drawn twice
+        keeps its later delta)"""
+        rows = torch.as_tensor(batch_indices, device=self.device).to(torch.int32).reshape(-1).contiguous()
+        td = torch.as_tensor(batch_priorities, device=self.device).to(torch.float32).reshape(-1).abs().contiguous()
+        _native.call('serl_per_update', self.tree, self.capacity, rows, td, int(rows.numel()), self.prob_alpha, device=self.device)
+
+    def leaves(self):
+        """the priorities of the stored rows (fp64 [len])"""
+        self._alloc()
+        return self.tree.view(-1, 2)[self.tree.numel() // 4:, 0][:len(self)]
 
 
 class PopulationBuffers:

@@ -61,14 +61,22 @@ class TD3:
         self.caps_dict = {'lambda_s': 0.5, 'lambda_t': 0.1, 'eps_sd': 0.05} if args.use_caps else None
 
     def update_parameters(self, batch, iteration, champion_policy=False):
-        state, action, next_state, reward, done = (b.to(self.args.device) for b in batch)
+        """batch: (state, action, next_state, reward, done), or a prioritized sample (DevicePrioritizedReplayMemory.sample:
+        ..., weights [B, 1], rows): then the critic loss is mean(w (q1 - y)^2) + mean(w (q2 - y)^2), and the per-row TD
+        error delta = (|q1 - y| + |q2 - y|) / 2 of the critic before its update is returned third, for update_priorities"""
+        state, action, next_state, reward, done = (b.to(self.args.device) for b in batch[:5])
+        weights = batch[5].to(self.args.device) if len(batch) > 5 else None
         with torch.no_grad():
             noise = (torch.randn_like(action) * self.args.noise_sd).clamp(-self.args.noise_clip, self.args.noise_clip)
             next_action = torch.clamp(noise + self.actor_target(next_state), -1, 1)
             q1, q2 = self.critic_target(next_state, next_action)
             target_q = reward + self.gamma * torch.min(q1, q2) * (1 - done)
         cq1, cq2 = self.critic(state, action)
-        td = F.mse_loss(cq1, target_q) + F.mse_loss(cq2, target_q)
+        if weights is None:
+            td = F.mse_loss(cq1, target_q) + F.mse_loss(cq2, target_q)
+        else:
+            td = torch.mean(weights * (cq1 - target_q) ** 2) + torch.mean(weights * (cq2 - target_q) ** 2)
+            delta = (((cq1 - target_q).abs() + (cq2 - target_q).abs()) * 0.5).detach().reshape(-1)
         self.critic_optim.zero_grad()
         td.backward()
         nn.utils.clip_grad_norm_(self.critic.parameters(), MAX_GRAD_NORM)
@@ -88,4 +96,6 @@ class TD3:
                 soft_update(self.actor_target, self.actor, self.tau)
             soft_update(self.critic_target, self.critic, self.tau)
             pgl = loss.data.cpu().numpy()
+        if weights is not None:
+            return pgl, td.data.cpu().numpy(), delta
         return pgl, td.data.cpu().numpy()

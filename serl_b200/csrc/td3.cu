@@ -22,7 +22,9 @@
 
 #include "../../include/serl_td3.h"
 #include "../../include/serl_td3_mixed.h"
+#include "../../include/serl_td3_per.h"
 #include "common.cuh"
+#include "per.cuh"
 
 namespace {
 
@@ -45,6 +47,13 @@ struct Args {
     const int* idx_in;
     float* losses; int* rec_idx; float* rec_noise; float* rec_caps; int* status;
     float* ws;
+};
+
+// what a PER launch adds (serl_td3_train_per): the priority tree and its parameters, the optional records
+struct Per {
+    double* tree; int leaves, n_valid;
+    double alpha, beta0, beta_frames;
+    float *rec_w, *rec_td;
 };
 
 // scratch layout (floats); per block of a net: Z (linear output, LN blocks), A (activation output), dU (gradient at the
@@ -111,19 +120,7 @@ __device__ __forceinline__ float warp_sum(float v)
     return v;
 }
 
-// Philox4x32-10 (Salmon et al., SC'11)
-__device__ __forceinline__ uint4 philox(uint4 c, uint2 k)
-{
-#pragma unroll
-    for (int i = 0; i < 10; ++i) {
-        const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
-        const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
-        c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
-        k.x += 0x9E3779B9u; k.y += 0xBB67AE85u;
-    }
-    return c;
-}
-enum { TAG_INDEX = 0, TAG_NOISE = 1, TAG_CAPS = 2 };
+enum { TAG_INDEX = 0, TAG_NOISE = 1, TAG_CAPS = 2 };      // TAG_CAPS + 1 too; PER_TAG (per.cuh) follows
 __device__ __forceinline__ uint4 draw(const Args& a, long long it, int row, int tag)
 {
     return philox(make_uint4((uint32_t)it, (uint32_t)((unsigned long long)it >> 32), (uint32_t)row, (uint32_t)tag),
@@ -505,9 +502,11 @@ __device__ void adam(float* p, float* m, float* v, float* tgt, const float* g, i
 
 // the step's batch (CTA 0): Floyd's sample of B distinct rows of [0, n_valid) — row j draws t_j uniform in
 // [0, n - B + j] and keeps it unless an earlier row holds it, else takes n - B + j — then the gathered transitions, the
-// clipped target-policy noise and the CAPS perturbation, written to the inputs of the step's networks
+// clipped target-policy noise and the CAPS perturbation, written to the inputs of the step's networks.  PER: B rows drawn
+// with replacement from the priority tree instead, and their importance weights (beta of the learner's critic step) in wt
+template <bool PER = false>
 __device__ void draw_batch(const Args& a, int k, long long it, int* pick, int* tdraw, float* Xt, float* Xs, float* Xp, float* Xa,
-                           float* rw, float* dn)
+                           float* rw, float* dn, const Per* p = nullptr, float* wt = nullptr)
 {
     const int B = a.B, n = a.n_valid, tid = threadIdx.x;
     if (a.idx_in) {
@@ -516,6 +515,8 @@ __device__ void draw_batch(const Args& a, int k, long long it, int* pick, int* t
             if (r < 0 || r >= n) { atomicOr(a.status, SERL_TD3_STATUS_INDEX); r = 0; }
             pick[j] = r;
         }
+    } else if constexpr (PER) {
+        for (int j = tid; j < B; j += NT) pick[j] = per_draw(p->tree, p->leaves, a.seed, it, j);
     } else {
         for (int j = tid; j < B; j += NT)
             tdraw[j] = (int)__umulhi(draw(a, it, j, TAG_INDEX).x, (uint32_t)(n - B + j + 1));
@@ -565,13 +566,21 @@ __device__ void draw_batch(const Args& a, int k, long long it, int* pick, int* t
         if (a.rec_caps)
 #pragma unroll
             for (int i = 0; i < SD; ++i) a.rec_caps[((size_t)k * B + j) * SD + i] = u[i];
+        if constexpr (PER) {
+            const double f = (double)(a.tc0 + k + 1);          // the learner's f-th sample (the reference's frame)
+            const float w = per_weight(p->tree, p->leaves, p->n_valid, pick[j], fmin(1.0, p->beta0 + f * (1.0 - p->beta0) / p->beta_frames));
+            wt[j] = w;
+            if (p->rec_w) p->rec_w[(size_t)k * B + j] = w;
+        }
     }
 }
 
 // One learner's n_steps on one cluster.  WIDE: the actor's hidden blocks take the tiled phases (fwd_wide / bwd_wide,
-// WIDE_SMEM bytes of shared memory).  G: the cluster is one of a group launch's (crank).
-template <int CS, bool WIDE, bool G>
-__device__ __forceinline__ void td3_learner(const Args a)
+// WIDE_SMEM bytes of shared memory).  G: the cluster is one of a group launch's (crank).  PER: prioritized replay (p) —
+// the batch from the priority tree, the critic loss weighted, and CTA 0 re-prioritises the batch's rows in the phase after
+// the critic's forward pass; the weights live after the scratch layout (B floats).
+template <int CS, bool WIDE, bool G, bool PER = false>
+__device__ __forceinline__ void td3_learner(const Args a, const Per* p = nullptr)
 {
     __shared__ int pick[SERL_TD3_MAX_BATCH], tdraw[SERL_TD3_MAX_BATCH];
     __shared__ float s_coef;
@@ -598,7 +607,11 @@ __device__ __forceinline__ void td3_learner(const Args a)
         const long long it = a.it0 + k;
         const bool actor_step = it % a.freq == 0;
         float td = 0.f, pg = __int_as_float(0x7fc00000);
-        if (crank<G>() == 0) draw_batch(a, k, it, pick, tdraw, Xt, Xs, Xp, Xa, rw, dn);
+        if constexpr (PER) {
+            if (crank<G>() == 0) draw_batch<true>(a, k, it, pick, tdraw, Xt, Xs, Xp, Xa, rw, dn, p, ws + l.total);
+        } else {
+            if (crank<G>() == 0) draw_batch(a, k, it, pick, tdraw, Xt, Xs, Xp, Xa, rw, dn);
+        }
         csync<CS>();
         // ---- target: a' = clamp(actor_target(s') + noise, +-1); y = r + gamma * min(q1', q2') * (1 - done)
         for (int kb = 0; kb <= la; ++kb) {
@@ -636,9 +649,22 @@ __device__ __forceinline__ void td3_learner(const Args a)
         }
         fwd_lin<CS, G>(critic, 2, 2, B, Xs, CI, [&](int hd, int r, int, float v) {
             critic.A(2)[hd * B + r] = v;
-            critic.dU(2)[hd * B + r] = 2.f * inv_b * (v - ld(yt + r));
+            if constexpr (PER) critic.dU(2)[hd * B + r] = 2.f * inv_b * ld(ws + l.total + r) * (v - ld(yt + r));
+            else critic.dU(2)[hd * B + r] = 2.f * inv_b * (v - ld(yt + r));
         });
         csync<CS>();
+        if constexpr (PER) {
+            if (crank<G>() == 0) {     // delta of the pre-update critic (in tdraw, which the tree's draw leaves unused)
+                float* td_row = reinterpret_cast<float*>(tdraw);
+                for (int r = threadIdx.x; r < B; r += NT) {
+                    const float y = ld(yt + r);
+                    td_row[r] = 0.5f * (fabsf(ld(critic.A(2) + r) - y) + fabsf(ld(critic.A(2) + B + r) - y));
+                    if (p->rec_td) p->rec_td[(size_t)k * B + r] = td_row[r];
+                }
+                __syncthreads();
+                per_reprioritise(p->tree, p->leaves, pick, td_row, B, p->alpha);
+            }
+        }
         bwd_lin<CS, G>(critic, 2, 2, B, Xs, CI, true, true); csync<CS>();
         bwd_ln<CS, G>(critic, 1, 2, B); csync<CS>();
         bwd_lin<CS, G>(critic, 1, 2, B, Xs, CI, true, true); csync<CS>();
@@ -648,7 +674,12 @@ __device__ __forceinline__ void td3_learner(const Args a)
             float s1 = 0.f, s2 = 0.f;
             for (int r = 0; r < B; ++r) {
                 const float y = ld(yt + r), d1 = ld(critic.A(2) + r) - y, d2 = ld(critic.A(2) + B + r) - y;
-                s1 = fmaf(d1, d1, s1); s2 = fmaf(d2, d2, s2);
+                if constexpr (PER) {
+                    const float w = ld(ws + l.total + r);
+                    s1 = fmaf(w * d1, d1, s1); s2 = fmaf(w * d2, d2, s2);
+                } else {
+                    s1 = fmaf(d1, d1, s1); s2 = fmaf(d2, d2, s2);
+                }
             }
             td = s1 / (float)B + s2 / (float)B;
         }
@@ -781,6 +812,15 @@ __global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_mixed_ke
     asm("mov.u32 %0, %%clusterid.x;" : "=r"(g));
     if (t.a[g].h > 128) td3_learner<CS, true, true>(t.a[g]);
     else narrow_learner<CS>(t.a[g]);
+}
+
+// A PER launch (serl_td3_train_per): one learner, its Args and Per as one __grid_constant__ parameter
+struct PerLaunch { Args a; Per p; };
+
+template <int CS, bool WIDE>
+__global__ void __cluster_dims__(CS, 1, 1) __launch_bounds__(NT, 1) td3_per_kernel(const __grid_constant__ PerLaunch t)
+{
+    td3_learner<CS, WIDE, false, true>(t.a, &t.p);
 }
 
 int64_t actor_floats(const serl_actor_shape& s)
@@ -955,4 +995,54 @@ extern "C" int serl_td3_train_group(const serl_td3_desc* descs, int n, void* str
 extern "C" int serl_td3_train_mixed(const serl_td3_desc* descs, int n, void* stream)
 {
     return train_group("serl_td3_train_mixed", descs, n, stream, false);
+}
+
+namespace {
+
+template <int CS>
+int launch_per(const PerLaunch& t, cudaStream_t s)
+{
+    if (t.a.h > 128) return serl_launch("td3_per_kernel (wide)", td3_per_kernel<CS, true>, dim3(CS), dim3(NT), 0, s, t);
+    return serl_launch("td3_per_kernel", td3_per_kernel<CS, false>, dim3(CS), dim3(NT), 0, s, t);
+}
+
+const char* per_error(const serl_td3_desc* d, const serl_td3_per_desc* p)
+{
+    if (!p) return "null per descriptor";
+    if (!p->d_tree) return "null d_tree";
+    if (p->capacity < 1 || p->capacity > SERL_PER_MAX_CAPACITY) return "capacity must be 1..SERL_PER_MAX_CAPACITY";
+    if (p->n_valid != d->n_valid || p->n_valid > p->capacity) return "n_valid must equal the desc's n_valid and be <= capacity";
+    if (!(p->alpha > 0.0 && p->alpha <= 1.0)) return "alpha must be in (0, 1]";
+    if (!(p->beta0 >= 0.0 && p->beta0 <= 1.0)) return "beta0 must be in [0, 1]";
+    if (!(p->beta_frames > 0.0)) return "beta_frames must be > 0";
+    return nullptr;
+}
+
+}  // namespace
+
+extern "C" int serl_td3_train_per(const serl_td3_desc* d, const serl_td3_per_desc* p, void* stream)
+{
+    if (!d) return serl_fail(SERL_ERR_ARG, "serl_td3_train_per: null descriptor");
+    const char* why = desc_error(d);
+    if (!why) why = per_error(d, p);
+    if (why) {
+        char msg[256];
+        snprintf(msg, sizeof(msg), "serl_td3_train_per: %s", why);
+        return serl_fail(SERL_ERR_ARG, msg);
+    }
+    if (d->n_steps == 0) return SERL_OK;
+    PerLaunch t;
+    t.a = make_args(d);
+    t.p = Per{p->d_tree, per_leaves(p->capacity), p->n_valid, p->alpha, p->beta0, p->beta_frames, p->d_rec_weights, p->d_rec_td};
+    const cudaStream_t s = (cudaStream_t)stream;
+    void* ws = nullptr;
+    const cudaError_t e = serl_scratch(SERL_SCRATCH_TD3, s, (scratch_floats(t.a) + t.a.B) * sizeof(float), &ws);    // + the weights
+    if (e != cudaSuccess) return serl_fail_cuda(e, "td3 scratch");
+    t.a.ws = (float*)ws;
+    switch (d->cluster_size ? d->cluster_size : 8) {
+    case 1: return launch_per<1>(t, s);
+    case 2: return launch_per<2>(t, s);
+    case 4: return launch_per<4>(t, s);
+    default: return launch_per<8>(t, s);
+    }
 }

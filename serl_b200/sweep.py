@@ -111,6 +111,9 @@ class Sweep:
                 raise ValueError('Sweep: run %d flies incremental control (state_dim 10), which fused_td3 (K7) does not train' % i)
             if (p.state_dim, p.action_dim) == (SYMMETRIC_STATE_DIM, SYMMETRIC_ACTION_DIM):
                 raise ValueError('Sweep: run %d flies symmetric control (state_dim 2, action_dim 1), which fused_td3 (K7) does not train' % i)
+            if getattr(p, 'per', False):
+                raise ValueError('Sweep: run %d sets per (prioritized experience replay), which the grouped K7 launch does not '
+                                 'train; train it alone with Agent' % i)
             if not getattr(p, 'fused_td3', False):
                 raise ValueError('Sweep: run %d does not set fused_td3 (the sweep trains every RL half in one K7 launch)' % i)
             if mixed_shapes:

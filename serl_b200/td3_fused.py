@@ -11,7 +11,7 @@ import numpy as np
 import torch
 
 from . import _native
-from .core import td3
+from .core import replay_memory, td3
 from .rollout import INCREMENTAL_STATE_DIM, SYMMETRIC_ACTION_DIM, SYMMETRIC_STATE_DIM, TRANSITION_COLS, actor_shape
 
 # steps per launch: keeps every launch well under a second at the largest population
@@ -20,8 +20,9 @@ LAUNCH_STEPS = 8192
 
 class TD3Launch:
     """what one or more K7 launches returned: losses [n, 2] (td, pg; pg NaN on critic-only steps), the recorded draws
-    (indices [n, B] int32, noise [n, B, 3], caps [n, B, 7]) when asked for, and the status word."""
-    __slots__ = ('losses', 'indices', 'noise', 'caps', 'status')
+    (indices [n, B] int32, noise [n, B, 3], caps [n, B, 7]; with prioritized replay also weights [n, B] and the TD errors
+    delta [n, B]) when asked for, and the status word."""
+    __slots__ = ('losses', 'indices', 'noise', 'caps', 'weights', 'td', 'status')
 
     def check(self):
         st = int(self.status.item())
@@ -63,36 +64,42 @@ class FusedTD3(td3.TD3):
             _bind(mod, self.state[off:off + k])
         self.status = torch.zeros(1, dtype=torch.int32, device=dev)
 
-    def run(self, rows, n_valid, n, first_iteration, champion_target=False, indices=None, record=False, cluster_size=None):
+    def run(self, rows, n_valid, n, first_iteration, champion_target=False, indices=None, record=False, cluster_size=None, per=None):
         """n consecutive gradient steps on global iterations first_iteration.. (launches of at most LAUNCH_STEPS) on the replay
-        rows [>= n_valid, >= 19] fp32 (device, row-contiguous).  indices [n, B] int32 replaces the sampler's draw."""
+        rows [>= n_valid, >= 19] fp32 (device, row-contiguous).  indices [n, B] int32 replaces the sampler's draw.  per: the
+        DevicePrioritizedReplayMemory whose rows these are — prioritized replay (serl_td3_train_per) on its tree."""
         B = int(self.args.batch_size)
         dev = self.state.device
         assert rows.is_cuda and rows.dtype == torch.float32 and rows.dim() == 2 and rows.shape[1] >= TRANSITION_COLS
         assert rows.stride(1) == 1 and rows.shape[0] >= n_valid
-        r = self._launch(n, record)
+        r = self._launch(n, record, per=per is not None)
         if indices is not None:
             assert indices.shape == (n, B) and indices.dtype == torch.int32 and indices.is_cuda and indices.is_contiguous()
         k0 = 0
         while k0 < n:
             m = min(LAUNCH_STEPS, n - k0)
             d = self._desc(rows, n_valid, m, int(first_iteration) + k0, champion_target, indices, r, k0, cluster_size)
-            _native.call('serl_td3_train', d, device=dev)
+            if per is None:
+                _native.call('serl_td3_train', d, device=dev)
+            else:
+                _native.call('serl_td3_train_per', d, self._per_desc(per, n_valid, r, k0), device=dev)
             self._advance(int(first_iteration) + k0, m)
             k0 += m
         if n:
             self._bump_versions()
         return r
 
-    def _launch(self, n, record, losses=None):
-        """a TD3Launch with losses [n, 2] (new, or the given view) and, when `record`, the draw records; its status word is
-        zeroed"""
+    def _launch(self, n, record, losses=None, per=False):
+        """a TD3Launch with losses [n, 2] (new, or the given view) and, when `record`, the draw records (and with `per` the
+        weight and TD-error records); its status word is zeroed"""
         B, dev = int(self.args.batch_size), self.state.device
         r = TD3Launch()
         r.losses = torch.empty((n, 2), dtype=torch.float32, device=dev) if losses is None else losses
         r.indices = torch.empty((n, B), dtype=torch.int32, device=dev) if record else None
         r.noise = torch.empty((n, B, 3), dtype=torch.float32, device=dev) if record else None
         r.caps = torch.empty((n, B, 7), dtype=torch.float32, device=dev) if record else None
+        r.weights = torch.empty((n, B), dtype=torch.float32, device=dev) if record and per else None
+        r.td = torch.empty((n, B), dtype=torch.float32, device=dev) if record and per else None
         r.status = self.status
         self.status.zero_()
         return r
@@ -119,6 +126,16 @@ class FusedTD3(td3.TD3):
         d.d_status = self.status.data_ptr()
         return d
 
+    @staticmethod
+    def _per_desc(buf, n_valid, r, k0):
+        """the TD3PerDesc of prioritized replay on the buffer `buf`'s tree, writing r's records from row k0"""
+        p = _native.TD3PerDesc()
+        p.d_tree, p.capacity, p.n_valid = buf.tree.data_ptr(), buf.capacity, int(n_valid)
+        p.alpha, p.beta0, p.beta_frames = buf.prob_alpha, buf.beta_start, buf.beta_frames
+        p.d_rec_weights = r.weights[k0:].data_ptr() if r.weights is not None else None
+        p.d_rec_td = r.td[k0:].data_ptr() if r.td is not None else None
+        return p
+
     def _advance(self, first, m):
         """the Adam step counts after m steps from global iteration `first`"""
         its = np.arange(first, first + m)
@@ -133,10 +150,12 @@ class FusedTD3(td3.TD3):
                 torch.autograd.graph.increment_version(q)
 
     def train_steps(self, replay, n, first_iteration, champion_target=False):
-        """n gradient steps sampling from `replay` (DeviceReplayMemory, or a [rows, >= 19] device tensor); returns the device
-        losses [n, 2] (td, pg; pg NaN on critic-only steps)."""
+        """n gradient steps sampling from `replay` (DeviceReplayMemory, DevicePrioritizedReplayMemory — prioritized replay
+        on its tree —, or a [rows, >= 19] device tensor); returns the device losses [n, 2] (td, pg; pg NaN on critic-only
+        steps)."""
         rows, n_valid = _rows(replay)
-        return self.run(rows, n_valid, int(n), first_iteration, champion_target).losses
+        per = replay if isinstance(replay, replay_memory.DevicePrioritizedReplayMemory) else None
+        return self.run(rows, n_valid, int(n), first_iteration, champion_target, per=per).losses
 
     def update_parameters(self, batch, iteration, champion_policy=False):
         """one step on the given batch (state, action, next_state, reward, done), as TD3.update_parameters"""
