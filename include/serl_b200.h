@@ -251,7 +251,9 @@ int serl_ssne_select(const double* d_fitness, int32_t pop, const int32_t* d_draw
 int serl_ssne_clone(float* d_weights, int32_t pop, int32_t P, const int32_t* d_pairs, int32_t n, void* stream);
 
 /* K4: per pair {g1,g2,src1,src2,op_begin,op_count} (d_pair_desc [n_pairs,6]): clone src1->g1, src2->g2 (:519-522)
- * then crossover_inplace (:61-93) as ordered copies d_ops [.,3] = {offset,len,dir} (dir 0: g1<-g2, 1: g2<-g1). */
+ * then crossover_inplace (:61-93) as ordered copies d_ops [.,3] = {offset,len,dir} (dir 0: g1<-g2, 1: g2<-g1).
+ * Ops that touch the same element must have the same offset and len (a whole row of a parameter matrix, or one element
+ * of a vector, as crossover_inplace copies them): the ops of a pair are kept in order without barriers. */
 int serl_ssne_crossover(float* d_weights, int32_t pop, int32_t P, const int32_t* d_pair_desc, int32_t n_pairs,
                         const int32_t* d_ops, void* stream);
 

@@ -7,8 +7,11 @@ mutate_inplace :329-369, clone :371-376, with the documented patches (SURVEY.md 
   * ranking is `np.argsort(fitness, kind='stable')[::-1]` — the reference calls the default (unstable) quicksort,
     whose order among exactly equal fitness values is platform dependent; stable-reversed is the documented rule.
 Random numbers are consumed from the stdlib `random` and legacy `np.random` global streams in the reference's order.
-Arithmetic follows torch's fp32 semantics for 0-d tensor (x) python-scalar expressions (validated against the
-reference module itself in tests/test_ssne_reference.py).
+Arithmetic follows torch's fp32 semantics for 0-d tensor (x) python-scalar expressions. A point mutation adds
+random.gauss(0, s*w) = 0 + z*(s*w), so a zero increment is +0.0 and a -0.0 weight comes out +0.0; NaN stays NaN through
+the clamp. Validated against the reference module itself: tests/golden/ssne_kat.npz (tests/test_oracle_ssne.py) and,
+over the engine's actor shapes with planted signed zeros, NaNs, infinities and subnormals,
+tests/golden/ssne_domain_kat.npz (tests/test_evo_domain.py).
 """
 import math
 import random
@@ -97,12 +100,12 @@ class SSNE:
                     w = W[g, k]
                     if random_num < 0.05:
                         z = random.gauss(0, 1)
-                        w = f32(w + f32(f32(z) * f32(f32(super_mut_strength) * w)))
+                        w = f32(w + f32(f32(0) + f32(f32(z) * f32(f32(super_mut_strength) * w))))
                     elif random_num < 0.1:
                         w = f32(random.gauss(0, 1))
                     else:
                         z = random.gauss(0, 1)
-                        w = f32(w + f32(f32(z) * f32(f32(mag) * w)))
+                        w = f32(w + f32(f32(0) + f32(f32(z) * f32(f32(mag) * w))))
                     W[g, k] = min(max(w, f32(-1000000)), f32(1000000))
 
     # :447-543 (classic branch)

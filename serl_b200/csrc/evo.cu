@@ -61,7 +61,8 @@ __global__ void ssne_clone_kernel(float* __restrict__ W, int P, const int* __res
 
 // ---- K4 ------------------------------------------------------------------------------------------------
 // desc[pair] = {g1, g2, src1, src2, op_begin, op_count}; ops[k] = {offset, len, dir}; dir 0: g1[..] = g2[..], 1: g2[..] = g1[..].
-// A thread always owns the same columns of a row, so ops on the same row stay ordered without barriers.
+// Every op on a row has that row's offset and length, so a thread always owns the same columns of a row, and ops on the
+// same row stay ordered without barriers.
 __global__ void ssne_crossover_kernel(float* __restrict__ W, int P, const int* __restrict__ desc, const int* __restrict__ ops)
 {
     const int* d = desc + 6 * blockIdx.x;
@@ -87,6 +88,8 @@ __global__ void ssne_crossover_kernel(float* __restrict__ W, int P, const int* _
 // ---- K5 ------------------------------------------------------------------------------------------------
 // seg[s] = {actor, op_begin, op_count}: the ordered point mutations of one 2-D parameter of one actor.
 // kind 0: w += z*(mag*w)   1: w += z*(10mag*w)   2: w = z ; then clamp to +-1e6   (mod_neuro_evo.py:360-369, :57-59)
+// The reference adds random.gauss(0, s*w) = 0 + z*(s*w): the increment is rounded through 0 + x, so a zero increment is
+// +0.0 and a -0.0 weight comes out +0.0. torch.clamp keeps NaN, which fminf / fmaxf would turn into -1e6.
 __global__ void ssne_mutate_kernel(float* __restrict__ W, int P, const int* __restrict__ seg, int n_seg,
                                    const int* __restrict__ op_off, const int* __restrict__ op_kind, const float* __restrict__ op_z,
                                    float mag32, float super32)
@@ -101,8 +104,9 @@ __global__ void ssne_mutate_kernel(float* __restrict__ W, int P, const int* __re
         const float z = op_z[k];
         float w = g[off];
         if (kind == 2) w = z;
-        else w = __fadd_rn(w, __fmul_rn(z, __fmul_rn(kind == 1 ? super32 : mag32, w)));
-        w = fminf(fmaxf(w, -1000000.0f), 1000000.0f);
+        else w = __fadd_rn(w, __fadd_rn(0.0f, __fmul_rn(z, __fmul_rn(kind == 1 ? super32 : mag32, w))));
+        const float c = fminf(fmaxf(w, -1000000.0f), 1000000.0f);
+        w = w != w ? w : c;
         g[off] = w;
     }
 }

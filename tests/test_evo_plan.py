@@ -1,5 +1,5 @@
-"""CPU tests of the neuro-evolution planner (serl_b200/evo.py): the op lists it emits, applied by a tiny numpy
-interpreter, must reproduce the genomes recorded from the reference module (tests/golden/ssne_kat.npz)."""
+"""CPU tests of the neuro-evolution planner (serl_b200/evo.py): the op lists it emits, applied by the numpy model of
+K3/K4/K5 (tests/ssne_domain_cases.py), must reproduce the genomes recorded from the reference module (tests/golden/ssne_kat.npz)."""
 import os
 import random
 
@@ -8,44 +8,10 @@ import pytest
 
 from serl_b200 import evo
 from oracle import ssne as OS
+from ssne_domain_cases import host_select, interpret
 
 KAT = np.load(os.path.join(os.path.dirname(__file__), 'golden', 'ssne_kat.npz'))
 CASES = sorted({k.split('_')[0] for k in KAT.files})
-
-
-def interpret(W, plan, mag):
-    """numpy model of K3/K4/K5 (csrc/evo.cu)."""
-    f32 = np.float32
-    for wave in plan.clone_waves:
-        src = W[wave[:, 0]].copy()
-        W[wave[:, 1]] = src                       # all ops of a launch are independent by construction
-    for desc, ops in plan.cross_waves:
-        snap = W.copy()
-        for g1, g2, s1, s2, b, n in desc:
-            W[g1] = snap[s1]
-            W[g2] = snap[s2]
-            for off, ln, d in ops[b:b + n]:
-                if d == 0:
-                    W[g1, off:off + ln] = W[g2, off:off + ln]
-                else:
-                    W[g2, off:off + ln] = W[g1, off:off + ln]
-    for a, b, n in plan.mut_seg:
-        for k in range(b, b + n):
-            w = W[a, plan.mut_off[k]]
-            z = plan.mut_z[k]
-            if plan.mut_kind[k] == 2:
-                w = z
-            else:
-                s = f32(10 * mag) if plan.mut_kind[k] == 1 else f32(mag)
-                w = f32(w + f32(z * f32(s * w)))
-            W[a, plan.mut_off[k]] = min(max(w, f32(-1e6)), f32(1e6))
-
-
-def host_select(fit, num_elitists):
-    pop = len(fit)
-    draws = np.stack([np.random.randint(pop, size=3) for _ in range(pop - num_elitists)])
-    rank = np.argsort(fit, kind='stable')[::-1]
-    return rank, rank[draws.min(1)]
 
 
 @pytest.mark.parametrize('native', [False, True])
