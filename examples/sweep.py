@@ -6,6 +6,8 @@ shape's population flies in a launch of its own.
 
     python examples/sweep.py -frames 20000 -pop_size 10 -seeds 7 8 9 -grid lr=0.0002,0.0004 noise_sd=0.2,0.3
     python examples/sweep.py -frames 20000 -pop_size 10 -grid hidden_size=72,96 activation_actor=tanh,relu
+    python examples/sweep.py -frames 20000 -pop_size 10 -seeds 7 8 9 -checkpoint_every 5     # ./tmp/checkpoint/ every 5
+    python examples/sweep.py -frames 40000 -pop_size 10 -seeds 7 8 9 -resume tmp/checkpoint    # continued to 40000 frames
 """
 import itertools
 import os
@@ -49,6 +51,8 @@ def make_runs(cla):
             p = Parameters(cla)
             p.hidden_size = cla.hidden_size
             p.fused_td3 = True
+            if cla.learn_start is not None:
+                p.learn_start = cla.learn_start
             label = ['seed=%d' % seed]
             for (name, _), text in zip(axes, combo):
                 if not hasattr(p, name):
@@ -66,6 +70,8 @@ if __name__ == '__main__':
     cla = parser.parse_args()
     runs = make_runs(cla)
     sweep = Sweep([(p, env) for _, p, env in runs], mixed_shapes=True)
+    if cla.resume:
+        sweep.load_checkpoint(cla.resume)
     print('Sweep of %d runs on' % len(runs), runs[0][1].env_name)
     start_time = time.time()
     while not sweep.finished:
@@ -76,4 +82,6 @@ if __name__ == '__main__':
             print('[%s]' % label, 'Episodes:', a.num_episodes, 'Frames:', a.num_frames, ' Train Max: %.2f' % stats['best_train_fitness'],
                   ' Test Max: %.2f' % stats['test_score'], ' Population Avg: %.2f' % stats['pop_avg'], ' Weakest: %.2f' % stats['pop_min'],
                   ' Avg. ep. len: %.2fs' % stats['avg_ep_len'], ' RL Reward: %.2f' % stats['rl_reward'], ' time %.1fs' % (time.time() - start_time))
+        if cla.checkpoint_every and max(r.agent.iterations for r in sweep.runs) % cla.checkpoint_every == 0:
+            sweep.save_checkpoint(os.path.join(runs[0][1].save_foldername, 'checkpoint'))
     sweep.save_agent()

@@ -50,8 +50,8 @@ class _Generation:
 class _Front:
     """the launches a generation starts with: RL exploration / validation flights, speculative champion validations, the
     population rollout — and the signature of what they read.  `pop_draws` holds the population's reference draws while
-    its launch is deferred (launch_population_group), `pop` the launched rollout."""
-    __slots__ = ('signature', 'f_explore', 'f_rlval', 'spec', 'val_draws', 'pop', 'pop_draws', 'sm_limit')
+    its launch is deferred (launch_population_group), `pop` the launched rollout, `draws` the draws either way."""
+    __slots__ = ('signature', 'f_explore', 'f_rlval', 'spec', 'val_draws', 'pop', 'pop_draws', 'draws', 'sm_limit')
 
 
 class _PopDraws:
@@ -155,8 +155,11 @@ class Agent:
         kw = {} if env.t_max == 20 else {'t_max': float(env.t_max), 'smooth_width': refsig.widths(env.t_max, sym)[1]}
         return dict(kw, gust=rollout.mode_gust(env.mode_code))
 
-    def _fly(self, agent, n, is_action_noise=False, store_transition=False, trace=False, stream=None, copy_genome=False, draws=None) -> _Flight:
-        """launch n episodes of one actor (fresh reference signals each, or the given `draws`) without waiting for them."""
+    def _fly(self, agent, n, is_action_noise=False, store_transition=False, trace=False, stream=None, copy_genome=False, draws=None,
+             noise_state=None) -> _Flight:
+        """launch n episodes of one actor (fresh reference signals each, or the given `draws`) without waiting for them.  The
+        action noise is drawn from the global np.random stream, or from the given legacy state `noise_state` (a flight
+        re-launched from a checkpoint), which leaves the global stream untouched."""
         env = self.env
         draws = draws if draws is not None else [env.draw_reference() for _ in range(n)]
         f = _Flight()
@@ -169,8 +172,14 @@ class Agent:
             # "exactly the steps that ran" once the episode length is known (collect)
             assert n == 1
             A = self.shape.action_dim
-            f.noise_state = np.random.get_state()
-            z = np.random.randn(horizon, A)
+            if noise_state is None:
+                f.noise_state = np.random.get_state()
+                z = np.random.randn(horizon, A)
+            else:
+                f.noise_state = noise_state
+                rs = np.random.RandomState()
+                rs.set_state(noise_state)
+                z = rs.randn(horizon, A)
             noise_host = np.clip(self.args.noise_sd * z, -self.args.noise_clip, self.args.noise_clip).astype(np.float32).reshape(1, 1, -1, A)
         f.stream = stream
         ctx = torch.cuda.stream(stream) if stream is not None else _null()
@@ -440,25 +449,30 @@ class Agent:
                 tuple(p._version for p in self.rl_agent.actor.parameters()),
                 id(env), env.mode_code, float(env.t_max), int(getattr(self.args, 'num_envs', self.args.num_evals)), len(self.pop))
 
-    def _launch_front(self):
+    def _launch_front(self, inputs=None):
         """queue a generation's front.  With defer_population the population's references are drawn at their place in the
-        front (the np.random stream advances as without it) and its launch is left to launch_population_group."""
+        front (the np.random stream advances as without it) and its launch is left to launch_population_group.  `inputs`
+        (checkpoint.front_inputs of a front launched earlier) re-launches that front from its host-side draws: the same
+        launches on the same inputs, and no draw from the global streams."""
         args = self.args
         fr = _Front()
         fr.signature = self._signature()
-        fr.pop_draws, fr.sm_limit = None, 0
+        fr.pop_draws, fr.draws, fr.sm_limit = None, None, 0
         log = bool(args.should_log)
+        given = inputs if inputs is not None else {}
         # RL exploration episode (agent.py:267-268): independent of the population -> side stream, launched first.  The RL
         # validation (:273-275) reads the RL actor AFTER train_rl; when no gradient step can happen it joins the side stream.
-        fr.f_explore = self._fly(self.rl_agent, 1, is_action_noise=True, store_transition=True, trace=log, stream=self._side)
-        fr.f_rlval = self._fly(self.rl_agent, self.validation_tests, trace=log, stream=self._side2) if args.frac_frames_train == 0 else None
+        fr.f_explore = self._fly(self.rl_agent, 1, is_action_noise=True, store_transition=True, trace=log, stream=self._side,
+                                 draws=given.get('explore'), noise_state=given.get('noise_state'))
+        fr.f_rlval = (self._fly(self.rl_agent, self.validation_tests, trace=log, stream=self._side2, draws=given.get('rlval'))
+                      if args.frac_frames_train == 0 else None)
         fr.spec, fr.val_draws, fr.pop = {}, None, None
         if len(self.pop):
             # Speculative champion validation: the champion is only known after the ranking, and its 5 validation episodes
             # are ~0.15 s of serial latency.  The ranked elites of the previous generation survive unchanged (and so do
             # their protected clones), and one of the best of them usually wins again: their validation episodes are
             # launched NOW, next to the population rollout; a miss falls back to the serial launch.
-            fr.val_draws = [self.env.draw_reference() for _ in range(self.validation_tests)]
+            fr.val_draws = given['val_draws'] if inputs is not None else [self.env.draw_reference() for _ in range(self.validation_tests)]
             plan = getattr(self.evolver, 'last_plan', None)
             if plan is not None and self.speculative_validations > 0:
                 for j, (o, c) in enumerate(list(zip(plan.elitist_index, plan.new_elitists))[:self.speculative_validations]):
@@ -467,10 +481,11 @@ class Agent:
             # leave one SM per flight that can be in the air next to the rollout: exploration, RL validation, the previous
             # generation's champion validation, speculative validations
             fr.sm_limit = -(3 + len(fr.spec) // 2)
+            fr.draws = given['pop_draws'] if inputs is not None else self._draw_population()
             if self.defer_population:
-                fr.pop_draws = self._draw_population()
+                fr.pop_draws = fr.draws
             else:
-                fr.pop = self._launch_population(sm_limit=fr.sm_limit)
+                fr.pop = self._launch_population(sm_limit=fr.sm_limit, draws=fr.draws)
         return fr
 
     def take_front(self):
@@ -616,6 +631,16 @@ class Agent:
         f.event = torch.cuda.Event()
         f.event.record()
         return self._collect(agent, f, want_history=True)[0]
+
+    def save_checkpoint(self, path, extra=None) -> None:
+        """write everything the next train() reads to `path` (serl_b200/checkpoint.py); `extra`: plain values kept with it"""
+        from .. import checkpoint
+        checkpoint.save(self, path, extra=extra)
+
+    def load_checkpoint(self, path):
+        """continue the run saved at `path` (this Agent must be built from the same Parameters and env); returns its `extra`"""
+        from .. import checkpoint
+        return checkpoint.load(self, path)
 
     def save_agent(self, parameters, elite_index: int = None) -> None:
         """agent.py:317-352: evo_nets.pkl ({'actor_i': state_dict}), elite_net.pkl, rl_net.pkl, state histories."""

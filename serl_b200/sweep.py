@@ -212,6 +212,38 @@ class Sweep:
                 out[i] = part
         return out
 
+    def save_checkpoint(self, folder):
+        """checkpoint every run between two train() calls: run i's Agent, generator states and last statistics go to
+        folder/run<i>.pt (serl_b200/checkpoint.py), and folder/manifest.json names the run count and each run's identifying
+        Parameters.  A finished run is saved as it stands and stays finished."""
+        from . import checkpoint
+        os.makedirs(folder, exist_ok=True)
+        for i, r in enumerate(self.runs):
+            checkpoint.save(r.agent, os.path.join(folder, 'run%d.pt' % i), rng=r.rng, extra={'stats': r.stats})
+        manifest = {'format': checkpoint.FORMAT, 'version': checkpoint.VERSION, 'runs': len(self.runs),
+                    'params': [checkpoint.identity(r.params) for r in self.runs]}
+        checkpoint.write(manifest, os.path.join(folder, 'manifest.json'), json_doc=True)
+
+    def load_checkpoint(self, folder):
+        """continue the sweep saved in `folder` in this Sweep, built from the same runs (Parameters and envs, in the same
+        order; `frames` may differ).  Every run is checked before any is written.  The runs' queued fronts are re-launched
+        and their populations launched in their launch groups, as the saved sweep's last train() left them."""
+        from . import checkpoint
+        manifest = checkpoint.read_json(os.path.join(folder, 'manifest.json'))
+        if manifest.get('runs') != len(self.runs):
+            raise ValueError('Sweep.load_checkpoint: %s holds %s runs, this sweep has %d' % (folder, manifest.get('runs'), len(self.runs)))
+        cks = []
+        for i, r in enumerate(self.runs):
+            ck = checkpoint.read(os.path.join(folder, 'run%d.pt' % i))
+            try:
+                checkpoint.check(ck, r.params)
+            except ValueError as e:
+                raise ValueError('Sweep.load_checkpoint: run %d: %s' % (i, e)) from None
+            cks.append(ck)
+        for r, ck in zip(self.runs, cks):
+            r.stats = checkpoint.apply(r.agent, ck, rng=r.rng)['stats']
+        self._launch_populations([(r, r.agent._prefetched) for r in self.runs])
+
     def save_agent(self, folder=None):
         """Agent.save_agent of every run into its own folder <folder or the run's save_foldername>/run<i>"""
         for i, r in enumerate(self.runs):
