@@ -2,10 +2,13 @@
 `Parameters` attributes whose Cartesian product makes the runs.  Every run's RL half shares one grouped K7 launch per
 generation (serl_b200/sweep.py), and every run computes exactly what it computes when trained alone.  The runs may differ
 in actor shape (hidden_size, num_layers, activation_actor): narrow and wide learners share the K7 launch, and each
-shape's population flies in a launch of its own.
+shape's population flies in a launch of its own.  Runs with prioritized experience replay (-per, or per in the grid) share
+the K7 launch with uniform ones, each sampling its own priority tree.
 
     python examples/sweep.py -frames 20000 -pop_size 10 -seeds 7 8 9 -grid lr=0.0002,0.0004 noise_sd=0.2,0.3
     python examples/sweep.py -frames 20000 -pop_size 10 -grid hidden_size=72,96 activation_actor=tanh,relu
+    python examples/sweep.py -frames 20000 -pop_size 10 -seeds 7 8 9 -per                   # every run prioritized
+    python examples/sweep.py -frames 20000 -pop_size 10 -seeds 7 8 9 -grid per=0,1          # PER against uniform replay
     python examples/sweep.py -frames 20000 -pop_size 10 -seeds 7 8 9 -checkpoint_every 5     # ./tmp/checkpoint/ every 5
     python examples/sweep.py -frames 40000 -pop_size 10 -seeds 7 8 9 -resume tmp/checkpoint    # continued to 40000 frames
 """
@@ -69,7 +72,7 @@ def make_runs(cla):
 if __name__ == '__main__':
     cla = parser.parse_args()
     runs = make_runs(cla)
-    sweep = Sweep([(p, env) for _, p, env in runs], mixed_shapes=True)
+    sweep = Sweep([(p, env) for _, p, env in runs], mixed_shapes=True, per=True)
     if cla.resume:
         sweep.load_checkpoint(cla.resume)
     print('Sweep of %d runs on' % len(runs), runs[0][1].env_name)

@@ -4,7 +4,8 @@ fails loudly when CUDA is unavailable.  tests/test_capi.py holds the signatures 
 tests/test_td3_oracle.py those of include/serl_td3.h (TD3_SIGNATURES, TD3Desc, TD3_*), tests/test_deep_actor.py those of
 include/serl_route.h (ROUTE_SIGNATURES), tests/test_td3_group.py those of include/serl_td3_group.h (TD3_GROUP_SIGNATURES,
 TD3_MAX_GROUP), tests/test_td3_mixed.py those of include/serl_td3_mixed.h (TD3_MIXED_SIGNATURES), tests/test_td3_per.py those of
-include/serl_td3_per.h (PER_SIGNATURES, TD3PerDesc, PER_MAX_CAPACITY)."""
+include/serl_td3_per.h (PER_SIGNATURES, TD3PerDesc, PER_MAX_CAPACITY), tests/test_td3_group_per.py those of
+include/serl_td3_group_per.h (TD3_GROUP_PER_SIGNATURES)."""
 import ctypes
 import os
 
@@ -132,6 +133,10 @@ PER_SIGNATURES = {
     'serl_per_sample': (_int, [_vp, _i32, _i32, _i32, ctypes.c_uint64, _i64, _f64, _vp, _vp, _vp]),
     'serl_td3_train_per': (_int, [ctypes.POINTER(TD3Desc), ctypes.POINTER(TD3PerDesc), _vp]),
 }
+# include/serl_td3_group_per.h: n descriptors, each with prioritized (a tree) or uniform replay, trained in one launch
+TD3_GROUP_PER_SIGNATURES = {
+    'serl_td3_train_group_per': (_int, [ctypes.POINTER(TD3Desc), ctypes.POINTER(TD3PerDesc), _i32, _vp]),
+}
 # include/serl_route.h: the kernel of a uniform actor (host only, no stream)
 ROUTE_SIGNATURES = {
     'serl_actor_tc_widths': (_i32, [_shape, _vp, _i32]),
@@ -151,7 +156,7 @@ def lib():
                               '(there is no CPU fallback)' % LIB_PATH)
         L = ctypes.CDLL(LIB_PATH)
         for name, (restype, argtypes) in {**SIGNATURES, **TD3_SIGNATURES, **TD3_GROUP_SIGNATURES, **TD3_MIXED_SIGNATURES,
-                                         **PER_SIGNATURES, **ROUTE_SIGNATURES}.items():
+                                         **PER_SIGNATURES, **TD3_GROUP_PER_SIGNATURES, **ROUTE_SIGNATURES}.items():
             f = getattr(L, name)
             f.restype, f.argtypes = restype, argtypes
         _lib = L

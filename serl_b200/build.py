@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libserl_b200.so')
-SOURCES = ['common.cu', 'rollout.cu', 'rollout_tc.cu', 'smoothness.cu', 'evo.cu', 'evo_plan.cpp', 'td3.cu', 'per.cu']
+SOURCES = ['common.cu', 'rollout.cu', 'rollout_tc.cu', 'smoothness.cu', 'evo.cu', 'evo_plan.cpp', 'td3.cu', 'td3_group_per.cu', 'per.cu']
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '-Xptxas', '-v']
 

@@ -6,7 +6,9 @@ generation (population rollout, SSNE epoch, exploration episode: Agent.train_hea
 every run's gradient steps on its own cluster (td3_fused.train_group), then every run's tail (validation, actor injection,
 next front: Agent.train_tail).  The runs may differ in seed and in any `Parameters` attribute that keeps the actor's shape;
 with `mixed_shapes` they may differ in actor shape too (hidden_size, num_layers, activation_actor, anywhere K7 trains):
-the K7 launch then trains narrow and wide actors together (serl_td3_train_mixed).
+the K7 launch then trains narrow and wide actors together (serl_td3_train_mixed).  With `per` the runs may set `per`
+(prioritized experience replay): the K7 launch then trains every run with a priority tree on it and every other run
+uniformly, of any shapes, together (serl_td3_train_group_per).
 
 A SERL10 population (10 actors x 3 envs) fills a few warps for the serial latency of one 2001-step trajectory, so the
 populations fly together too: every run draws its front's references at their usual place (its np.random stream advances
@@ -98,9 +100,10 @@ def _shape(p):
 
 
 class Sweep:
-    def __init__(self, runs, mixed_shapes=False):
+    def __init__(self, runs, mixed_shapes=False, per=False):
         """runs: a list of (Parameters, env), each seeded and built as base/train.py:88-94 builds one run.  mixed_shapes: the
-        runs' actor shapes may differ (each inside K7's domain); without it they must agree."""
+        runs' actor shapes may differ (each inside K7's domain); without it they must agree.  per: runs may set `per`
+        (prioritized replay) and train beside uniform ones; without it a `per` run is refused."""
         runs = list(runs)
         if not runs:
             raise ValueError('Sweep: no runs')
@@ -111,9 +114,9 @@ class Sweep:
                 raise ValueError('Sweep: run %d flies incremental control (state_dim 10), which fused_td3 (K7) does not train' % i)
             if (p.state_dim, p.action_dim) == (SYMMETRIC_STATE_DIM, SYMMETRIC_ACTION_DIM):
                 raise ValueError('Sweep: run %d flies symmetric control (state_dim 2, action_dim 1), which fused_td3 (K7) does not train' % i)
-            if getattr(p, 'per', False):
+            if getattr(p, 'per', False) and not per:
                 raise ValueError('Sweep: run %d sets per (prioritized experience replay), which the grouped K7 launch does not '
-                                 'train; train it alone with Agent' % i)
+                                 'train; build the Sweep with per=True, or train it alone with Agent' % i)
             if not getattr(p, 'fused_td3', False):
                 raise ValueError('Sweep: run %d does not set fused_td3 (the sweep trains every RL half in one K7 launch)' % i)
             if mixed_shapes:
@@ -125,6 +128,7 @@ class Sweep:
                 raise ValueError('Sweep: run %d has actor shape %s, run 0 has %s (one K7 launch trains one shape)'
                                  % (i, _shape(p), _shape(runs[0][0])))
         self.mixed_shapes = bool(mixed_shapes)
+        self.per = bool(per)
         self._streams = []             # the population launch groups' streams after the first, created once and kept
         self.runs = []
         outer = RNGState.capture()
@@ -163,9 +167,12 @@ class Sweep:
             with rng_scope(r.rng):
                 plans.append(r.agent.plan_rl_fused(r.agent.gen_frames))
         group = [(r, n) for r, n in zip(live, plans) if n]
+        # the heads appended their rows (and, with per, inserted them into the runs' trees) on the current stream, after
+        # joining the population streams: the K7 launch, queued on it too, sees every run's rows and tree
         launches = td3_fused.train_group([r.agent.rl_agent for r, _ in group], [r.agent.replay_buffer for r, _ in group],
                                          [n for _, n in group], [r.agent.rl_iteration + 1 for r, _ in group],
-                                         [r.agent.args.use_champion_target for r, _ in group], mixed_shapes=self.mixed_shapes)
+                                         [r.agent.args.use_champion_target for r, _ in group], mixed_shapes=self.mixed_shapes,
+                                         prioritized=self.per)
         losses = dict(zip((id(r) for r, _ in group), td3_fused.group_losses(launches)))
         for r, n in zip(live, plans):
             with rng_scope(r.rng):

@@ -173,13 +173,16 @@ def _rows(replay):
     return (replay.data, len(replay)) if hasattr(replay, 'data') else (replay, replay.shape[0])
 
 
-def train_group(learners, replays, ns, firsts, champion_targets, record=False, mixed_shapes=False):
+def train_group(learners, replays, ns, firsts, champion_targets, record=False, mixed_shapes=False, prioritized=False):
     """learner g takes ns[g] gradient steps on global iterations firsts[g].. sampling from replays[g] (as
     learners[g].train_steps would), all learners in the same K7 launches (serl_td3_train_group): one cluster per learner,
     lockstep chunks of LAUNCH_STEPS steps, at most TD3_MAX_GROUP learners per launch.  The learners must share cluster
     size, and actor shape unless `mixed_shapes` (serl_td3_train_mixed: narrow and wide actors of any shape K7 trains, in
-    the same launches); each gets exactly the bits its solo run gives.  Returns one TD3Launch per learner; their losses
-    are views into one device buffer, so `group_losses` reads them back in one copy."""
+    the same launches); each gets exactly the bits its solo run gives.  `prioritized`: a learner whose replay is a
+    DevicePrioritizedReplayMemory trains with prioritized replay on its tree, the others uniformly, all of any shapes in the
+    same launches (serl_td3_train_group_per); with `record` the prioritized learners' launches also carry the weights and
+    TD errors.  Returns one TD3Launch per learner; their losses are views into one device buffer, so `group_losses` reads
+    them back in one copy."""
     G = len(learners)
     assert G == len(replays) == len(ns) == len(firsts) == len(champion_targets)
     assert len(set(id(f) for f in learners)) == G, 'a learner appears twice in the group'
@@ -192,9 +195,11 @@ def train_group(learners, replays, ns, firsts, champion_targets, record=False, m
     for (t, nv) in rows:
         assert t.is_cuda and t.dtype == torch.float32 and t.dim() == 2 and t.shape[1] >= TRANSITION_COLS
         assert t.stride(1) == 1 and t.shape[0] >= nv
+    pers = [r if prioritized and isinstance(r, replay_memory.DevicePrioritizedReplayMemory) else None for r in replays]
     flat = torch.empty(2 * sum(ns), dtype=torch.float32, device=dev)
     offs = np.concatenate([[0], np.cumsum(ns)]) * 2
-    out = [f._launch(n, record, flat[offs[g]:offs[g + 1]].view(n, 2)) for g, (f, n) in enumerate(zip(learners, ns))]
+    out = [f._launch(n, record, flat[offs[g]:offs[g + 1]].view(n, 2), per=pers[g] is not None)
+           for g, (f, n) in enumerate(zip(learners, ns))]
     k0 = 0
     while k0 < max(ns):
         live = [g for g in range(G) if ns[g] > k0]
@@ -204,7 +209,14 @@ def train_group(learners, replays, ns, firsts, champion_targets, record=False, m
             for j, g in enumerate(part):
                 m = min(LAUNCH_STEPS, ns[g] - k0)
                 descs[j] = learners[g]._desc(rows[g][0], rows[g][1], m, firsts[g] + k0, champion_targets[g], None, out[g], k0)
-            _native.call('serl_td3_train_mixed' if mixed_shapes else 'serl_td3_train_group', descs, len(part), device=dev)
+            if prioritized:
+                per_descs = (_native.TD3PerDesc * len(part))()          # zeroed: a null d_tree samples uniformly
+                for j, g in enumerate(part):
+                    if pers[g] is not None:
+                        per_descs[j] = FusedTD3._per_desc(pers[g], rows[g][1], out[g], k0)
+                _native.call('serl_td3_train_group_per', descs, per_descs, len(part), device=dev)
+            else:
+                _native.call('serl_td3_train_mixed' if mixed_shapes else 'serl_td3_train_group', descs, len(part), device=dev)
             for g in part:
                 learners[g]._advance(firsts[g] + k0, min(LAUNCH_STEPS, ns[g] - k0))
         k0 += LAUNCH_STEPS
