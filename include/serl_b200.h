@@ -286,10 +286,10 @@ const char* serl_last_error(void);
 }
 #endif
 
-/* K7, the fused TD3 learner (serl_td3_train, serl_td3_state_floats; serl_td3_train_group through serl_td3_group.h) */
+/* K7, the fused TD3 learner (serl_td3_learn, serl_td3_state_floats) */
 #include "serl_td3.h"
+/* prioritized replay's priority tree (serl_per_*) */
+#include "serl_td3_per.h"
 /* the kernel of a uniform actor: K1, or K1-TC with the widths [h] * (L + 1) (serl_actor_tc_widths) */
 #include "serl_route.h"
-/* K7 for learners of different actor shapes in one launch (serl_td3_train_mixed) */
-#include "serl_td3_mixed.h"
 #endif

@@ -32,7 +32,7 @@ extern "C" {
  * beta, W, b (5185 floats per head).  The critic uses the actor's activation. */
 int64_t serl_td3_state_floats(const serl_actor_shape* shape);
 
-/* One launch = n_steps consecutive TD3.update_parameters calls on global iterations first_iteration, first_iteration + 1, ...
+/* One learner: n_steps consecutive TD3.update_parameters calls on global iterations first_iteration, first_iteration + 1, ...
  *   d_replay     [>= n_valid, replay_cols] fp32 transition rows (obs 7 | action 3 | next_obs 7 | reward | done, the first
  *                19 columns; replay_cols >= 19 is the row stride); every step samples `batch` distinct rows of [0, n_valid)
  *   critic_adam_steps / actor_adam_steps   Adam step counts before the launch (bias corrections continue from there)
@@ -70,12 +70,45 @@ typedef struct {
     int32_t* d_rec_indices; float* d_rec_noise; float* d_rec_caps;
     int32_t* d_status;
 } serl_td3_desc;
-int serl_td3_train(const serl_td3_desc* desc, void* stream);
+/* the largest launch: the learners' launch arguments travel as the kernel parameter, which sm_90 caps at 32,764 bytes */
+#define SERL_TD3_MAX_GROUP 64
+
+/* What prioritized replay (PER) adds to a learner: every step draws its `batch` rows from the priority tree d_tree
+ * (include/serl_td3_per.h) as serl_per_sample does (rows given in the serl_td3_desc's d_indices replace the draw and are
+ * weighted by their leaves), with beta = min(1, beta0 + k (1 - beta0) / beta_frames) at the learner's k-th sample (k = its
+ * critic Adam step count after the step).  The critic loss is mean(w (q1 - y)^2) + mean(w (q2 - y)^2) (the td loss
+ * reported); the actor loss is unweighted.  After the critic's forward pass, row j of the batch gets priority
+ * (delta_j + 1e-5)^alpha with delta_j = (|q1 - y| + |q2 - y|) / 2 of the critic before its update (batch order, the later
+ * of two equal rows kept), so the next step samples from the updated tree.  The result is bitwise the same for every
+ * cluster size and launch split.
+ *   n_valid      rows stored in the tree; must equal the serl_td3_desc's n_valid, <= capacity
+ *   d_rec_weights / d_rec_td   optional records [n_steps, batch] fp32 of the weights and of delta
+ * A learner with a tree is refused when capacity is outside 1..SERL_PER_MAX_CAPACITY, n_valid differs from the desc's or
+ * exceeds capacity, alpha is not in (0, 1], beta0 not in [0, 1] or beta_frames not > 0. */
+typedef struct {
+    double* d_tree; int32_t capacity; int32_t n_valid;
+    double alpha; double beta0; double beta_frames;
+    float* d_rec_weights; float* d_rec_td;
+} serl_td3_per_desc;
+
+/* descs[0 .. n) trained in ONE launch, one cluster of cluster_size CTAs per learner with steps: learner g takes its
+ * n_steps, and gets exactly the bits its launch alone (n = 1) gives, whatever else is in the launch, in any order.  Shapes
+ * may differ anywhere in K7's domain; all learners share `cluster_size` (0 and 8 are the same size).
+ *   pers         NULL: every learner samples uniformly.  Otherwise pers[g].d_tree NULL: learner g samples uniformly and
+ *                the other fields of pers[g] are not read; a tree: learner g trains with prioritized replay on it.
+ * Learners never wait for each other: one with fewer steps finishes early, one with n_steps = 0 gets no cluster, a call
+ * in which no learner has steps makes no launch, and more learners than the GPU holds at once run in waves.  Each
+ * learner's state, losses, records, tree and status word are its own (they must not overlap another learner's); its
+ * status word receives only its own bits.
+ * The kernel follows from the learners with steps: one runs the solo kernel (uniform or PER, narrow or wide), several
+ * uniform ones of one width class (hidden <= 128, or above) the group kernel of that class, several uniform ones of both
+ * classes the mixed kernel, and several with at least one prioritized the group PER kernel.
+ * SERL_ERR_ARG before any CUDA call when descs is NULL, n is outside 1..SERL_TD3_MAX_GROUP, or a learner fails a check
+ * above or differs from learner 0 in cluster_size; a learner's failure reads "serl_td3_learn: learner i: ..." in
+ * serl_last_error. */
+int serl_td3_learn(const serl_td3_desc* descs, const serl_td3_per_desc* pers, int n, void* stream);
 
 #ifdef __cplusplus
 }
 #endif
-
-/* several learners in one launch (serl_td3_train_group) */
-#include "serl_td3_group.h"
 #endif

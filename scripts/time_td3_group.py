@@ -1,4 +1,4 @@
-"""Time K7's group launch (serl_td3_train_group) and the sweep driver.
+"""Time K7's group launch (serl_td3_learn with one learner per run) and the sweep driver.
 
 (a) G learners at h = 72, L = 3, batch 86, CAPS on, on a replay of 800,000 K1 flight rows, cluster size 8 (and G = 32 at
     cluster size 4), three arms alternated twice: ONE grouped launch of G clusters, G solo launches in sequence (the only

@@ -1,9 +1,9 @@
-"""Time K7's group launch of prioritized learners (serl_td3_train_group_per) against what it replaces and against uniform
+"""Time K7's group launch of prioritized learners (serl_td3_learn) against what it replaces and against uniform
 replay in a group.  h = 72, L = 3, batch 86, CAPS on, cluster size 8, 800,000 replay rows from K1 flights in every tree,
 the trees' priorities made uneven by 5,000 PER steps before the timing (each learner gets its own copy of that tree).
 
-(a) S prioritized learners in ONE serl_td3_train_group_per launch, against S solo serl_td3_train_per launches back to back.
-(b) The same S learners uniform in ONE serl_td3_train_group launch, against prioritized in the new launch.
+(a) S prioritized learners in ONE serl_td3_learn launch, against S solo prioritized launches back to back.
+(b) The same S learners uniform in ONE serl_td3_learn launch, against prioritized in one launch.
     For S = 1, 4, 16, 64: the three arms alternate three times over `--steps` steps each (CUDA events after warm-up);
     us per step of the group (every learner takes one step).
 (c) Two Sweeps of S SERL10-sized runs (pop 10, 3 envs, h = 72, fused_td3), one with every run prioritized (Sweep(...,

@@ -1,4 +1,4 @@
-"""Time K7's mixed-shape group launch (serl_td3_train_mixed) and a mixed-shape sweep.
+"""Time K7's mixed-shape group launch (serl_td3_learn with learners of different shapes) and a mixed-shape sweep.
 
 (a) Eight learners at batch 86, CAPS on, on a replay of 800,000 K1 flight rows, cluster size 8: the shapes (72, 3, tanh),
     (96, 3, relu), (32, 3, tanh) and (256, 3, tanh), two of each.  Three arms, alternated: ONE mixed launch, one uniform

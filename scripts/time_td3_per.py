@@ -1,4 +1,4 @@
-"""Time K7 with prioritized replay (serl_td3_train_per) against K7's uniform sampler (serl_td3_train): h = 72, L = 3,
+"""Time K7 with prioritized replay (serl_td3_learn with a tree) against K7's uniform sampler (serl_td3_learn without): h = 72, L = 3,
 batch 86, CAPS on, 800,000 replay rows from K1 flights, the tree's priorities made uneven by PER steps before the timing.
 Per cluster size, the two alternate three times over `--steps` steps each (CUDA events after warm-up).  Also times the
 insert of one SERL10 generation's rows into the tree (serl_per_insert: the max reduction and the rebuild).  Prints one

@@ -1,11 +1,9 @@
 """ctypes binding of the C-ABI library (include/serl_b200.h): the only module that binds it.  The product path has no CPU
 fallback: importing succeeds without a GPU (so host logic is testable), but the library must exist and every compute call
 fails loudly when CUDA is unavailable.  tests/test_capi.py holds the signatures and constants below to the header,
-tests/test_td3_oracle.py those of include/serl_td3.h (TD3_SIGNATURES, TD3Desc, TD3_*), tests/test_deep_actor.py those of
-include/serl_route.h (ROUTE_SIGNATURES), tests/test_td3_group.py those of include/serl_td3_group.h (TD3_GROUP_SIGNATURES,
-TD3_MAX_GROUP), tests/test_td3_mixed.py those of include/serl_td3_mixed.h (TD3_MIXED_SIGNATURES), tests/test_td3_per.py those of
-include/serl_td3_per.h (PER_SIGNATURES, TD3PerDesc, PER_MAX_CAPACITY), tests/test_td3_group_per.py those of
-include/serl_td3_group_per.h (TD3_GROUP_PER_SIGNATURES)."""
+tests/test_td3_oracle.py those of include/serl_td3.h (TD3_SIGNATURES, TD3Desc, TD3_*), tests/test_td3_wide.py its wide
+bounds, tests/test_td3_per.py those of include/serl_td3_per.h (PER_SIGNATURES, TD3PerDesc, PER_MAX_CAPACITY),
+tests/test_deep_actor.py those of include/serl_route.h (ROUTE_SIGNATURES)."""
 import ctypes
 import os
 
@@ -38,9 +36,8 @@ TD3_MAX_HIDDEN = 320
 TD3_MAX_WIDE_LAYERS = 8
 TD3_CHAMPION_TARGET = 1
 TD3_STATUS_INDEX = 4
-# include/serl_td3_group.h (K7 for a group of learners in one launch)
 TD3_MAX_GROUP = 64
-# include/serl_td3_per.h (prioritized replay: the priority tree and K7 with it)
+# include/serl_td3_per.h (prioritized replay's priority tree)
 PER_MAX_CAPACITY = 1 << 30
 
 
@@ -79,7 +76,7 @@ class TD3Desc(ctypes.Structure):
 
 
 class TD3PerDesc(ctypes.Structure):
-    """serl_td3_per_desc (include/serl_td3_per.h)"""
+    """serl_td3_per_desc (include/serl_td3.h)"""
     _fields_ = [('d_tree', ctypes.c_void_p), ('capacity', ctypes.c_int32), ('n_valid', ctypes.c_int32),
                 ('alpha', ctypes.c_double), ('beta0', ctypes.c_double), ('beta_frames', ctypes.c_double),
                 ('d_rec_weights', ctypes.c_void_p), ('d_rec_td', ctypes.c_void_p)]
@@ -114,28 +111,15 @@ SIGNATURES = {
 # the entry points of include/serl_td3.h (included by serl_b200.h), bound the same way
 TD3_SIGNATURES = {
     'serl_td3_state_floats': (_i64, [_shape]),
-    'serl_td3_train': (_int, [ctypes.POINTER(TD3Desc), _vp]),
+    'serl_td3_learn': (_int, [ctypes.POINTER(TD3Desc), ctypes.POINTER(TD3PerDesc), _i32, _vp]),
 }
-# include/serl_td3_group.h: n descriptors trained in one launch
-TD3_GROUP_SIGNATURES = {
-    'serl_td3_train_group': (_int, [ctypes.POINTER(TD3Desc), _i32, _vp]),
-}
-# include/serl_td3_mixed.h: n descriptors of any actor shapes trained in one launch
-TD3_MIXED_SIGNATURES = {
-    'serl_td3_train_mixed': (_int, [ctypes.POINTER(TD3Desc), _i32, _vp]),
-}
-# include/serl_td3_per.h: the priority tree's entry points and K7 with prioritized replay
+# include/serl_td3_per.h: the priority tree's entry points
 PER_SIGNATURES = {
     'serl_per_tree_doubles': (_i64, [_i32]),
     'serl_per_rebuild': (_int, [_vp, _i32, _vp]),
     'serl_per_insert': (_int, [_vp, _i32, _i32, _i32, _i32, _vp]),
     'serl_per_update': (_int, [_vp, _i32, _vp, _vp, _i32, _f64, _vp]),
     'serl_per_sample': (_int, [_vp, _i32, _i32, _i32, ctypes.c_uint64, _i64, _f64, _vp, _vp, _vp]),
-    'serl_td3_train_per': (_int, [ctypes.POINTER(TD3Desc), ctypes.POINTER(TD3PerDesc), _vp]),
-}
-# include/serl_td3_group_per.h: n descriptors, each with prioritized (a tree) or uniform replay, trained in one launch
-TD3_GROUP_PER_SIGNATURES = {
-    'serl_td3_train_group_per': (_int, [ctypes.POINTER(TD3Desc), ctypes.POINTER(TD3PerDesc), _i32, _vp]),
 }
 # include/serl_route.h: the kernel of a uniform actor (host only, no stream)
 ROUTE_SIGNATURES = {
@@ -155,8 +139,7 @@ def lib():
             raise NativeError('serl_b200: %s is missing — build it with `python -m serl_b200.build` '
                               '(there is no CPU fallback)' % LIB_PATH)
         L = ctypes.CDLL(LIB_PATH)
-        for name, (restype, argtypes) in {**SIGNATURES, **TD3_SIGNATURES, **TD3_GROUP_SIGNATURES, **TD3_MIXED_SIGNATURES,
-                                         **PER_SIGNATURES, **TD3_GROUP_PER_SIGNATURES, **ROUTE_SIGNATURES}.items():
+        for name, (restype, argtypes) in {**SIGNATURES, **TD3_SIGNATURES, **PER_SIGNATURES, **ROUTE_SIGNATURES}.items():
             f = getattr(L, name)
             f.restype, f.argtypes = restype, argtypes
         _lib = L

@@ -1,7 +1,8 @@
 // K7's learner (csrc/td3.cu): one TD3 learner's n_steps on one thread-block cluster (td3_learner), its launch arguments,
-// scratch layout and the host-side checks of its descriptors.  td3.cu instantiates it in the solo, group, mixed and PER
-// kernels; td3_group_per.cu in the group launch of prioritized and uniform learners.  The kernels of each translation unit
-// are compiled from this one source, so a learner's code (and its bits) is the same in every launch that runs it.
+// scratch layout, the host-side checks of its descriptors and the packing of a serl_td3_learn call's learners for one
+// launch.  td3.cu instantiates it in the solo, group, mixed and PER kernels; td3_group_per.cu in the group launch of
+// prioritized and uniform learners.  The kernels of each translation unit are compiled from this one source, so a
+// learner's code (and its bits) is the same in every launch that runs it.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -37,7 +38,7 @@ struct Args {
     float* ws;
 };
 
-// what a PER launch adds (serl_td3_train_per): the priority tree and its parameters, the optional records
+// what prioritized replay adds (serl_td3_per_desc): the priority tree and its parameters, the optional records
 struct Per {
     double* tree; int leaves, n_valid;
     double alpha, beta0, beta_frames;
@@ -780,7 +781,7 @@ bool shape_ok(const serl_actor_shape* s)
            s->num_layers >= 1 && s->activation >= SERL_ACT_TANH && s->activation <= SERL_ACT_LEAKY_RELU;
 }
 
-// why a descriptor cannot be trained (nullptr: it can); the checks of serl_td3_train, made before any CUDA call
+// why a descriptor cannot be trained (nullptr: it can); checked before any CUDA call
 const char* desc_error(const serl_td3_desc* d)
 {
     if (!shape_ok(&d->shape))
@@ -829,4 +830,35 @@ const char* per_error(const serl_td3_desc* d, const serl_td3_per_desc* p)
     return nullptr;
 }
 
+// The learners with steps of a checked serl_td3_learn call, in order, packed for one launch: a[m] and p[m] (p[m].tree null
+// for a uniform learner), each with its own slice of one scratch buffer.  Slices are aligned to 128 bytes, and a
+// prioritized learner's slice holds its batch's B weights after the layout.  Returns the number of learners packed, or a
+// negative serl_status when the scratch cannot be had.
+int pack(const serl_td3_desc* descs, const serl_td3_per_desc* pers, int n, cudaStream_t s, Args* a, Per* p)
+{
+    int m = 0;
+    size_t total = 0;
+    size_t off[SERL_TD3_MAX_GROUP];
+    for (int i = 0; i < n; ++i) {
+        if (descs[i].n_steps == 0) continue;
+        a[m] = make_args(descs + i);
+        const serl_td3_per_desc* q = pers && pers[i].d_tree ? pers + i : nullptr;
+        p[m] = q ? Per{q->d_tree, per_leaves(q->capacity), q->n_valid, q->alpha, q->beta0, q->beta_frames, q->d_rec_weights, q->d_rec_td}
+                 : Per{};
+        off[m] = total;
+        total += (scratch_floats(a[m]) + (q ? a[m].B : 0) + 31) / 32 * 32;
+        ++m;
+    }
+    if (m == 0) return 0;
+    void* ws = nullptr;
+    const cudaError_t e = serl_scratch(SERL_SCRATCH_TD3, s, total * sizeof(float), &ws);
+    if (e != cudaSuccess) return serl_fail_cuda(e, "td3 scratch");
+    for (int g = 0; g < m; ++g) a[g].ws = (float*)ws + off[g];
+    return m;
+}
+
 }  // namespace
+
+// td3_group_per_kernel<CS> (td3_group_per.cu) on the learners with steps of a checked serl_td3_learn call
+template <int CS>
+int launch_group_per(const serl_td3_desc* descs, const serl_td3_per_desc* pers, int n, cudaStream_t s);

@@ -6,9 +6,9 @@ generation (population rollout, SSNE epoch, exploration episode: Agent.train_hea
 every run's gradient steps on its own cluster (td3_fused.train_group), then every run's tail (validation, actor injection,
 next front: Agent.train_tail).  The runs may differ in seed and in any `Parameters` attribute that keeps the actor's shape;
 with `mixed_shapes` they may differ in actor shape too (hidden_size, num_layers, activation_actor, anywhere K7 trains):
-the K7 launch then trains narrow and wide actors together (serl_td3_train_mixed).  With `per` the runs may set `per`
+the K7 launch then trains narrow and wide actors together.  With `per` the runs may set `per`
 (prioritized experience replay): the K7 launch then trains every run with a priority tree on it and every other run
-uniformly, of any shapes, together (serl_td3_train_group_per).
+uniformly, of any shapes, together.
 
 A SERL10 population (10 actors x 3 envs) fills a few warps for the serial latency of one 2001-step trajectory, so the
 populations fly together too: every run draws its front's references at their usual place (its np.random stream advances

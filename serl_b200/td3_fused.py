@@ -27,9 +27,9 @@ class TD3Launch:
     def check(self):
         st = int(self.status.item())
         if st & _native.STATUS_NONFINITE:
-            raise _native.NativeError('serl_td3_train: a loss became NaN or infinite')
+            raise _native.NativeError('serl_td3_learn: a loss became NaN or infinite')
         if st & _native.TD3_STATUS_INDEX:
-            raise _native.NativeError('serl_td3_train: a given row index was outside the replay rows')
+            raise _native.NativeError('serl_td3_learn: a given row index was outside the replay rows')
 
 
 def state_floats(shape):
@@ -67,26 +67,14 @@ class FusedTD3(td3.TD3):
     def run(self, rows, n_valid, n, first_iteration, champion_target=False, indices=None, record=False, cluster_size=None, per=None):
         """n consecutive gradient steps on global iterations first_iteration.. (launches of at most LAUNCH_STEPS) on the replay
         rows [>= n_valid, >= 19] fp32 (device, row-contiguous).  indices [n, B] int32 replaces the sampler's draw.  per: the
-        DevicePrioritizedReplayMemory whose rows these are — prioritized replay (serl_td3_train_per) on its tree."""
+        DevicePrioritizedReplayMemory whose rows these are — prioritized replay on its tree."""
         B = int(self.args.batch_size)
-        dev = self.state.device
         assert rows.is_cuda and rows.dtype == torch.float32 and rows.dim() == 2 and rows.shape[1] >= TRANSITION_COLS
         assert rows.stride(1) == 1 and rows.shape[0] >= n_valid
         r = self._launch(n, record, per=per is not None)
         if indices is not None:
             assert indices.shape == (n, B) and indices.dtype == torch.int32 and indices.is_cuda and indices.is_contiguous()
-        k0 = 0
-        while k0 < n:
-            m = min(LAUNCH_STEPS, n - k0)
-            d = self._desc(rows, n_valid, m, int(first_iteration) + k0, champion_target, indices, r, k0, cluster_size)
-            if per is None:
-                _native.call('serl_td3_train', d, device=dev)
-            else:
-                _native.call('serl_td3_train_per', d, self._per_desc(per, n_valid, r, k0), device=dev)
-            self._advance(int(first_iteration) + k0, m)
-            k0 += m
-        if n:
-            self._bump_versions()
+        _learn([self], [(rows, n_valid)], [per], [int(n)], [int(first_iteration)], [champion_target], [r], indices, cluster_size)
         return r
 
     def _launch(self, n, record, losses=None, per=False):
@@ -105,7 +93,7 @@ class FusedTD3(td3.TD3):
         return r
 
     def _desc(self, rows, n_valid, m, first, champion_target, indices, r, k0, cluster_size=None):
-        """the TD3Desc of m steps from global iteration `first`, writing r's rows k0.. (solo and group launches alike)"""
+        """the TD3Desc of m steps from global iteration `first`, writing r's rows k0.."""
         a = self.args
         caps = self.caps_dict or {'lambda_t': 0.0, 'lambda_s': 0.0, 'eps_sd': 0.0}
         p = lambda t: t[k0:].data_ptr() if t is not None else None
@@ -175,17 +163,21 @@ def _rows(replay):
 
 def train_group(learners, replays, ns, firsts, champion_targets, record=False, mixed_shapes=False, prioritized=False):
     """learner g takes ns[g] gradient steps on global iterations firsts[g].. sampling from replays[g] (as
-    learners[g].train_steps would), all learners in the same K7 launches (serl_td3_train_group): one cluster per learner,
-    lockstep chunks of LAUNCH_STEPS steps, at most TD3_MAX_GROUP learners per launch.  The learners must share cluster
-    size, and actor shape unless `mixed_shapes` (serl_td3_train_mixed: narrow and wide actors of any shape K7 trains, in
-    the same launches); each gets exactly the bits its solo run gives.  `prioritized`: a learner whose replay is a
-    DevicePrioritizedReplayMemory trains with prioritized replay on its tree, the others uniformly, all of any shapes in the
-    same launches (serl_td3_train_group_per); with `record` the prioritized learners' launches also carry the weights and
-    TD errors.  Returns one TD3Launch per learner; their losses are views into one device buffer, so `group_losses` reads
-    them back in one copy."""
+    learners[g].train_steps would), all learners in the same K7 launches: one cluster per learner, lockstep chunks of
+    LAUNCH_STEPS steps, at most TD3_MAX_GROUP learners per launch.  The learners must share cluster size, and actor shape
+    unless `mixed_shapes` (narrow and wide actors of any shape K7 trains, in the same launches); each gets exactly the bits
+    its solo run gives.  `prioritized`: a learner whose replay is a DevicePrioritizedReplayMemory trains with prioritized
+    replay on its tree, the others uniformly, all of any shapes in the same launches; with `record` the prioritized
+    learners' launches also carry the weights and TD errors.  Returns one TD3Launch per learner; their losses are views
+    into one device buffer, so `group_losses` reads them back in one copy."""
     G = len(learners)
     assert G == len(replays) == len(ns) == len(firsts) == len(champion_targets)
     assert len(set(id(f) for f in learners)) == G, 'a learner appears twice in the group'
+    if not (mixed_shapes or prioritized):
+        for g, f in enumerate(learners):
+            if bytes(f.shape) != bytes(learners[0].shape):
+                raise _native.NativeError("train_group: learner %d: actor shape differs from learner 0's (one launch trains one "
+                                          'shape unless mixed_shapes)' % g)
     ns = [int(n) for n in ns]
     firsts = [int(f) for f in firsts]
     if not G:
@@ -200,30 +192,35 @@ def train_group(learners, replays, ns, firsts, champion_targets, record=False, m
     offs = np.concatenate([[0], np.cumsum(ns)]) * 2
     out = [f._launch(n, record, flat[offs[g]:offs[g + 1]].view(n, 2), per=pers[g] is not None)
            for g, (f, n) in enumerate(zip(learners, ns))]
+    _learn(learners, rows, pers, ns, firsts, champion_targets, out)
+    return out
+
+
+def _learn(learners, rows, pers, ns, firsts, champion_targets, out, indices=None, cluster_size=None):
+    """learner g's ns[g] steps from global iteration firsts[g] on rows[g] = (rows, n_valid), prioritized on the buffer
+    pers[g] unless it is None, writing out[g]: serl_td3_learn launches of lockstep chunks of LAUNCH_STEPS steps, at most
+    TD3_MAX_GROUP learners with steps each.  indices and cluster_size: FusedTD3.run's, for a single learner."""
+    dev = learners[0].state.device
     k0 = 0
     while k0 < max(ns):
-        live = [g for g in range(G) if ns[g] > k0]
+        live = [g for g in range(len(learners)) if ns[g] > k0]
         for c in range(0, len(live), _native.TD3_MAX_GROUP):
             part = live[c:c + _native.TD3_MAX_GROUP]
             descs = (_native.TD3Desc * len(part))()
+            per_descs = (_native.TD3PerDesc * len(part))()          # zeroed: a null d_tree samples uniformly
             for j, g in enumerate(part):
                 m = min(LAUNCH_STEPS, ns[g] - k0)
-                descs[j] = learners[g]._desc(rows[g][0], rows[g][1], m, firsts[g] + k0, champion_targets[g], None, out[g], k0)
-            if prioritized:
-                per_descs = (_native.TD3PerDesc * len(part))()          # zeroed: a null d_tree samples uniformly
-                for j, g in enumerate(part):
-                    if pers[g] is not None:
-                        per_descs[j] = FusedTD3._per_desc(pers[g], rows[g][1], out[g], k0)
-                _native.call('serl_td3_train_group_per', descs, per_descs, len(part), device=dev)
-            else:
-                _native.call('serl_td3_train_mixed' if mixed_shapes else 'serl_td3_train_group', descs, len(part), device=dev)
+                descs[j] = learners[g]._desc(rows[g][0], rows[g][1], m, firsts[g] + k0, champion_targets[g], indices, out[g], k0,
+                                             cluster_size)
+                if pers[g] is not None:
+                    per_descs[j] = FusedTD3._per_desc(pers[g], rows[g][1], out[g], k0)
+            _native.call('serl_td3_learn', descs, per_descs, len(part), device=dev)
             for g in part:
                 learners[g]._advance(firsts[g] + k0, min(LAUNCH_STEPS, ns[g] - k0))
         k0 += LAUNCH_STEPS
     for f, n in zip(learners, ns):
         if n:
             f._bump_versions()
-    return out
 
 
 def group_losses(launches):

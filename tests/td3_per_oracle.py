@@ -1,5 +1,5 @@
 """oracle/td3.update_parameters with prioritized replay's importance weights: the reference K7's PER learner
-(serl_td3_train_per) and the weighted torch path (core/td3.py) are held to.
+(serl_td3_learn with a priority tree) and the weighted torch path (core/td3.py) are held to.
 
 `update_parameters(agent, rows, iteration, noise, caps_u, champion_policy, norms, weights)` is oracle.td3.update_parameters
 with the critic loss mean(w (q1 - y)^2) + mean(w (q2 - y)^2) and returns, after (pg, td), the per-row TD error

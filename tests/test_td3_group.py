@@ -1,99 +1,28 @@
-"""K7 group launch and the sweep driver without a GPU: the binding of include/serl_td3_group.h, the argument checks
-serl_td3_train_group makes before any CUDA call, the per-run generator swap and the runs a Sweep refuses."""
-import ctypes
+"""K7 group launch and the sweep driver without a GPU: the shapes train_group refuses to group, the per-run generator swap
+and the runs a Sweep refuses."""
 import os
 import random
-import re
-import subprocess
 import types
 
 import numpy as np
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_binding_matches_the_group_header(tmp_path):
-    from serl_b200 import _native
-    text = re.sub(r'/\*.*?\*/', '', open(os.path.join(ROOT, 'include', 'serl_td3_group.h')).read(), flags=re.S)
-    protos = {n: (r.strip(), [p.strip() for p in ps.split(',')])
-              for r, n, ps in re.findall(r'([A-Za-z_][\w ]*\**)\s*\b(serl_[a-z0-9_]+)\s*\(([^)]*)\)\s*;', text)}
-    assert sorted(protos) == sorted(_native.TD3_GROUP_SIGNATURES) == ['serl_td3_train_group']
-    assert '#include "serl_td3_group.h"' in open(os.path.join(ROOT, 'include', 'serl_td3.h')).read()
-    restype, argtypes = _native.TD3_GROUP_SIGNATURES['serl_td3_train_group']
-    ret, params = protos['serl_td3_train_group']
-    assert ret == 'int' and restype is ctypes.c_int
-    assert len(params) == len(argtypes) == 3
-    assert argtypes[0]._type_ is _native.TD3Desc and argtypes[1] is ctypes.c_int32 and argtypes[2] is ctypes.c_void_p
-    src = tmp_path / 'c.c'
-    src.write_text('#include "serl_b200.h"\n'
-                   'int (*f)(const serl_td3_desc*, int, void*) = serl_td3_train_group;\n')
-    subprocess.check_call(['gcc', '-fsyntax-only', '-Wall', '-Werror', '-I', os.path.join(ROOT, 'include'), str(src)])
-    out = subprocess.check_output(['gcc', '-E', '-dM', '-I', os.path.join(ROOT, 'include'), str(src)], text=True)
-    assert '#define SERL_TD3_MAX_GROUP %d' % _native.TD3_MAX_GROUP in out
-    from serl_b200 import build
-    build.build()
-    assert hasattr(ctypes.CDLL(_native.LIB_PATH), 'serl_td3_train_group')
-
-
-def _desc(**kw):
-    from serl_b200 import _native, rollout
-    d = _native.TD3Desc()
-    d.shape = rollout.actor_shape(72)
-    d.d_state, d.d_replay, d.d_losses = 0x10000, 0x20000, 0x30000          # non-null, never read
-    d.replay_cols, d.n_valid, d.batch, d.n_steps, d.policy_update_freq = 19, 1000, 86, 10, 3
-    for k, v in kw.items():
-        setattr(d, k, v)
-    return d
-
-
-def _group(descs, n=None):
-    from serl_b200 import _native
-    arr = (_native.TD3Desc * max(len(descs), 1))(*descs)
-    rc = _native.lib().serl_td3_train_group(arr, len(descs) if n is None else n, None)
-    return rc, _native.lib().serl_last_error().decode()
-
-
-def test_group_is_rejected_before_any_cuda_call():
-    """every failure is SERL_ERR_ARG with a message; the device pointers are never dereferenced"""
-    from serl_b200 import build, _native, rollout
-    build.build()
-    ok = [_desc(seed=s) for s in range(3)]
-    rc, msg = _group(ok, 0)
-    assert rc == -1 and 'n must be' in msg
-    rc, msg = _group([_desc()] * (_native.TD3_MAX_GROUP + 1))
-    assert rc == -1 and 'n must be' in msg
-    rc = _native.lib().serl_td3_train_group(None, 2, None)
-    assert rc == -1 and 'null' in _native.lib().serl_last_error().decode()
-    rc, msg = _group(ok[:2] + [_desc(shape=rollout.actor_shape(64))])
-    assert rc == -1 and 'learner 2' in msg and 'shape' in msg
-    rc, msg = _group(ok[:1] + [_desc(shape=rollout.actor_shape(72, 2))])
-    assert rc == -1 and 'learner 1' in msg and 'shape' in msg
-    rc, msg = _group(ok[:1] + [_desc(cluster_size=4)])
-    assert rc == -1 and 'learner 1' in msg and 'cluster_size' in msg
-    # every check of serl_td3_train, per learner, naming it
-    for kw in (dict(batch=129), dict(batch=0), dict(n_valid=85), dict(replay_cols=18), dict(policy_update_freq=0),
-               dict(cluster_size=3), dict(flags=2), dict(d_state=None), dict(d_losses=None), dict(n_steps=-1),
-               dict(first_iteration=-1), dict(shape=rollout.actor_shape(48)), dict(shape=rollout.actor_shape(400, 3))):
-        rc, msg = _group(ok[:1] + [_desc(**kw)] + ok[1:])
-        assert rc == -1 and msg.startswith('serl_td3_train_group: learner 1:'), (kw, rc, msg)
-    rc, msg = _group([_desc(shape=rollout.actor_shape(100))] * 2)
-    assert rc == -1 and 'learner 0' in msg and 'shape' in msg
-    # the same shape everywhere, cluster_size 0 and 8 agreeing, and nothing to do: no launch
-    before = _native.lib().serl_launch_count()
-    assert _group([_desc(n_steps=0, cluster_size=c) for c in (0, 8, 0)])[0] == 0
-    assert _native.lib().serl_launch_count() == before
-
-
-def test_solo_entry_point_keeps_its_messages():
-    from serl_b200 import build, _native
-    build.build()
-    L = _native.lib()
-    assert L.serl_td3_train(ctypes.byref(_desc(batch=129)), None) == -1
-    assert L.serl_last_error().decode() == 'serl_td3_train: batch must be 1..128'
-    assert L.serl_td3_train(ctypes.byref(_desc(cluster_size=3)), None) == -1
-    assert L.serl_last_error().decode() == 'serl_td3_train: cluster_size must be 0, 1, 2, 4 or 8'
+def test_train_group_refuses_shapes_it_cannot_group():
+    """train_group refuses learners of different actor shapes before it reads their replays or launches, unless
+    mixed_shapes or prioritized lets one launch train them; serl_td3_learn's own refusals are in test_td3_oracle.py"""
+    from serl_b200 import _native, rollout, td3_fused
+    learner = lambda *shape: types.SimpleNamespace(shape=rollout.actor_shape(*shape), state=torch.zeros(1))
+    for bad in ((64,), (72, 2), (72, 3, 'elu')):
+        learners = [learner(72), learner(72), learner(*bad)]
+        with pytest.raises(_native.NativeError, match=r"train_group: learner 2: actor shape differs from learner 0's"):
+            td3_fused.train_group(learners, [None] * 3, [10] * 3, [1] * 3, [False] * 3)
+    learners = [learner(72), learner(256)]
+    for kw in (dict(mixed_shapes=True), dict(prioritized=True)):
+        with pytest.raises(AssertionError):          # past the shape check: the CPU rows are refused
+            td3_fused.train_group(learners, [torch.zeros(100, 19)] * 2, [10] * 2, [1] * 2, [False] * 2, **kw)
 
 
 def _draws():

@@ -1,4 +1,4 @@
-"""K7's group launch (serl_td3_train_group, td3_fused.train_group) and the sweep driver (serl_b200/sweep.py) on the GPU.
+"""K7's group launch (serl_td3_learn, td3_fused.train_group) and the sweep driver (serl_b200/sweep.py) on the GPU.
 Every comparison is bitwise against the same learners trained alone (FusedTD3.run, Agent.train) from copies of the same
 initial state: the learner state, the losses, the recorded draws (batch rows, target noise, CAPS uniforms), the status
 word and the Adam step counts."""
@@ -147,7 +147,7 @@ def test_group_split_into_chunks_and_launches_equals_one_launch(monkeypatch):
         assert_same(a, b)
 
 
-def test_bad_index_sets_the_status_of_its_own_learner_only():
+def test_bad_index_in_one_learn_call_sets_only_its_learners_status():
     from serl_b200 import _native
     specs = [dict(s, n=5) for s in SPECS[:3]]
     fs = [learner(s) for s in specs]
@@ -159,7 +159,7 @@ def test_bad_index_sets_the_status_of_its_own_learner_only():
         r = f._launch(5, False)
         rs.append(r)
         descs[j] = f._desc(rows[j], s['n_valid'], 5, s['first'], s['champ'], bad if j == 1 else None, r, 0)
-    _native.call('serl_td3_train_group', descs, 3, device=DEV)
+    _native.call('serl_td3_learn', descs, None, 3, device=DEV)
     torch.cuda.synchronize()
     assert [int(r.status.item()) for r in rs] == [0, _native.TD3_STATUS_INDEX, 0]
     with pytest.raises(_native.NativeError):

@@ -1,4 +1,4 @@
-"""K7's group launch of prioritized and uniform learners (serl_td3_train_group_per, td3_fused.train_group(prioritized=True))
+"""K7's group launch of prioritized and uniform learners (serl_td3_learn, td3_fused.train_group(prioritized=True))
 and Sweep(per=True) on the GPU.  Every comparison is bitwise against the same learners or runs trained alone
 (FusedTD3.run with and without its priority tree, Agent.train) from copies of the same initial state: the learner state,
 the losses, the recorded draws (rows, target noise, CAPS uniforms, and for prioritized learners the weights and TD errors),
@@ -44,7 +44,7 @@ def source(spec):
 
 
 def solo(specs, shapes, **kw):
-    """each learner alone: serl_td3_train_per on its tree, or serl_td3_train"""
+    """each learner alone: FusedTD3.run, on its tree or uniformly"""
     out = []
     for s, sh in zip(specs, shapes):
         f, src = learner(s, sh, **kw), source(s)
@@ -117,7 +117,7 @@ def test_per_and_uniform_narrow_and_wide_in_one_launch():
 
 
 def test_uniform_only_group_equals_solo_runs():
-    """no learner with a tree: the group takes serl_td3_train_mixed's kernels, in one launch"""
+    """no learner with a tree: the group takes the uniform learners' kernels, in one launch"""
     idx = [1, 3, 5]
     specs, shapes = [MIX[i] for i in idx], [MIX_SHAPES[i] for i in idx]
     ref = solo(specs, shapes)
@@ -169,7 +169,7 @@ def test_launch_split_equals_one_launch(monkeypatch):
         assert_same(a, b)
 
 
-def test_bad_index_sets_the_status_of_its_own_learner_only():
+def test_bad_index_in_one_learn_call_sets_only_its_learners_status():
     from serl_b200 import _native
     from serl_b200.td3_fused import FusedTD3
     specs = [dict(MIX[k], n=5) for k in (1, 0, 2)]           # uniform, prioritized (the bad one), prioritized wide
@@ -185,7 +185,7 @@ def test_bad_index_sets_the_status_of_its_own_learner_only():
         descs[j] = f._desc(rows, s['n_valid'], 5, s['first'], s['champ'], bad if j == 1 else None, r, 0)
         if s.get('per'):
             pers[j] = FusedTD3._per_desc(src, s['n_valid'], r, 0)
-    _native.call('serl_td3_train_group_per', descs, pers, 3, device=DEV)
+    _native.call('serl_td3_learn', descs, pers, 3, device=DEV)
     torch.cuda.synchronize()
     assert [int(r.status.item()) for r in rs] == [0, _native.TD3_STATUS_INDEX, 0]
     with pytest.raises(_native.NativeError):

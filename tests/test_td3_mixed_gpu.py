@@ -1,4 +1,4 @@
-"""K7 for learners of different actor shapes in one launch (serl_td3_train_mixed, td3_fused.train_group(mixed_shapes=True))
+"""K7 for learners of different actor shapes in one launch (serl_td3_learn, td3_fused.train_group(mixed_shapes=True))
 and the mixed-shape sweep driver on the GPU.  Every comparison is bitwise against the same learners trained alone
 (FusedTD3.run, Agent.train) from copies of the same initial state, as in test_td3_group_gpu.py."""
 import random
@@ -99,7 +99,7 @@ def test_full_mixed_group_runs_in_waves_and_matches():
         assert_same(a, got[k], record=False)
 
 
-def test_bad_index_sets_the_status_of_its_own_learner_only():
+def test_bad_index_in_one_learn_call_sets_only_its_learners_status():
     from serl_b200 import _native
     specs = [dict(MIXED[k], n=5) for k in (0, 4, 1)]
     shapes = [SHAPES[k] for k in (0, 4, 1)]
@@ -112,7 +112,7 @@ def test_bad_index_sets_the_status_of_its_own_learner_only():
         r = f._launch(5, False)
         rs.append(r)
         descs[j] = f._desc(rows[j], s['n_valid'], 5, s['first'], s['champ'], bad if j == 1 else None, r, 0)
-    _native.call('serl_td3_train_mixed', descs, 3, device=DEV)
+    _native.call('serl_td3_learn', descs, None, 3, device=DEV)
     torch.cuda.synchronize()
     assert [int(r.status.item()) for r in rs] == [0, _native.TD3_STATUS_INDEX, 0]
 

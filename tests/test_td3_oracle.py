@@ -1,6 +1,6 @@
 """K7 (the fused TD3 learner, csrc/td3.cu) without a GPU: the explicit-draw oracle (oracle/td3.py) against TD3.update_parameters
-bit for bit, the C-ABI of include/serl_td3.h (binding, descriptor layout, constants, state size) and the argument checks
-that reject an unsupported learner before any CUDA call."""
+bit for bit, and the C-ABI of include/serl_td3.h and serl_td3_per.h: the binding, the descriptor layouts, the constants, the
+state size, and the checks with which serl_td3_learn refuses a learner or a call before any CUDA call."""
 import copy
 import ctypes
 import os
@@ -144,20 +144,65 @@ def header_text(name):
     return re.sub(r'/\*.*?\*/', '', open(os.path.join(ROOT, 'include', name)).read(), flags=re.S)
 
 
-def test_binding_matches_the_td3_header():
-    """_native.TD3_SIGNATURES against the prototypes of include/serl_td3.h (pointer / integer kinds and arity)"""
+def prototypes(name):
+    return {n: (r.strip(), [p.strip() for p in ps.split(',')])
+            for r, n, ps in re.findall(r'([A-Za-z_][\w ]*\**)\s*\b(serl_[a-z0-9_]+)\s*\(([^)]*)\)\s*;', header_text(name))}
+
+
+def test_binding_matches_the_learn_prototype():
+    """_native.TD3_SIGNATURES against the prototypes of include/serl_td3.h (return, pointer and integer kinds, arity), the
+    headers serl_b200.h includes, and a library that exports no other K7 entry point"""
     from serl_b200 import _native
-    protos = {n: [p.strip() for p in ps.split(',')]
-              for _, n, ps in re.findall(r'([A-Za-z_][\w ]*\**)\s*\b(serl_[a-z0-9_]+)\s*\(([^)]*)\)\s*;', header_text('serl_td3.h'))}
-    assert sorted(protos) == sorted(_native.TD3_SIGNATURES) == ['serl_td3_state_floats', 'serl_td3_train']
-    assert '#include "serl_td3.h"' in open(os.path.join(ROOT, 'include', 'serl_b200.h')).read()
-    for name, params in protos.items():
+    kinds = {'int': ctypes.c_int32, 'int32_t': ctypes.c_int32, 'int64_t': ctypes.c_int64}
+    protos = prototypes('serl_td3.h')
+    assert sorted(protos) == sorted(_native.TD3_SIGNATURES) == ['serl_td3_learn', 'serl_td3_state_floats']
+    for name, (ret, params) in protos.items():
         restype, argtypes = _native.TD3_SIGNATURES[name]
-        assert len(argtypes) == len(params)
+        assert kinds[ret] is restype, name
+        assert len(argtypes) == len(params), name
         for decl, t in zip(params, argtypes):
             assert ('*' in decl) == (t is ctypes.c_void_p or issubclass(t, ctypes._Pointer)), (name, decl)
-    assert _native.TD3_SIGNATURES['serl_td3_state_floats'][0] is ctypes.c_int64
-    assert _native.TD3_SIGNATURES['serl_td3_train'][0] is ctypes.c_int
+            if '*' not in decl:
+                assert kinds[decl.split()[0]] is t, (name, decl)
+    text = open(os.path.join(ROOT, 'include', 'serl_b200.h')).read()
+    assert all('#include "%s"' % h in text for h in ('serl_td3.h', 'serl_td3_per.h', 'serl_route.h'))
+    from serl_b200 import build
+    build.build()
+    syms = subprocess.check_output(['nm', '-D', '--defined-only', _native.LIB_PATH], text=True).split()
+    assert sorted(x for x in syms if x.startswith('serl_td3_')) == ['serl_td3_learn', 'serl_td3_state_floats']
+
+
+def test_learn_takes_per_descriptors():
+    """serl_td3_learn's parameters, declared and bound: the learners, their per descriptors, their count and the stream"""
+    from serl_b200 import _native
+    ret, params = prototypes('serl_td3.h')['serl_td3_learn']
+    assert ret == 'int' and params == ['const serl_td3_desc* descs', 'const serl_td3_per_desc* pers', 'int n', 'void* stream']
+    restype, argtypes = _native.TD3_SIGNATURES['serl_td3_learn']
+    assert restype is ctypes.c_int and len(argtypes) == 4
+    assert argtypes[0]._type_ is _native.TD3Desc and argtypes[1]._type_ is _native.TD3PerDesc
+    assert argtypes[2] is ctypes.c_int32 and argtypes[3] is ctypes.c_void_p
+
+
+def test_max_group_matches_the_header(tmp_path):
+    from serl_b200 import _native
+    src = tmp_path / 'c.c'
+    src.write_text('#include "serl_b200.h"\n'
+                   'int (*f)(const serl_td3_desc*, const serl_td3_per_desc*, int, void*) = serl_td3_learn;\n')
+    out = subprocess.check_output(['gcc', '-E', '-dM', '-I', os.path.join(ROOT, 'include'), str(src)], text=True)
+    assert '#define SERL_TD3_MAX_GROUP %d' % _native.TD3_MAX_GROUP in out
+    assert _native.TD3_MAX_GROUP == 64
+
+
+def test_k7_headers_compile_alone_in_any_order(tmp_path):
+    """serl_b200.h, serl_td3.h and serl_td3_per.h each declare all of K7 on their own, whichever is included first"""
+    src = tmp_path / 'c.c'
+    for first in ('serl_b200.h', 'serl_td3.h', 'serl_td3_per.h', 'serl_route.h'):
+        for second in ('', 'serl_b200.h', 'serl_td3.h', 'serl_td3_per.h'):
+            src.write_text('#include "%s"\n' % first + ('#include "%s"\n' % second if second else '') +
+                           'int (*f)(const serl_td3_desc*, const serl_td3_per_desc*, int, void*) = serl_td3_learn;\n'
+                           'int64_t (*g)(int32_t) = serl_per_tree_doubles;\nint m = SERL_TD3_MAX_GROUP;\n')
+            subprocess.check_call(['gcc', '-fsyntax-only', '-Wall', '-Werror', '-I', os.path.join(ROOT, 'include'), str(src)])
+
 
 
 def test_ctypes_mirror_of_the_td3_descriptor_matches_the_header(tmp_path):
@@ -192,28 +237,212 @@ def test_state_size_is_the_four_modules_and_their_adam_moments():
     assert td3_fused.state_floats(rollout.actor_shape(72)) * 4 == 437_840       # 438 KB at h = 72, L = 3
 
 
-def test_unsupported_learner_is_rejected_before_any_cuda_call():
-    """bad shapes, batch sizes and launch parameters fail with SERL_ERR_ARG; the device pointers are never dereferenced"""
+def _desc(shape=None, **kw):
+    from serl_b200 import _native, rollout
+    d = _native.TD3Desc()
+    d.shape = shape or rollout.actor_shape(72)
+    d.d_state, d.d_replay, d.d_losses = 0x10000, 0x20000, 0x30000          # non-null, never read
+    d.replay_cols, d.n_valid, d.batch, d.n_steps, d.policy_update_freq = 19, 1000, 86, 10, 3
+    for k, v in kw.items():
+        setattr(d, k, v)
+    return d
+
+
+def _per(tree=0x40000, **kw):
+    from serl_b200 import _native
+    p = _native.TD3PerDesc()
+    p.d_tree, p.capacity, p.n_valid = tree, 2000, 1000                    # non-null, never read
+    p.alpha, p.beta0, p.beta_frames = 0.6, 0.4, 1e5
+    for k, v in kw.items():
+        setattr(p, k, v)
+    return p
+
+
+def learn(descs, pers=None, n=None):
+    """serl_td3_learn on the given descriptors (and per descriptors, or NULL): (status, serl_last_error)"""
+    from serl_b200 import _native
+    a = (_native.TD3Desc * max(len(descs), 1))(*descs)
+    b = None if pers is None else (_native.TD3PerDesc * max(len(pers), 1))(*pers)
+    rc = _native.lib().serl_td3_learn(a, b, len(descs) if n is None else n, None)
+    return rc, _native.lib().serl_last_error().decode()
+
+
+def _group():
+    """a prioritized narrow learner, a uniform narrow one and a prioritized wide one, all valid"""
+    from serl_b200 import rollout
+    shapes = [rollout.actor_shape(32, 1, 'tanh'), rollout.actor_shape(72, 3, 'elu'), rollout.actor_shape(256, 3, 'relu')]
+    return shapes, [_desc(s, seed=k) for k, s in enumerate(shapes)], [_per(), _per(tree=None), _per()]
+
+
+def _bad_shapes():
+    from serl_b200 import _native, rollout
+    return [rollout.actor_shape(48), rollout.actor_shape(100, 3), rollout.actor_shape(72, 0), rollout.actor_shape(400, 3),
+            rollout.actor_shape(256, 9), rollout.actor_shape(72, 3, 'tanh', state_dim=6), _native.ActorShape(8, 3, 72, 3, 0),
+            _native.ActorShape(7, 3, 72, 3, 3)]
+
+
+def _bad_fields():
+    return [dict(batch=129), dict(batch=0), dict(n_valid=85), dict(replay_cols=18), dict(policy_update_freq=0),
+            dict(cluster_size=3), dict(cluster_size=16), dict(flags=2), dict(d_state=None), dict(d_replay=None),
+            dict(d_losses=None), dict(n_steps=-1), dict(first_iteration=-1), dict(critic_adam_steps=-1),
+            dict(actor_adam_steps=-1)]
+
+
+def test_unsupported_learner_is_refused_alone():
+    """bad shapes, batch sizes and launch parameters of one learner (n = 1) fail with SERL_ERR_ARG; the device pointers are
+    never dereferenced"""
+    from serl_b200 import build, _native, rollout, td3_fused
+    build.build()
+    before = _native.lib().serl_launch_count()
+    for shape in _bad_shapes():
+        rc, msg = learn([_desc(shape)])
+        assert rc == -1 and msg.startswith('serl_td3_learn: learner 0: unsupported actor shape'), (shape.hidden, msg)
+        with pytest.raises(_native.NativeError):
+            td3_fused.state_floats(shape)
+    for kw in _bad_fields():
+        rc, msg = learn([_desc(**kw)])
+        assert rc == -1 and msg.startswith('serl_td3_learn: learner 0: '), (kw, rc, msg)
+    assert 'batch' in learn([_desc(batch=129)])[1]
+    assert _native.lib().serl_launch_count() == before
+    assert learn([_desc(n_steps=0)])[0] == 0                  # nothing to do: no launch
+    with pytest.raises(_native.NativeError):
+        td3_fused.state_floats(rollout.actor_shape(100))
+
+
+def test_shapes_outside_the_wide_domain_are_refused():
+    from serl_b200 import build, _native, rollout, td3_fused
+    build.build()
+    bad = [rollout.actor_shape(321, 3), rollout.actor_shape(256, 9), rollout.actor_shape(320, 9), rollout.actor_shape(256, 0),
+           _native.ActorShape(8, 3, 256, 3, 0), _native.ActorShape(7, 4, 256, 3, 0), _native.ActorShape(7, 3, 256, 3, 3)]
+    for shape in bad:
+        rc, msg = learn([_desc(shape)])
+        assert rc == -1 and 'shape' in msg, (shape.hidden, shape.num_layers, rc, msg)
+        with pytest.raises(_native.NativeError):
+            td3_fused.state_floats(shape)
+    for kw in _bad_fields():
+        rc, msg = learn([_desc(rollout.actor_shape(256, 3), **kw)])
+        assert rc == -1 and msg.startswith('serl_td3_learn: learner 0: '), (kw, rc, msg)
+    for h, nl in ((129, 1), (256, 3), (320, 8)):
+        assert learn([_desc(rollout.actor_shape(h, nl), n_steps=0)])[0] == 0          # accepted; nothing to do, no launch
+
+
+def test_refusals_keep_their_messages():
+    from serl_b200 import build
+    build.build()
+    assert learn([_desc(batch=129)]) == (-1, 'serl_td3_learn: learner 0: batch must be 1..128')
+    assert learn([_desc(cluster_size=3)]) == (-1, 'serl_td3_learn: learner 0: cluster_size must be 0, 1, 2, 4 or 8')
+    assert learn([_desc()], [_per(alpha=0.0)]) == (-1, 'serl_td3_learn: learner 0: alpha must be in (0, 1]')
+    assert learn([_desc(), _desc(cluster_size=4)]) == (-1, "serl_td3_learn: learner 1: cluster_size differs from learner 0's")
+
+
+def test_call_is_refused_before_any_cuda_call():
+    """the call's own checks, and every check of a learner made for each learner of a group, naming it"""
     from serl_b200 import build, _native, rollout
     build.build()
     L = _native.lib()
+    before = L.serl_launch_count()
+    ok = [_desc(seed=s) for s in range(3)]
+    assert L.serl_td3_learn(None, None, 2, None) == -1
+    assert L.serl_last_error().decode() == 'serl_td3_learn: null descriptors'
+    assert learn(ok, None, 0) == (-1, 'serl_td3_learn: n must be 1..SERL_TD3_MAX_GROUP (64)')
+    assert learn([_desc()] * (_native.TD3_MAX_GROUP + 1)) == (-1, 'serl_td3_learn: n must be 1..SERL_TD3_MAX_GROUP (64)')
+    rc, msg = learn(ok[:1] + [_desc(cluster_size=4)])
+    assert rc == -1 and 'learner 1' in msg and 'cluster_size' in msg
+    for kw in _bad_fields() + [dict(shape=s) for s in _bad_shapes()]:
+        rc, msg = learn(ok[:1] + [_desc(**kw)] + ok[1:])
+        assert rc == -1 and msg.startswith('serl_td3_learn: learner 1:'), (kw, rc, msg)
+    rc, msg = learn([_desc(rollout.actor_shape(100))] * 2)
+    assert rc == -1 and 'learner 0' in msg and 'shape' in msg
+    # the same shape everywhere, cluster_size 0 and 8 agreeing, and nothing to do: no launch
+    assert learn([_desc(n_steps=0, cluster_size=c) for c in (0, 8, 0)])[0] == 0
+    assert L.serl_launch_count() == before
 
-    def run(**kw):
-        d = _native.TD3Desc()
-        d.shape = rollout.actor_shape(72)
-        d.d_state, d.d_replay, d.d_losses = 0x10000, 0x20000, 0x30000          # non-null, never read
-        d.replay_cols, d.n_valid, d.batch, d.n_steps, d.policy_update_freq = 19, 1000, 86, 10, 3
-        for k, v in kw.items():
-            setattr(d, k, v)
-        return L.serl_td3_train(ctypes.byref(d), None), L.serl_last_error().decode()
 
-    for kw in (dict(shape=rollout.actor_shape(48)), dict(shape=rollout.actor_shape(72, 0)), dict(shape=_native.ActorShape(8, 3, 72, 3, 0)),
-               dict(shape=_native.ActorShape(7, 3, 72, 3, 3)), dict(batch=129), dict(batch=0), dict(n_valid=85), dict(replay_cols=18),
-               dict(policy_update_freq=0), dict(cluster_size=3), dict(cluster_size=16), dict(flags=2), dict(d_state=None)):
-        rc, msg = run(**kw)
-        assert rc == -1 and msg.startswith('serl_td3'), (kw, rc, msg)
-    assert 'batch' in run(batch=129)[1] and 'shape' in run(shape=rollout.actor_shape(48))[1]
-    assert run(n_steps=0)[0] == 0                         # nothing to do: no launch
-    with pytest.raises(_native.NativeError):
-        from serl_b200 import td3_fused
-        td3_fused.state_floats(rollout.actor_shape(100))
+def test_learner_is_refused_at_every_place_of_a_mixed_group():
+    """narrow and wide, prioritized and uniform learners: a bad learner anywhere is named, with or without per descriptors,
+    and nothing is launched"""
+    from serl_b200 import build, _native
+    build.build()
+    before = _native.lib().serl_launch_count()
+    shapes, ok, pers = _group()
+    for kw in _bad_fields() + [dict(shape=s) for s in _bad_shapes()]:
+        for i in range(3):                  # learners 0 and 2 are prioritized, learner 1 uniform
+            descs = list(ok)
+            descs[i] = _desc(**dict(dict(shape=shapes[i]), **kw))
+            for p in (pers, None):
+                rc, msg = learn(descs, p)
+                assert rc == -1 and msg.startswith('serl_td3_learn: learner %d: ' % i), (kw, i, rc, msg)
+    rc, msg = learn(ok[:2] + [_desc(shapes[2], cluster_size=4)], pers)
+    assert (rc, msg) == (-1, "serl_td3_learn: learner 2: cluster_size differs from learner 0's")
+    assert _native.lib().serl_launch_count() == before
+
+
+def test_mixed_learners_without_steps_make_no_launch():
+    from serl_b200 import build, _native
+    build.build()
+    before = _native.lib().serl_launch_count()
+    shapes, _, _ = _group()
+    # different shapes, both hidden classes, cluster_size 0 and 8 agreeing, and nothing to do
+    assert learn([_desc(s, n_steps=0, cluster_size=c) for s, c in zip(shapes, (0, 8, 0))])[0] == 0
+    assert _native.lib().serl_launch_count() == before
+
+
+def test_bad_per_learner_is_refused_alone():
+    """every check of prioritized replay for one learner with a tree, naming the field"""
+    from serl_b200 import build, _native
+    build.build()
+    before = _native.lib().serl_launch_count()
+    for kw, word in _per_cases():
+        rc, msg = learn([_desc()], [_per(**kw)])
+        assert rc == -1 and msg.startswith('serl_td3_learn: learner 0: ') and word in msg, (kw, rc, msg)
+    for kw in (dict(batch=129), dict(cluster_size=3), dict(d_state=None)):
+        rc, msg = learn([_desc(**kw)], [_per()])
+        assert rc == -1 and msg.startswith('serl_td3_learn: learner 0: '), (kw, msg)
+    assert _native.lib().serl_launch_count() == before
+    assert learn([_desc(n_steps=0)], [_per()])[0] == 0                  # nothing to do: no launch
+
+
+def _per_cases():
+    return ((dict(alpha=0.0), 'alpha'), (dict(alpha=1.5), 'alpha'), (dict(alpha=float('nan')), 'alpha'),
+            (dict(beta0=-0.1), 'beta0'), (dict(beta0=1.1), 'beta0'), (dict(beta_frames=0.0), 'beta_frames'),
+            (dict(beta_frames=float('nan')), 'beta_frames'), (dict(capacity=999, n_valid=1000), 'n_valid'),
+            (dict(n_valid=999), 'n_valid'), (dict(capacity=0), 'capacity'), (dict(capacity=(1 << 30) + 1), 'capacity'))
+
+
+def test_bad_per_learner_is_refused_in_a_group():
+    """every check of a learner, for a prioritized and a uniform one, and every check of prioritized replay for a learner
+    with a tree in a group; a learner without a tree does not read the rest of its per descriptor"""
+    from serl_b200 import build, _native
+    build.build()
+    before = _native.lib().serl_launch_count()
+    shapes, ok, pers = _group()
+    for kw in _bad_fields():
+        for j in (0, 1):                  # learner 0 is prioritized, learner 1 uniform
+            descs = list(ok)
+            descs[j] = _desc(shapes[j], **kw)
+            rc, msg = learn(descs, pers)
+            assert rc == -1 and msg.startswith('serl_td3_learn: learner %d:' % j), (kw, j, rc, msg)
+    for kw, word in _per_cases():
+        rc, msg = learn(ok, pers[:2] + [_per(**kw)])
+        assert rc == -1 and msg.startswith('serl_td3_learn: learner 2: ') and word in msg, (kw, rc, msg)
+        # ...which a learner without a tree ignores
+        assert learn([_desc(s, n_steps=0) for s in shapes], pers[:2] + [_per(tree=None, **kw)])[0] == 0, kw
+    assert _native.lib().serl_launch_count() == before
+
+
+def test_prioritized_and_uniform_learners_without_steps_make_no_launch():
+    """prioritized and uniform, narrow and wide learners (cluster_size 0 and 8 agreeing) with nothing to do are accepted
+    and launch nothing, with per descriptors, without, and one by one"""
+    from serl_b200 import build, _native, rollout
+    build.build()
+    L = _native.lib()
+    before = L.serl_launch_count()
+    shapes = [rollout.actor_shape(72), rollout.actor_shape(256), rollout.actor_shape(72, 2), rollout.actor_shape(320, 8),
+              rollout.actor_shape(129, 1), rollout.actor_shape(32, 1, 'elu')]
+    descs = [_desc(s, n_steps=0, cluster_size=c) for s, c in zip(shapes, (0, 8, 0, 8, 0, 8))]
+    per_descs = [_per(), _per(tree=None), _per(tree=None), _per(), _per(), _per(tree=None)]
+    assert learn(descs, per_descs)[0] == 0
+    assert learn(descs)[0] == 0
+    for d, p in zip(descs, per_descs):
+        assert learn([d], [p])[0] == 0 and learn([d])[0] == 0
+    assert L.serl_launch_count() == before

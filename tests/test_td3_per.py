@@ -1,7 +1,8 @@
 """Prioritized experience replay (include/serl_td3_per.h, csrc/per.cu, K7's PER learner) on the CPU: the priority tree
 restated in numpy against the reference's PrioritizedReplayMemory, the weight and beta formulas against its arithmetic, the
-ctypes mirror of the header, the refusals made before any CUDA call, and the weighted oracle (tests/td3_per_oracle.py)
-against oracle/td3.py and the torch TD3's weighted path."""
+ctypes mirror of the header, the tree entry points' refusals, and the weighted oracle (tests/td3_per_oracle.py) against
+oracle/td3.py and the torch TD3's weighted path.  serl_td3_learn's refusals of a prioritized learner are in
+test_td3_oracle.py."""
 import copy
 import ctypes
 import importlib.util
@@ -144,41 +145,12 @@ def test_ctypes_mirror_of_the_per_descriptor_matches_the_header(tmp_path):
     assert out[-1] == _native.PER_MAX_CAPACITY
 
 
-def test_bad_per_launches_are_rejected_before_any_cuda_call():
-    """bad alpha / beta, a null tree, n_valid > capacity (and every serl_td3_train check) fail with SERL_ERR_ARG; the device
-    pointers are never dereferenced"""
-    from serl_b200 import build, _native, rollout
+def test_tree_entry_points_refuse_bad_arguments():
+    """the tree's entry points refuse bad sizes, rows and parameters with SERL_ERR_ARG; the device pointers are never
+    dereferenced"""
+    from serl_b200 import build, _native
     build.build()
     L = _native.lib()
-
-    def run(desc=None, **kw):
-        d = _native.TD3Desc()
-        d.shape = rollout.actor_shape(72)
-        d.d_state, d.d_replay, d.d_losses = 0x10000, 0x20000, 0x30000          # non-null, never read
-        d.replay_cols, d.n_valid, d.batch, d.n_steps, d.policy_update_freq = 19, 1000, 86, 10, 3
-        for k, v in (desc or {}).items():
-            setattr(d, k, v)
-        p = _native.TD3PerDesc()
-        p.d_tree, p.capacity, p.n_valid, p.alpha, p.beta0, p.beta_frames = 0x40000, 2000, 1000, 0.6, 0.4, 1e5
-        for k, v in kw.items():
-            setattr(p, k, v)
-        return L.serl_td3_train_per(ctypes.byref(d), ctypes.byref(p), None), L.serl_last_error().decode()
-
-    for kw, word in ((dict(d_tree=None), 'd_tree'), (dict(alpha=0.0), 'alpha'), (dict(alpha=1.5), 'alpha'),
-                     (dict(alpha=float('nan')), 'alpha'), (dict(beta0=-0.1), 'beta0'), (dict(beta0=1.1), 'beta0'),
-                     (dict(beta_frames=0.0), 'beta_frames'), (dict(capacity=999, n_valid=1000), 'n_valid'),
-                     (dict(n_valid=999), 'n_valid'), (dict(capacity=0), 'capacity')):
-        rc, msg = run(**kw)
-        assert rc == -1 and msg.startswith('serl_td3_train_per: ') and word in msg, (kw, rc, msg)
-    for desc in (dict(batch=129), dict(shape=rollout.actor_shape(48)), dict(cluster_size=3), dict(d_state=None)):
-        rc, msg = run(desc)
-        assert rc == -1 and msg.startswith('serl_td3_train_per: '), (desc, msg)
-    d = _native.TD3Desc()
-    d.shape, d.d_state, d.d_replay, d.d_losses = rollout.actor_shape(72), 0x10000, 0x20000, 0x30000
-    d.replay_cols, d.n_valid, d.batch, d.n_steps, d.policy_update_freq = 19, 1000, 86, 10, 3
-    assert L.serl_td3_train_per(ctypes.byref(d), None, None) == -1 and 'null per' in L.serl_last_error().decode()
-    assert run(dict(n_steps=0))[0] == 0                   # nothing to do: no launch
-    # the tree's own entry points
     assert L.serl_per_tree_doubles(800_000) == 4 * (1 << 20) and L.serl_per_tree_doubles(1) == 4
     assert L.serl_per_tree_doubles(0) == -1 and L.serl_per_tree_doubles(-5) == -1
     assert L.serl_per_insert(0x40000, 100, 101, 0, 1, None) == -1

@@ -1,4 +1,4 @@
-"""K7 with prioritized replay (serl_td3_train_per) and the device priority tree (csrc/per.cu) on the GPU.
+"""K7 with prioritized replay (serl_td3_learn with a priority tree) and the device priority tree (csrc/per.cu) on the GPU.
 
 Every K7 case runs with its draws recorded (rows, weights, TD errors, noise, CAPS uniforms) and replays them on the CPU
 through the weighted fp32 oracle and its float64 copy (tests/td3_per_oracle.py), under the error budget of

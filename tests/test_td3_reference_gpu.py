@@ -1,5 +1,5 @@
 """K7, the fused TD3 learner (csrc/td3.cu, serl_b200/td3_fused.py), against a float64 reference across the inputs
-serl_td3_train accepts.
+serl_td3_learn accepts.
 
 Every case runs K7 with its draws recorded (batch rows, clipped target-policy noise, CAPS uniforms) and replays them on the
 CPU through the fp32 oracle (oracle/td3.py, bit-exact against TD3.update_parameters) and through its float64 copy

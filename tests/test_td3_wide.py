@@ -1,5 +1,5 @@
-"""K7 (csrc/td3.cu) for actors wider than 128, without a GPU: the state size of the wide shapes, the header's bounds of
-the wide domain against _native, and the argument checks that reject a shape outside it before any CUDA call."""
+"""K7 (csrc/td3.cu) for actors wider than 128, without a GPU: the state size of the wide shapes and the header's bounds of
+the wide domain against _native.  serl_td3_learn's refusal of shapes outside it is in test_td3_oracle.py."""
 import ctypes
 import os
 import subprocess
@@ -8,7 +8,6 @@ import types
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ERR_ARG = -1                  # SERL_ERR_ARG (include/serl_b200.h)
 
 
 def td3_args(hidden, num_layers, activation='tanh'):
@@ -41,35 +40,3 @@ def test_wide_bounds_match_the_header(tmp_path):
     out = [int(x) for x in subprocess.check_output([str(exe)], text=True).split()]
     assert out == [_native.TD3_MAX_HIDDEN, _native.TD3_MAX_WIDE_LAYERS, _native.TD3_MAX_BATCH, _native.TD3_CRITIC_HIDDEN]
     assert (_native.TD3_MAX_HIDDEN, _native.TD3_MAX_WIDE_LAYERS) == (320, 8)
-
-
-def test_shapes_outside_the_wide_domain_are_rejected_before_any_cuda_call():
-    """the descriptor's device pointers are never dereferenced: every case fails with SERL_ERR_ARG in the argument checks"""
-    from serl_b200 import build, _native, rollout, td3_fused
-    build.build()
-    L = _native.lib()
-
-    def run(**kw):
-        d = _native.TD3Desc()
-        d.shape = rollout.actor_shape(256, 3)
-        d.d_state, d.d_replay, d.d_losses = 0x10000, 0x20000, 0x30000          # non-null, never read
-        d.replay_cols, d.n_valid, d.batch, d.n_steps, d.policy_update_freq = 19, 1000, 86, 10, 3
-        for k, v in kw.items():
-            setattr(d, k, v)
-        return L.serl_td3_train(ctypes.byref(d), None), L.serl_last_error().decode()
-
-    bad_shapes = [rollout.actor_shape(321, 3), rollout.actor_shape(256, 9), rollout.actor_shape(320, 9),
-                  rollout.actor_shape(256, 0), rollout.actor_shape(48, 3), rollout.actor_shape(100, 3),
-                  _native.ActorShape(8, 3, 256, 3, 0), _native.ActorShape(7, 4, 256, 3, 0), _native.ActorShape(7, 3, 256, 3, 3)]
-    for shape in bad_shapes:
-        rc, msg = run(shape=shape)
-        assert rc == ERR_ARG and 'shape' in msg, (shape.hidden, shape.num_layers, rc, msg)
-        with pytest.raises(_native.NativeError):
-            td3_fused.state_floats(shape)
-    for kw in (dict(batch=129), dict(batch=0), dict(n_valid=85), dict(replay_cols=18), dict(policy_update_freq=0),
-               dict(cluster_size=3), dict(cluster_size=16), dict(flags=2), dict(d_state=None), dict(d_replay=None),
-               dict(d_losses=None), dict(n_steps=-1), dict(first_iteration=-1)):
-        rc, msg = run(**kw)
-        assert rc == ERR_ARG and msg.startswith('serl_td3'), (kw, rc, msg)
-    for h, nl in ((129, 1), (256, 3), (320, 8)):
-        assert run(shape=rollout.actor_shape(h, nl), n_steps=0)[0] == 0          # accepted; nothing to do, no launch
