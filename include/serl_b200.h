@@ -64,12 +64,13 @@ int64_t serl_actor_num_params(const serl_actor_shape* shape);
 /* Population rollout — replaces the loop `for net in pop: for i in range(num_evals): evaluate(net)` of
  * base/core/agent.py:234-241 with Agent.evaluate (agent.py:63-138), CitationEnv.reset/step
  * (envs/phlabenv.py:401-482), Actor.select_action (genetic_agent.py:107-109) and the native plant
- * step (envs/<variant>/_citation*.so: step @0x6030) fused in one kernel.
+ * step (envs/<variant>/_citation*.so: step @0x6030) fused in one kernel, described by a serl_rollout_desc.
  *
  *   d_weights   [pop, P] fp32, row = one actor genome
  *   d_ref_levels[n_envs, 2, SERL_REF_BLOCKS] f64 (deg), d_ref_starts same shape (s)
  *   d_env_mode  [n_envs] int32, variant | fault << 8
- *   horizon     max steps per episode (reference: 2001, phlabenv.py:82,181,392)
+ *   horizon     max steps per episode (reference: 2001, phlabenv.py:82,181,392); with t_max > 0 it must cover
+ *               t_max / 0.01 + 1 steps
  *   d_action_noise optional [pop, n_envs, horizon, 3] fp32: clipped exploration noise added to the policy output
  *               (base/core/agent.py:90-93, is_action_noise=True); NULL for fitness evaluation
  * outputs
@@ -81,24 +82,10 @@ int64_t serl_actor_num_params(const serl_actor_shape* shape);
  *               12-14 commanded deflection last_u, 15 reward, 16-18 action fed to the env, 19-21 tracking error
  *   d_actions   optional [pop, n_envs, horizon, 3] fp32: commanded deflection last_u of every executed step (agent.py:98),
  *               the input of the smoothness metric (serl_smoothness, which computes its DFT in fp32)
- */
-#define SERL_TRACE_COLS 22
-int serl_rollout(const float* d_weights, int32_t pop, const serl_actor_shape* shape,
-                 const double* d_ref_levels, const double* d_ref_starts, const int32_t* d_env_mode,
-                 int32_t n_envs, int32_t horizon, const float* d_action_noise,
-                 double* d_returns, int32_t* d_steps, double* d_fitness, double* d_trace, float* d_actions,
-                 void* stream);
-
-/* Same with the episode length and reference-transition width of the reference's evaluation mode
- * (envs/phlabenv.py:295-301 set_eval_mode: t_max = 80 s; init_ref :303-345: smooth_width = t_max // 6, block_width =
- * t_max // 5 are encoded in d_ref_starts by the caller); horizon must cover t_max / 0.01 + 1 steps. */
-int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shape* shape,
-                      const double* d_ref_levels, const double* d_ref_starts, const int32_t* d_env_mode,
-                      int32_t n_envs, int32_t horizon, const float* d_action_noise,
-                      double* d_returns, int32_t* d_steps, double* d_fitness, double* d_trace, float* d_actions,
-                      double t_max, double smooth_width, void* stream);
-
-/* The same launch described by a struct, with the optional inputs / outputs the two entry points above do not carry.
+ *   t_max, smooth_width  the episode length [s] and the width of the reference's raised-cosine transitions [s].  t_max <= 0
+ *               selects the training episode (20 s, smooth width 3 s).  The reference's evaluation mode
+ *               (envs/phlabenv.py:295-301 set_eval_mode) is t_max = 80 with smooth_width = t_max // 6 (init_ref :303-345;
+ *               its block_width = t_max // 5 is encoded in d_ref_starts by the caller); smooth_width must be > 0 when t_max > 0
  *   d_env_order  optional [n_envs] int32 permutation: lane slot j flies env d_env_order[j] (the host sorts envs so that
  *                the 32 lanes of a warp share fault shims / trim; results are still written at the env's own index)
  *   d_replay     optional [pop, horizon, SERL_REPLAY_COLS] fp32: the transitions of env `replay_env` of every actor, the
@@ -176,8 +163,8 @@ int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shap
  *                The tracking sums of incremental control are the attitude ones, with the integrated deflection u in the
  *                trace and d_actions.  With symmetric control d_track holds sum |e_theta|, 0, 0, sum e_theta, e_theta =
  *                ref_theta(t_k) (with the 0.22 deg trim) - theta of the state env.x holds when step k starts; the d_cost
- *                tally is the attitude one (it still tests alpha, phi and V)
- * t_max <= 0 selects the training defaults (20 s, smooth width 3 s). */
+ *                tally is the attitude one (it still tests alpha, phi and V) */
+#define SERL_TRACE_COLS 22
 #define SERL_TRACK_COLS 4
 #define SERL_REPLAY_COLS 20                       /* = SERL_REPLAY_COLS_OF(7) */
 #define SERL_REPLAY_COLS_OF(S) (2 * (S) + 6)      /* obs S | action 3 | next_obs S | reward | done | cost */

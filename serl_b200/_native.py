@@ -83,12 +83,9 @@ class TD3PerDesc(ctypes.Structure):
 
 
 _vp, _i32, _i64, _f64, _int, _shape = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_double, ctypes.c_int, ctypes.POINTER(ActorShape)
-_rollout_args = [_vp, _i32, _shape, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp]
 # entry point -> (restype, argtypes), in the header's order; every entry point returning a serl_status takes the stream last
 SIGNATURES = {
     'serl_actor_num_params': (_i64, [_shape]),
-    'serl_rollout': (_int, _rollout_args + [_vp]),
-    'serl_rollout_eval': (_int, _rollout_args + [_f64, _f64, _vp]),
     'serl_rollout_run': (_int, [ctypes.POINTER(RolloutDesc), _vp]),
     'serl_actor_forward': (_int, [_vp, _shape, _vp, _i32, _vp, _vp]),
     'serl_actor_num_params_wide': (_i64, [_vp, _i32]),

@@ -12,7 +12,7 @@
 // (genome, reference-signal parameters) and end (return, step count) unless a trace / action history is requested.
 //
 // Two actor implementations:
-//   rollout_kernel_persist<H, TABS, GUST>  persistent grid, one CTA per SM.  The MLP is a register-tiled GEMM inside a warp
+//   rollout_kernel_persist<H, TABS, ...>   persistent grid, one CTA per SM.  The MLP is a register-tiled GEMM inside a warp
 //                           (lane = 1/8 of the output neurons x 8 envs, float2 pairs, activations exchanged through a
 //                           per-warp shared-memory buffer, weights broadcast from shared memory; h in {32,64,72,96,128}).  The CTA's warps take
 //                           their steps in lockstep (one barrier per step: shared instruction fetch), genomes arrive by bulk
@@ -22,6 +22,7 @@
 
 #define PLANT_SMEM_BUCKETS          // K1 stages the bucketed searches' byte tables with the plant tables (plant_env.cuh)
 #include "plant_env.cuh"
+#include "rollout_variant.h"
 
 // ---- simple actor: every thread evaluates the whole MLP for its own observation -------------------------
 __device__ void actor_forward_simple(const float* __restrict__ w, const serl_actor_shape sh, float* bufA, float* bufB,
@@ -423,18 +424,16 @@ __global__ void genome_layout_kernel(const float* __restrict__ w, float* __restr
 // the slot's warps meet at its named barrier for that and for the slot-uniform decisions of the lockstep loop (see there).
 // TABS: plant tables staged in shared memory (true) or read from global memory through L1 (false: h = 128, whose
 // 207 KB genome leaves no room for them).
-// GUST: the launch contains envs of the gust build (serl_rollout_desc.flags & SERL_ROLLOUT_GUST); the training instantiation
-// carries no trace of the feature (a gust env in it raises SERL_STATUS_GUST_FLAG)
-// TRACK: the launch writes the tracking-error sums `tk` (serl_rollout_desc.d_track; instantiated with GUST only); the
-// sums travel in the hand-over records too
+// GUST, TRACK, PER_ACTOR, INC, SYM: the launch's variant (rollout_variant.h lists the instantiated ones).
+// GUST: the launch contains envs of the gust build (serl_rollout_desc.flags & SERL_ROLLOUT_GUST); an instantiation without
+// it carries no trace of the feature (a gust env in it raises SERL_STATUS_GUST_FLAG)
+// TRACK: the launch writes the tracking-error sums `tk` (serl_rollout_desc.d_track); the sums travel in the hand-over
+// records too
 // PER_ACTOR: every actor flies its own env block (SERL_ROLLOUT_PER_ACTOR_REFS): env `env` of actor `actor` binds row
 // actor * n_envs + env of env_mode / ref_levels / ref_starts, also when a slot resumes it from a hand-over record
-// (instantiated without TRACK, with both GUST values)
-// INC: incremental control (SERL_ROLLOUT_INCREMENTAL; instantiated without GUST and TRACK, and with both for the evaluation
-// suite, SERL_ROLLOUT_SUITE): a 10-entry observation and the env's last_u, both carried in the hand-over records too
-// (OBS_DIM: plant_env.cuh), next to the tracking sums of a TRACK instantiation.
-// SYM: symmetric control (SERL_ROLLOUT_SYMMETRIC; instantiated without GUST and TRACK, and with both for the evaluation
-// suite): a 2-entry observation, one action
+// INC: incremental control (SERL_ROLLOUT_INCREMENTAL): a 10-entry observation and the env's last_u, both carried in the
+// hand-over records too (OBS_DIM: plant_env.cuh), next to the tracking sums of a TRACK instantiation.
+// SYM: symmetric control (SERL_ROLLOUT_SYMMETRIC): a 2-entry observation, one action
 template <int H, bool TABS, bool GUST, bool TRACK = false, bool PER_ACTOR = false, bool INC = false, bool SYM = false>
 __global__ void __launch_bounds__(MAX_CTA_THREADS, 1)
 rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
@@ -639,8 +638,7 @@ rollout_kernel_persist(RolloutArgs ar, TrackArgs tk)
 }
 
 // ---- cross-check kernel: every thread evaluates the whole MLP for its own env (any hidden size that fits) ------
-// PER_ACTOR as in rollout_kernel_persist
-// INC, SYM as in rollout_kernel_persist (instantiated without TRACK, and with it for the evaluation suite)
+// TRACK, PER_ACTOR, INC, SYM as in rollout_kernel_persist; the gust schedule is always compiled in
 template <bool TRACK = false, bool PER_ACTOR = false, bool INC = false, bool SYM = false>
 __global__ void __launch_bounds__(128)
 rollout_kernel_simple(RolloutArgs ar, TrackArgs tk)
@@ -802,17 +800,10 @@ static bool force_simple()
     return v;
 }
 
-// the observation / action widths of the PH-LAB tasks: attitude control 7 -> 3, incremental 10 -> 3, symmetric 2 -> 1
-static bool task_dims(const serl_actor_shape& sh)
-{
-    return ((sh.state_dim == 7 || sh.state_dim == 10) && sh.action_dim == 3) || (sh.state_dim == 2 && sh.action_dim == 1);
-}
-static bool is_symmetric(const serl_actor_shape& sh) { return sh.state_dim == 2 && sh.action_dim == 1; }
-
 // the uniform actors of the PH-LAB tasks the kernels of this file implement
 static bool actor_shape_ok(const serl_actor_shape& sh)
 {
-    return task_dims(sh) && sh.hidden >= 2 && sh.hidden <= 256 && sh.num_layers >= 0 && sh.activation >= 0 && sh.activation <= 2;
+    return task_of_shape(sh) && sh.hidden >= 2 && sh.hidden <= 256 && sh.num_layers >= 0 && sh.activation >= 0 && sh.activation <= 2;
 }
 
 // CTA shape of the persistent kernel: `apc` genome slots x `wps` warps.  A slot's warps fly wps*32 envs of one actor;
@@ -842,8 +833,7 @@ static void choose_shape(int pop, int n_envs, int apc_max, int sms, int* apc_out
 }
 
 template <int H, bool TABS>
-static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust, bool stagger, bool per_actor, bool inc, bool sym,
-                          cudaStream_t s)
+static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool stagger, const RolloutVariant& v, cudaStream_t s)
 {
     const int sms = ar.sm_limit > 0 && ar.sm_limit < serl_device_sms() ? ar.sm_limit : serl_device_sms();
     int apc, wps;
@@ -862,10 +852,9 @@ static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust,
     // scratch: genomes in the shared-memory layout + hand-over records of the time-split schedule (stream-ordered)
     const size_t wt_bytes = (size_t)ar.pop * ar.P4 * 4;
     const long long hn = ar.n_tasks > ar.n_slots ? ar.n_slots * wps * 32 : 0;
-    // a record's observation: 7 floats, 10 floats and last_u (3 f64) with incremental control, 2 floats with symmetric
-    // control (Handoff.obs).  A tracking record (tk.ho) follows the flags, after all of these: an incremental-control
-    // tracking launch carries both
-    const size_t ho_obs = inc ? 10 * 4 + 3 * 8 : sym ? 2 * 4 : 7 * 4;
+    // a record's observation: the task's observation floats, and last_u (3 f64) with incremental control (Handoff.obs).  A
+    // tracking record (tk.ho) follows the flags, after all of these: an incremental-control tracking launch carries both
+    const size_t ho_obs = (size_t)v.task.obs * 4 + (v.task.inc ? 3 * 8 : 0);
     const size_t ho_bytes = (size_t)hn * (NX * 8 + 8 + 8 + ho_obs + 4) + (size_t)(hn / 32) * 4 + (tk.out ? (size_t)hn * TRACK_CARRY * 8 + 8 : 0);
     void* scratch = nullptr;
     cudaError_t e = serl_scratch(SERL_SCRATCH_K1, s, wt_bytes + ho_bytes + 512, &scratch);
@@ -892,16 +881,12 @@ static int launch_persist(RolloutArgs& ar, TrackArgs tk, int apc_max, bool gust,
                                ar.sh.state_dim, H, ar.sh.num_layers);
     if (rc != SERL_OK) return rc;
     const size_t smem = (TABS ? (size_t)PLANT_TABN2 * sizeof(real) : 0) + (size_t)apc * ar.P4 * 4 +
-                        (size_t)apc * wps * (inc ? actor_xbuf_floats(H, 10) : actor_xbuf_floats(H)) * 4;
-    void (*const kernel)(RolloutArgs, TrackArgs) =
-        inc && tk.out ? rollout_kernel_persist<H, TABS, true, true, false, true>          // the suite's tracking launches
-        : sym && tk.out ? rollout_kernel_persist<H, TABS, true, true, false, false, true>
-        : inc       ? (per_actor ? rollout_kernel_persist<H, TABS, false, false, true, true> : rollout_kernel_persist<H, TABS, false, false, false, true>)
-        : sym       ? (per_actor ? rollout_kernel_persist<H, TABS, false, false, true, false, true>
-                                 : rollout_kernel_persist<H, TABS, false, false, false, false, true>)
-        : tk.out    ? rollout_kernel_persist<H, TABS, true, true>
-        : per_actor ? (gust ? rollout_kernel_persist<H, TABS, true, false, true> : rollout_kernel_persist<H, TABS, false, false, true>)
-        : gust      ? rollout_kernel_persist<H, TABS, true> : rollout_kernel_persist<H, TABS, false>;
+                        (size_t)apc * wps * actor_xbuf_floats(H, v.task.obs) * 4;
+    void (*kernel)(RolloutArgs, TrackArgs) = nullptr;
+    visit_rollout_variant(v, [&](auto f) {
+        using V = decltype(f);
+        kernel = rollout_kernel_persist<H, TABS, V::GUST, V::TRACK, V::PER_ACTOR, V::INC, V::SYM>;
+    });
     return serl_launch("rollout_kernel launch", kernel, (unsigned)grid, apc * wps * 32, smem, s, ar, tk);
 }
 
@@ -929,8 +914,7 @@ constexpr size_t K1_TAB_BYTES = (size_t)PLANT_TABN2 * sizeof(real);
 static size_t k1_slot_bytes(const serl_actor_shape& sh)
 {
     const size_t P4 = ((size_t)serl_actor_num_params(&sh) + 3) & ~(size_t)3;
-    const int xb = sh.state_dim == 10 ? actor_xbuf_floats(sh.hidden, 10) : actor_xbuf_floats(sh.hidden);
-    return P4 * 4 + 4ull * xb * 4;        // h = 128, L = 3: 218 KB
+    return P4 * 4 + 4ull * actor_xbuf_floats(sh.hidden, sh.state_dim) * 4;        // h = 128, L = 3: 218 KB
 }
 
 // K1's kernel for a valid shape: the warp actor when it can be launched — the hidden size is instantiated and one slot fits
@@ -954,7 +938,7 @@ extern "C" int32_t serl_actor_tc_widths(const serl_actor_shape* shape, int32_t* 
 {
     if (!shape) return serl_fail(SERL_ERR_ARG, "serl_actor_tc_widths: null shape");
     const serl_actor_shape& sh = *shape;
-    const bool task = task_dims(sh) && sh.hidden >= 2 && sh.num_layers >= 1 && sh.activation >= 0 && sh.activation <= 2;
+    const bool task = task_of_shape(sh) && sh.hidden >= 2 && sh.num_layers >= 1 && sh.activation >= 0 && sh.activation <= 2;
     if (!task || (actor_shape_ok(sh) && k1_fits(sh))) return 0;
     const int n = sh.num_layers + 1;
     if (!widths_out || cap < n) return serl_fail(SERL_ERR_ARG, "serl_actor_tc_widths: widths_out holds fewer than num_layers + 1 widths");
@@ -963,7 +947,7 @@ extern "C" int32_t serl_actor_tc_widths(const serl_actor_shape* shape, int32_t* 
 }
 
 // K1 launch: the checks only this kernel needs, then the genome part of the argument block and the kernel for the hidden size
-static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t s)
+static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, const RolloutVariant& v, cudaStream_t s)
 {
     const TrackArgs tk = {d.d_track, nullptr, d.d_cost};
     if (!actor_shape_ok(d.shape))
@@ -971,20 +955,17 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
     if (d.pop > 65535) return serl_fail(SERL_ERR_ARG, "serl_rollout: pop must be <= 65535 per call");       // grid.y of the simple kernel
     if (d.horizon >= (1 << 30)) return serl_fail(SERL_ERR_ARG, "serl_rollout: horizon too long");        // Handoff.k: steps | done << 30
     const int H = d.shape.hidden;
-    const bool per_actor = (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) != 0, inc = (d.flags & SERL_ROLLOUT_INCREMENTAL) != 0;
-    const bool sym = (d.flags & SERL_ROLLOUT_SYMMETRIC) != 0;
     ar.weights = d.d_weights; ar.P = (int)serl_actor_num_params(&d.shape); ar.sh = d.shape;
     ar.P4 = (ar.P + 3) & ~3;
     if (!k1_warp(d.shape)) {
         if (!k1_fits(d.shape)) return serl_fail(SERL_ERR_UNSUPPORTED, "serl_rollout: genome + activations exceed 227 KB of shared memory");
         const size_t smem = (size_t)ar.P4 * 4 + 2ull * H * 128 * 4;
-        return serl_launch("rollout_kernel launch",
-                           inc && d.d_track ? rollout_kernel_simple<true, false, true>
-                           : sym && d.d_track ? rollout_kernel_simple<true, false, false, true>
-                           : inc       ? (per_actor ? rollout_kernel_simple<false, true, true> : rollout_kernel_simple<false, false, true>)
-                           : sym       ? (per_actor ? rollout_kernel_simple<false, true, false, true> : rollout_kernel_simple<false, false, false, true>)
-                           : d.d_track ? rollout_kernel_simple<true> : per_actor ? rollout_kernel_simple<false, true> : rollout_kernel_simple<false>,
-                           dim3((d.n_envs + 127) / 128, d.pop), 128, smem, s, ar, tk);
+        void (*kernel)(RolloutArgs, TrackArgs) = nullptr;
+        visit_rollout_variant(v, [&](auto f) {
+            using V = decltype(f);
+            kernel = rollout_kernel_simple<V::TRACK, V::PER_ACTOR, V::INC, V::SYM>;
+        });
+        return serl_launch("rollout_kernel launch", kernel, dim3((d.n_envs + 127) / 128, d.pop), 128, smem, s, ar, tk);
     }
     // as many genome slots per CTA as shared memory holds next to the plant tables (L = 3: two for h <= 72, one for h = 96);
     // h = 128 from L = 3 on (207 KB genome) reads the tables through L1 instead (k1_warp: every other shape has room for them)
@@ -993,22 +974,22 @@ static int rollout_impl(const serl_rollout_desc& d, RolloutArgs ar, cudaStream_t
     int apc_max = (int)(((tabs ? K1_SMEM_BUDGET - K1_TAB_BYTES : K1_SMEM_BUDGET)) / slot_bytes);
     if (apc_max > 4) apc_max = 4;
     if (apc_max > 2 && H > 32) apc_max = 2;
-    const bool gust = (d.flags & SERL_ROLLOUT_GUST) != 0, stagger = (d.flags & SERL_ROLLOUT_STAGGER) != 0;
+    const bool stagger = (d.flags & SERL_ROLLOUT_STAGGER) != 0;
     int rc = SERL_OK;
     warp_hidden(H, [&](auto h) {
         constexpr int HH = decltype(h)::value;
         if constexpr (HH == 128)          // the one size instantiated with the tables in global memory too
-            rc = tabs ? launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, per_actor, inc, sym, s)
-                      : launch_persist<HH, false>(ar, tk, apc_max, gust, stagger, per_actor, inc, sym, s);
+            rc = tabs ? launch_persist<HH, true>(ar, tk, apc_max, stagger, v, s) : launch_persist<HH, false>(ar, tk, apc_max, stagger, v, s);
         else
-            rc = launch_persist<HH, true>(ar, tk, apc_max, gust, stagger, per_actor, inc, sym, s);
+            rc = launch_persist<HH, true>(ar, tk, apc_max, stagger, v, s);
     });
     return rc;
 }
 
-int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, cudaStream_t s);     // rollout_tc.cu
+int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, const RolloutVariant& v, cudaStream_t s);     // rollout_tc.cu
 
-// the checks of a launch description that hold for both kernels
+// The checks of a launch description that hold for both kernels.  Besides the launch's own consistency they refuse every
+// combination no kernel is instantiated for, so that visit_rollout_variant finds the variant of each description that passes.
 static int check_desc(const serl_rollout_desc& d)
 {
     if (!d.d_weights || !d.d_ref_levels || !d.d_ref_starts || !d.d_env_mode || !d.d_returns || !d.d_steps)
@@ -1033,18 +1014,18 @@ static int check_desc(const serl_rollout_desc& d)
     // incremental control: a 10-entry observation, on the training instantiations of K1 and K1-TC (and their tracking
     // instantiations in suite launches)
     if (d.flags & SERL_ROLLOUT_INCREMENTAL) {
-        if (d.shape.state_dim != 10) return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) needs state_dim = 10");
+        if (d.shape.state_dim != TASK_INCREMENTAL.obs) return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) needs state_dim = 10");
         if (!suite && (d.d_track || d.d_cost))
             return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) does not take d_track / d_cost");
         if (d.flags & SERL_ROLLOUT_GUST) return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) does not take SERL_ROLLOUT_GUST");
         if (d.d_sensor_noise) return serl_fail(SERL_ERR_ARG, "serl_rollout: incremental control (SERL_ROLLOUT_INCREMENTAL) does not take d_sensor_noise");
-    } else if (d.n_widths == 0 && d.shape.state_dim == 10) {
+    } else if (d.n_widths == 0 && d.shape.state_dim == TASK_INCREMENTAL.obs) {
         return serl_fail(SERL_ERR_ARG, "serl_rollout: state_dim = 10 is the observation of incremental control: it needs SERL_ROLLOUT_INCREMENTAL");
     }
     // symmetric control: a 2-entry observation and one action, on the training instantiations of K1 and K1-TC (and, in suite
     // launches, their tracking instantiations, which carry the gust schedule, and the sensor-noise shim of every instantiation)
     if (d.flags & SERL_ROLLOUT_SYMMETRIC) {
-        if (d.shape.state_dim != 2 || d.shape.action_dim != 1)
+        if (d.shape.state_dim != TASK_SYMMETRIC.obs || d.shape.action_dim != TASK_SYMMETRIC.act)
             return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) needs state_dim = 2 and action_dim = 1");
         if (d.flags & SERL_ROLLOUT_INCREMENTAL)
             return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) does not take SERL_ROLLOUT_INCREMENTAL");
@@ -1056,7 +1037,7 @@ static int check_desc(const serl_rollout_desc& d)
             return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC | SERL_ROLLOUT_SUITE) takes SERL_ROLLOUT_GUST with d_track only");
         if (!suite && d.d_sensor_noise)
             return serl_fail(SERL_ERR_ARG, "serl_rollout: symmetric control (SERL_ROLLOUT_SYMMETRIC) does not take d_sensor_noise");
-    } else if (d.n_widths == 0 && is_symmetric(d.shape)) {
+    } else if (d.n_widths == 0 && task_of_shape(d.shape) == &TASK_SYMMETRIC) {
         return serl_fail(SERL_ERR_ARG, "serl_rollout: state_dim = 2, action_dim = 1 is the actor of symmetric control: it needs SERL_ROLLOUT_SYMMETRIC");
     }
     return SERL_OK;
@@ -1077,8 +1058,8 @@ static RolloutArgs rollout_args(const serl_rollout_desc& d)
     return ar;
 }
 
-// Every population rollout comes through here: the shared checks, the kernel of the actor form (widths: K1-TC, else K1),
-// whose own checks also come before any CUDA call, then the per-actor fitness.
+// Every population rollout comes through here: the shared checks, the task and kernel variant they leave, the kernel of the
+// actor form (widths: K1-TC, else K1), whose own checks also come before any CUDA call, then the per-actor fitness.
 extern "C" int serl_rollout_run(const serl_rollout_desc* desc, void* stream)
 {
     if (!desc) return serl_fail(SERL_ERR_ARG, "serl_rollout_run: null descriptor");
@@ -1086,49 +1067,11 @@ extern "C" int serl_rollout_run(const serl_rollout_desc* desc, void* stream)
     int rc = check_desc(d);
     if (rc != SERL_OK) return rc;
     cudaStream_t s = (cudaStream_t)stream;
-    rc = d.n_widths > 0 ? rollout_tc_impl(d, rollout_args(d), s) : rollout_impl(d, rollout_args(d), s);
+    const RolloutVariant v = rollout_variant(d, task_of_flags(d.flags));
+    rc = d.n_widths > 0 ? rollout_tc_impl(d, rollout_args(d), v, s) : rollout_impl(d, rollout_args(d), v, s);
     if (rc != SERL_OK || !d.d_fitness) return rc;
     return serl_launch("fitness_mean_kernel launch", fitness_mean_kernel, (d.pop + 127) / 128, 128, 0, s, d.d_returns, d.pop, d.n_envs,
                        d.d_fitness);
-}
-
-static serl_rollout_desc make_desc(const float* d_weights, int32_t pop, const serl_actor_shape* shape,
-                                   const double* d_ref_levels, const double* d_ref_starts, const int32_t* d_env_mode,
-                                   int32_t n_envs, int32_t horizon, const float* d_action_noise,
-                                   double* d_returns, int32_t* d_steps, double* d_fitness, double* d_trace, float* d_actions)
-{
-    serl_rollout_desc d;
-    memset(&d, 0, sizeof(d));
-    d.d_weights = d_weights; d.pop = pop; d.shape = *shape;
-    d.d_ref_levels = d_ref_levels; d.d_ref_starts = d_ref_starts; d.d_env_mode = d_env_mode; d.n_envs = n_envs; d.horizon = horizon;
-    d.d_action_noise = d_action_noise; d.d_returns = d_returns; d.d_steps = d_steps; d.d_fitness = d_fitness; d.d_trace = d_trace;
-    d.d_actions = d_actions;
-    return d;
-}
-
-extern "C" int serl_rollout(const float* d_weights, int32_t pop, const serl_actor_shape* shape,
-                            const double* d_ref_levels, const double* d_ref_starts, const int32_t* d_env_mode,
-                            int32_t n_envs, int32_t horizon, const float* d_action_noise,
-                            double* d_returns, int32_t* d_steps, double* d_fitness, double* d_trace, float* d_actions, void* stream)
-{
-    if (!shape) return serl_fail(SERL_ERR_ARG, "serl_rollout: null pointer argument");
-    const serl_rollout_desc d = make_desc(d_weights, pop, shape, d_ref_levels, d_ref_starts, d_env_mode, n_envs, horizon, d_action_noise,
-                                          d_returns, d_steps, d_fitness, d_trace, d_actions);
-    return serl_rollout_run(&d, stream);
-}
-
-extern "C" int serl_rollout_eval(const float* d_weights, int32_t pop, const serl_actor_shape* shape,
-                                 const double* d_ref_levels, const double* d_ref_starts, const int32_t* d_env_mode,
-                                 int32_t n_envs, int32_t horizon, const float* d_action_noise,
-                                 double* d_returns, int32_t* d_steps, double* d_fitness, double* d_trace, float* d_actions,
-                                 double t_max, double smooth_width, void* stream)
-{
-    if (!shape) return serl_fail(SERL_ERR_ARG, "serl_rollout_eval: null pointer argument");
-    if (!(t_max > 0.0) || !(smooth_width > 0.0)) return serl_fail(SERL_ERR_ARG, "serl_rollout_eval: t_max and smooth_width must be > 0");
-    serl_rollout_desc d = make_desc(d_weights, pop, shape, d_ref_levels, d_ref_starts, d_env_mode, n_envs, horizon, d_action_noise,
-                                    d_returns, d_steps, d_fitness, d_trace, d_actions);
-    d.t_max = t_max; d.smooth_width = smooth_width;
-    return serl_rollout_run(&d, stream);
 }
 
 extern "C" int serl_actor_forward(const float* d_genome, const serl_actor_shape* shape, const float* d_obs, int32_t n,
@@ -1138,21 +1081,24 @@ extern "C" int serl_actor_forward(const float* d_genome, const serl_actor_shape*
     if (!actor_shape_ok(*shape)) return serl_fail(SERL_ERR_ARG, "serl_actor_forward: unsupported actor shape");
     cudaStream_t s = (cudaStream_t)stream;
     const int P = (int)serl_actor_num_params(shape), H = shape->hidden;
-    const bool inc = shape->state_dim == 10;        // the observation of incremental control
-    const bool sym = is_symmetric(*shape);
+    const RolloutTask& task = *task_of_shape(*shape);
     const int grid = (n + 127) / 128;
     const size_t smem = (size_t)((P + 3) & ~3) * 4;
     int rc = SERL_OK;
-    const size_t warp_smem = smem + 4ull * (inc ? actor_xbuf_floats(H, 10) : actor_xbuf_floats(H)) * 4;      // genome + 4 warps' buffers
+    const size_t warp_smem = smem + 4ull * actor_xbuf_floats(H, task.obs) * 4;      // genome + 4 warps' buffers
     const auto warp_launch = [&](auto h) {
-        rc = serl_launch("actor_forward_kernel", inc ? actor_forward_kernel<decltype(h)::value, 10>
-                                                 : sym ? actor_forward_kernel<decltype(h)::value, 2, 1> : actor_forward_kernel<decltype(h)::value>,
-                         grid, 128, warp_smem, s, d_genome, P, *shape, d_obs, n, d_actions);
+        visit_task(task, [&](auto S, auto A) {
+            rc = serl_launch("actor_forward_kernel", actor_forward_kernel<decltype(h)::value, decltype(S)::value, decltype(A)::value>,
+                             grid, 128, warp_smem, s, d_genome, P, *shape, d_obs, n, d_actions);
+        });
     };
     // the warp kernel when it holds the genome, else the one-thread-per-env kernel (no static shared memory in either)
     if (!force_simple() && warp_smem <= SERL_SMEM_OPTIN && warp_hidden(H, warp_launch)) return rc;
     const size_t sm2 = smem + 2ull * H * 128 * 4;
     if (sm2 > SERL_SMEM_OPTIN) return serl_fail(SERL_ERR_UNSUPPORTED, "serl_actor_forward: genome + activations exceed shared memory");
-    return serl_launch("actor_forward_kernel", inc ? actor_forward_kernel_simple<10> : sym ? actor_forward_kernel_simple<2, 1> : actor_forward_kernel_simple<>,
-                       grid, 128, sm2, s, d_genome, P, *shape, d_obs, n, d_actions);
+    visit_task(task, [&](auto S, auto A) {
+        rc = serl_launch("actor_forward_kernel", actor_forward_kernel_simple<decltype(S)::value, decltype(A)::value>,
+                         grid, 128, sm2, s, d_genome, P, *shape, d_obs, n, d_actions);
+    });
+    return rc;
 }

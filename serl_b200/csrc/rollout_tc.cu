@@ -27,6 +27,7 @@
 // Numerics: tensor-core accumulation order is not reproducible on a CPU, so this path is checked against the torch fp32
 // oracle with a tolerance (tests/test_wide_actor_gpu.py), not bit for bit like K1.
 #include "plant_env.cuh"
+#include "rollout_variant.h"
 
 #define TC_THREADS 128             // a group: one warpgroup
 #define TC_M 64                    // rows (envs) of one wgmma
@@ -645,14 +646,13 @@ __device__ __forceinline__ void tc_load_small(TcCtx& c, const TcArgs& ar, int ac
     group_sync(c.grp);
 }
 
-// GUST as in rollout_kernel_persist: the launch has envs of the gust build, and reset and step share the one plant_step
-// instance of the kernel; without it a gust env raises SERL_STATUS_GUST_FLAG.  DEEP: more than two widths
-// (tc_actor_forward_deep); the two-width instantiations run tc_actor_forward.  TRACK: the launch writes the tracking-error
-// sums `tk` (serl_rollout_desc.d_track; instantiated with GUST only).  PER_ACTOR: env `env` of actor `actor` binds row
-// actor * n_envs + env of env_mode / ref_levels / ref_starts (SERL_ROLLOUT_PER_ACTOR_REFS; instantiated without TRACK).
-// INC: incremental control (SERL_ROLLOUT_INCREMENTAL; instantiated without GUST and TRACK, and with both for the evaluation
-// suite): a 10-entry observation, layer 0 with 10 inputs, and the env's last_u.  SYM: symmetric control
-// (SERL_ROLLOUT_SYMMETRIC; instantiated without GUST and TRACK, and with both for the evaluation suite): a 2-entry
+// GUST, TRACK, PER_ACTOR, INC, SYM: the launch's variant, as in rollout_kernel_persist (rollout_variant.h lists the
+// instantiated ones).  GUST: the launch has envs of the gust build, and reset and step share the one plant_step instance of
+// the kernel; without it a gust env raises SERL_STATUS_GUST_FLAG.  DEEP: more than two widths (tc_actor_forward_deep); the
+// two-width instantiations run tc_actor_forward.  TRACK: the launch writes the tracking-error sums `tk`
+// (serl_rollout_desc.d_track).  PER_ACTOR: env `env` of actor `actor` binds row actor * n_envs + env of env_mode /
+// ref_levels / ref_starts (SERL_ROLLOUT_PER_ACTOR_REFS).  INC: incremental control (SERL_ROLLOUT_INCREMENTAL): a 10-entry
+// observation, layer 0 with 10 inputs, and the env's last_u.  SYM: symmetric control (SERL_ROLLOUT_SYMMETRIC): a 2-entry
 // observation, layer 0 with 2 inputs, and action 0 of the output block as the elevator
 template <int ACT, bool GUST, bool DEEP, bool TRACK = false, bool PER_ACTOR = false, bool INC = false, bool SYM = false>
 __global__ void __launch_bounds__(2 * TC_THREADS, 1)
@@ -732,11 +732,12 @@ extern "C" int64_t serl_actor_num_params_wide(const int32_t* widths, int32_t n_w
 }
 
 // Checks the widths and sizes the layer table, the kernel layout and the shared memory (all before any CUDA call), then
-// brings the genomes into the kernel layout (K0-TC) in the stream's scratch buffer.
-// S: observation entries (7, 10 with incremental control, 2 with symmetric control); A: actions (3, or 1 with symmetric control)
+// brings the genomes into the kernel layout (K0-TC) in the stream's scratch buffer.  The task sets the widths of layer 0's
+// input and of the output block.
 static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t* widths, int n_widths, cudaStream_t s, size_t* smem_out,
-                      int S = 7, int A = 3)
+                      const RolloutTask& task = TASK_ATTITUDE)
 {
+    const int S = task.obs, A = task.act;
     if (!widths || n_widths < 2 || n_widths > TC_MAXL + 1)
         return serl_fail(SERL_ERR_UNSUPPORTED, "wide actors: the tensor-core path takes 2 to 9 widths [w0, w1, ..., w_{n-1}]");
     if (widths[0] < 8 || widths[0] > 1024) return serl_fail(SERL_ERR_UNSUPPORTED, "wide actors: need 8 <= w0 <= 1024");
@@ -787,84 +788,51 @@ static int tc_prepare(TcArgs& ar, const float* d_weights, int pop, const int32_t
     ar.small = small; ar.tiles = tiles;
     const long long total = (long long)pop * ((long long)ar.small_floats + ar.tile_floats);
     const int grid = (int)((total + 255) / 256 < 8192 ? (total + 255) / 256 : 8192);
-    return serl_launch("tc_layout_kernel", S == 7 ? tc_layout_kernel<7> : S == 2 ? tc_layout_kernel<2, 1> : tc_layout_kernel<10>, grid, 256, 0,
-                       s, d_weights, pop, P, ar, small, tiles);
+    int rc = SERL_OK;
+    visit_task(task, [&](auto S, auto A) {
+        rc = serl_launch("tc_layout_kernel", tc_layout_kernel<decltype(S)::value, decltype(A)::value>, grid, 256, 0, s, d_weights, pop, P, ar,
+                         small, tiles);
+    });
+    return rc;
 }
 
-// K1-TC launch (serl_rollout_run has checked the descriptor and built the env / output arguments `r`)
-int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, cudaStream_t s)
+// calls f(ACT, DEEP) with a K1-TC kernel's activation (SERL_ACT_*) and depth as std::integral_constant
+template <typename F>
+static void tc_form(int activation, bool deep, F&& f)
+{
+    const auto with_act = [&](auto act) {
+        if (deep) f(act, std::true_type());
+        else f(act, std::false_type());
+    };
+    if (activation == SERL_ACT_TANH) with_act(std::integral_constant<int, SERL_ACT_TANH>());
+    else if (activation == SERL_ACT_ELU) with_act(std::integral_constant<int, SERL_ACT_ELU>());
+    else with_act(std::integral_constant<int, SERL_ACT_LEAKY_RELU>());
+}
+
+// K1-TC launch (serl_rollout_run has checked the descriptor, chosen the variant `v` and built the env / output arguments `r`)
+int rollout_tc_impl(const serl_rollout_desc& d, const RolloutArgs& r, const RolloutVariant& v, cudaStream_t s)
 {
     TcArgs ar;
     memset(&ar, 0, sizeof(ar));
     ar.r = r;
     size_t smem = 0;
-    const bool inc = (d.flags & SERL_ROLLOUT_INCREMENTAL) != 0, sym = (d.flags & SERL_ROLLOUT_SYMMETRIC) != 0;
-    const int rc = tc_prepare(ar, d.d_weights, d.pop, d.widths, d.n_widths, s, &smem, inc ? 10 : sym ? 2 : 7, sym ? 1 : 3);
+    const int rc = tc_prepare(ar, d.d_weights, d.pop, d.widths, d.n_widths, s, &smem, v.task);
     if (rc != SERL_OK) return rc;
     ar.n_chunks = (d.n_envs + TC_THREADS - 1) / TC_THREADS;
     ar.n_tasks = (long long)d.pop * ar.n_chunks;
     int sms = serl_device_sms();
     if (d.sm_limit > 0 && d.sm_limit < sms) sms = d.sm_limit;
     const long long grid = (ar.n_tasks + 1) / 2 < sms ? (ar.n_tasks + 1) / 2 : sms;
-    static void (*const kernels[3][2][2])(TcArgs, TrackArgs) = {          // [SERL_ACT_*][gust][deep]
-        {{rollout_kernel_tc<SERL_ACT_TANH, false, false>, rollout_kernel_tc<SERL_ACT_TANH, false, true>},
-         {rollout_kernel_tc<SERL_ACT_TANH, true, false>, rollout_kernel_tc<SERL_ACT_TANH, true, true>}},
-        {{rollout_kernel_tc<SERL_ACT_ELU, false, false>, rollout_kernel_tc<SERL_ACT_ELU, false, true>},
-         {rollout_kernel_tc<SERL_ACT_ELU, true, false>, rollout_kernel_tc<SERL_ACT_ELU, true, true>}},
-        {{rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true>},
-         {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, false>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, true>}}};
-    static void (*const track_kernels[3][2])(TcArgs, TrackArgs) = {                                  // [SERL_ACT_*][deep]
-        {rollout_kernel_tc<SERL_ACT_TANH, true, false, true>, rollout_kernel_tc<SERL_ACT_TANH, true, true, true>},
-        {rollout_kernel_tc<SERL_ACT_ELU, true, false, true>, rollout_kernel_tc<SERL_ACT_ELU, true, true, true>},
-        {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, false, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, true, true>}};
-    static void (*const per_actor_kernels[3][2][2])(TcArgs, TrackArgs) = {   // [SERL_ACT_*][gust][deep]
-        {{rollout_kernel_tc<SERL_ACT_TANH, false, false, false, true>, rollout_kernel_tc<SERL_ACT_TANH, false, true, false, true>},
-         {rollout_kernel_tc<SERL_ACT_TANH, true, false, false, true>, rollout_kernel_tc<SERL_ACT_TANH, true, true, false, true>}},
-        {{rollout_kernel_tc<SERL_ACT_ELU, false, false, false, true>, rollout_kernel_tc<SERL_ACT_ELU, false, true, false, true>},
-         {rollout_kernel_tc<SERL_ACT_ELU, true, false, false, true>, rollout_kernel_tc<SERL_ACT_ELU, true, true, false, true>}},
-        {{rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, true>},
-         {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, false, false, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, true, false, true>}}};
-    static void (*const inc_kernels[3][2][2])(TcArgs, TrackArgs) = {   // [SERL_ACT_*][per actor][deep]
-        {{rollout_kernel_tc<SERL_ACT_TANH, false, false, false, false, true>, rollout_kernel_tc<SERL_ACT_TANH, false, true, false, false, true>},
-         {rollout_kernel_tc<SERL_ACT_TANH, false, false, false, true, true>, rollout_kernel_tc<SERL_ACT_TANH, false, true, false, true, true>}},
-        {{rollout_kernel_tc<SERL_ACT_ELU, false, false, false, false, true>, rollout_kernel_tc<SERL_ACT_ELU, false, true, false, false, true>},
-         {rollout_kernel_tc<SERL_ACT_ELU, false, false, false, true, true>, rollout_kernel_tc<SERL_ACT_ELU, false, true, false, true, true>}},
-        {{rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, false, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, false, true>},
-         {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, true, true>, rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, true, true>}}};
-    static void (*const sym_kernels[3][2][2])(TcArgs, TrackArgs) = {   // [SERL_ACT_*][per actor][deep]
-        {{rollout_kernel_tc<SERL_ACT_TANH, false, false, false, false, false, true>, rollout_kernel_tc<SERL_ACT_TANH, false, true, false, false, false, true>},
-         {rollout_kernel_tc<SERL_ACT_TANH, false, false, false, true, false, true>, rollout_kernel_tc<SERL_ACT_TANH, false, true, false, true, false, true>}},
-        {{rollout_kernel_tc<SERL_ACT_ELU, false, false, false, false, false, true>, rollout_kernel_tc<SERL_ACT_ELU, false, true, false, false, false, true>},
-         {rollout_kernel_tc<SERL_ACT_ELU, false, false, false, true, false, true>, rollout_kernel_tc<SERL_ACT_ELU, false, true, false, true, false, true>}},
-        {{rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, false, false, true>,
-          rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, false, false, true>},
-         {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, false, false, true, false, true>,
-          rollout_kernel_tc<SERL_ACT_LEAKY_RELU, false, true, false, true, false, true>}}};
-    // the evaluation suite's tracking launches of incremental / symmetric control (SERL_ROLLOUT_SUITE)
-    static void (*const inc_track_kernels[3][2])(TcArgs, TrackArgs) = {                              // [SERL_ACT_*][deep]
-        {rollout_kernel_tc<SERL_ACT_TANH, true, false, true, false, true>, rollout_kernel_tc<SERL_ACT_TANH, true, true, true, false, true>},
-        {rollout_kernel_tc<SERL_ACT_ELU, true, false, true, false, true>, rollout_kernel_tc<SERL_ACT_ELU, true, true, true, false, true>},
-        {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, false, true, false, true>,
-         rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, true, true, false, true>}};
-    static void (*const sym_track_kernels[3][2])(TcArgs, TrackArgs) = {                              // [SERL_ACT_*][deep]
-        {rollout_kernel_tc<SERL_ACT_TANH, true, false, true, false, false, true>,
-         rollout_kernel_tc<SERL_ACT_TANH, true, true, true, false, false, true>},
-        {rollout_kernel_tc<SERL_ACT_ELU, true, false, true, false, false, true>,
-         rollout_kernel_tc<SERL_ACT_ELU, true, true, true, false, false, true>},
-        {rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, false, true, false, false, true>,
-         rollout_kernel_tc<SERL_ACT_LEAKY_RELU, true, true, true, false, false, true>}};
+    void (*kernel)(TcArgs, TrackArgs) = nullptr;
+    tc_form(d.shape.activation, ar.n_layers > 1, [&](auto act, auto deep) {
+        visit_rollout_variant(v, [&](auto f) {
+            using V = decltype(f);
+            kernel = rollout_kernel_tc<decltype(act)::value, V::GUST, decltype(deep)::value, V::TRACK, V::PER_ACTOR, V::INC, V::SYM>;
+        });
+    });
     const TrackArgs tk = {d.d_track, nullptr, d.d_cost};
-    const bool gust = (d.flags & SERL_ROLLOUT_GUST) != 0, deep = ar.n_layers > 1;
-    const bool per_actor = (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) != 0;
     // one CTA = the two groups of TC_THREADS threads
-    return serl_launch("rollout_kernel_tc launch", inc && d.d_track ? inc_track_kernels[d.shape.activation][deep]
-                                                   : sym && d.d_track ? sym_track_kernels[d.shape.activation][deep]
-                                                   : inc ? inc_kernels[d.shape.activation][per_actor][deep]
-                                                   : sym ? sym_kernels[d.shape.activation][per_actor][deep]
-                                                   : d.d_track ? track_kernels[d.shape.activation][deep]
-                                                   : (d.flags & SERL_ROLLOUT_PER_ACTOR_REFS) ? per_actor_kernels[d.shape.activation][gust][deep]
-                                                                                             : kernels[d.shape.activation][gust][deep],
-                       (unsigned)grid, 2 * TC_THREADS, smem, s, ar, tk);
+    return serl_launch("rollout_kernel_tc launch", kernel, (unsigned)grid, 2 * TC_THREADS, smem, s, ar, tk);
 }
 
 extern "C" int serl_actor_forward_wide(const float* d_genome, const int32_t* widths, int32_t n_widths, int32_t activation,
@@ -882,9 +850,9 @@ extern "C" int serl_actor_forward_wide(const float* d_genome, const int32_t* wid
     const int blocks = (n + 2 * TC_THREADS - 1) / (2 * TC_THREADS);
     const int sms = serl_device_sms();
     const int grid = blocks < sms ? blocks : sms;
-    static void (*const kernels[3][2])(TcArgs) = {                                                     // [SERL_ACT_*][deep]
-        {actor_forward_tc_kernel<SERL_ACT_TANH, false>, actor_forward_tc_kernel<SERL_ACT_TANH, true>},
-        {actor_forward_tc_kernel<SERL_ACT_ELU, false>, actor_forward_tc_kernel<SERL_ACT_ELU, true>},
-        {actor_forward_tc_kernel<SERL_ACT_LEAKY_RELU, false>, actor_forward_tc_kernel<SERL_ACT_LEAKY_RELU, true>}};
-    return serl_launch("actor_forward_tc_kernel", kernels[activation][ar.n_layers > 1], (unsigned)grid, 2 * TC_THREADS, smem, s, ar);
+    tc_form(activation, ar.n_layers > 1, [&](auto act, auto deep) {
+        rc = serl_launch("actor_forward_tc_kernel", actor_forward_tc_kernel<decltype(act)::value, decltype(deep)::value>, (unsigned)grid,
+                         2 * TC_THREADS, smem, s, ar);
+    });
+    return rc;
 }

@@ -44,12 +44,12 @@ def _matches(decl, ctype, is_param):
     return ctype is _SCALARS[decl.split()[-2] if is_param else decl]
 
 
-def test_binding_declares_every_entry_point_with_the_header_signature():
+def test_binding_declares_the_header_entry_points_with_their_signatures():
     """_native.SIGNATURES (read without loading the library) against every prototype of include/serl_b200.h: the same entry
     points, the same number of arguments and the same C kind for each argument and for the result."""
     from serl_b200 import _native
     protos = declared_prototypes()
-    assert len(protos) == len(declared_symbols()) == 21
+    assert len(protos) == len(declared_symbols()) == 19
     assert sorted(_native.SIGNATURES) == sorted(protos)
     for name, (ret, params) in protos.items():
         restype, argtypes = _native.SIGNATURES[name]
@@ -59,12 +59,12 @@ def test_binding_declares_every_entry_point_with_the_header_signature():
             assert _matches(decl, t, True), (name, decl, t)
 
 
-def test_library_exports_all_declared_symbols():
+def test_library_exports_every_declared_entry_point():
     from serl_b200 import build, _native
     build.build()
     lib = ctypes.CDLL(_native.LIB_PATH)
     syms = declared_symbols()
-    assert 'serl_rollout' in syms
+    assert 'serl_rollout_run' in syms
     for s in syms:
         assert hasattr(lib, s), s
 
@@ -120,7 +120,8 @@ def test_ctypes_mirror_of_the_rollout_descriptor_matches_the_header(tmp_path):
     from serl_b200 import _native, rollout
     fields = [f for f, _ in _native.RolloutDesc._fields_]
     names = sorted(set(re.findall(r'\b(SERL_(?:PLANT|FAULT|ACT|STATUS)_[A-Z0-9_]+)\s*=', header_text())))
-    names += ['SERL_TRACE_COLS', 'SERL_REPLAY_COLS', 'SERL_MODE_GUST', 'SERL_MODE_GUST_UP', 'SERL_ROLLOUT_GUST']
+    flags = sorted(set(re.findall(r'#define\s+(SERL_ROLLOUT_[A-Z_]+)\s', header_text())))
+    names += ['SERL_TRACE_COLS', 'SERL_REPLAY_COLS', 'SERL_MODE_GUST', 'SERL_MODE_GUST_UP'] + flags
     src = tmp_path / 'layout.c'
     src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "serl_b200.h"\nint main(void) {\n'
                    '  printf("%zu %zu\\n", sizeof(serl_rollout_desc), sizeof(serl_actor_shape));\n' +
@@ -144,7 +145,9 @@ def test_ctypes_mirror_of_the_rollout_descriptor_matches_the_header(tmp_path):
          'SERL_ACT_LEAKY_RELU': _native.ACTIVATIONS['relu']}
     assert len(_native.ACTIVATIONS) == 3
     assert (c['SERL_TRACE_COLS'], c['SERL_REPLAY_COLS']) == (_native.TRACE_COLS, _native.REPLAY_COLS)
-    assert (c['SERL_MODE_GUST'], c['SERL_MODE_GUST_UP'], c['SERL_ROLLOUT_GUST']) == (rollout.MODE_GUST, rollout.MODE_GUST_UP, _native.ROLLOUT_GUST)
+    assert (c['SERL_MODE_GUST'], c['SERL_MODE_GUST_UP']) == (rollout.MODE_GUST, rollout.MODE_GUST_UP)
+    assert flags == ['SERL_ROLLOUT_' + f for f in ('GUST', 'INCREMENTAL', 'PER_ACTOR_REFS', 'STAGGER', 'SUITE', 'SYMMETRIC')]
+    assert {f: c[f] for f in flags} == {f: getattr(_native, f[len('SERL_'):]) for f in flags}
     assert {k: v for k, v in c.items() if k.startswith('SERL_STATUS_')} == \
         {'SERL_STATUS_NONFINITE': _native.STATUS_NONFINITE, 'SERL_STATUS_GUST_FLAG': _native.STATUS_GUST_FLAG}
     assert rollout.REPLAY_COST == rollout.TRANSITION_COLS == _native.REPLAY_COLS - 1

@@ -84,7 +84,7 @@ def test_repeat_launches_are_bitwise_deterministic():
     assert np.array_equal(a, b)
 
 
-def test_capi_argument_errors_are_reported():
+def test_rollout_run_argument_errors_are_reported():
     from serl_b200 import _native, rollout
     L = _native.lib()
     sh = rollout.actor_shape(72)
@@ -94,20 +94,26 @@ def test_capi_argument_errors_are_reported():
     md = torch.zeros(1, dtype=torch.int32, device=dev)
     ret = torch.zeros((1, 1), dtype=torch.float64, device=dev)
     stp = torch.zeros((1, 1), dtype=torch.int32, device=dev)
-    p = lambda t: ctypes.c_void_p(t.data_ptr())
-    rc = L.serl_rollout(None, 1, ctypes.byref(sh), p(lv), p(lv), p(md), 1, 10, None, p(ret), p(stp), None, None, None, None)
+
+    def run(weights, pop, shape):
+        d = _native.RolloutDesc()
+        d.d_weights, d.pop, d.shape = weights, pop, shape
+        d.d_ref_levels, d.d_ref_starts, d.d_env_mode, d.n_envs, d.horizon = lv.data_ptr(), lv.data_ptr(), md.data_ptr(), 1, 10
+        d.d_returns, d.d_steps = ret.data_ptr(), stp.data_ptr()
+        return L.serl_rollout_run(ctypes.byref(d), None)
+    rc = run(None, 1, sh)
     assert rc == -1 and b'null pointer' in L.serl_last_error()
-    rc = L.serl_rollout(p(w), 0, ctypes.byref(sh), p(lv), p(lv), p(md), 1, 10, None, p(ret), p(stp), None, None, None, None)
+    rc = run(w.data_ptr(), 0, sh)
     assert rc == -1
     bad = rollout.actor_shape(72); bad.state_dim = 9
-    rc = L.serl_rollout(p(w), 1, ctypes.byref(bad), p(lv), p(lv), p(md), 1, 10, None, p(ret), p(stp), None, None, None, None)
+    rc = run(w.data_ptr(), 1, bad)
     assert rc == -1 and b'state_dim' in L.serl_last_error()
     big = rollout.actor_shape(160)
     wb = torch.zeros((1, rollout.num_params(big)), device=dev)
-    rc = L.serl_rollout(p(wb), 1, ctypes.byref(big), p(lv), p(lv), p(md), 1, 10, None, p(ret), p(stp), None, None, None, None)
+    rc = run(wb.data_ptr(), 1, big)
     assert rc == -3          # SERL_ERR_UNSUPPORTED: a h=160 genome (324 KB) does not fit in shared memory
     with pytest.raises(_native.NativeError):
-        _native.check(rc, 'serl_rollout')
+        _native.check(rc, 'serl_rollout_run')
     assert L.serl_ssne_select(None, 4, None, 0, None, None, None) == -1
 
 

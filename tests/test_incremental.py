@@ -126,7 +126,7 @@ def test_replay_layout_has_one_rule_that_the_header_and_every_buffer_follow(tmp_
 
 
 # ---- launch checks (no CUDA call) --------------------------------------------------------------------------------------------
-def test_the_incremental_flag_is_checked_before_any_cuda_call():
+def test_rollout_run_checks_the_incremental_flag_before_any_cuda_call():
     from serl_b200 import _native, build
     build.build()
     L = _native.lib()
@@ -149,11 +149,7 @@ def test_the_incremental_flag_is_checked_before_any_cuda_call():
     for kw in cases:
         rc, msg = run(**kw)
         assert rc == -1 and 'incremental' in msg.lower(), (kw, rc, msg)
-    # the legacy entry point cannot carry the flag: a 10-input shape is refused there
-    sh = _native.ActorShape(10, 3, 72, 3, 0)
-    fake = [0x10000 + 0x1000 * i for i in range(8)]
-    rc = L.serl_rollout(fake[0], 4, ctypes.byref(sh), fake[1], fake[2], fake[3], 8, 100, None, fake[4], fake[5], None, None, None, None)
-    assert rc == -1 and 'SERL_ROLLOUT_INCREMENTAL' in L.serl_last_error().decode()
+    assert 'SERL_ROLLOUT_INCREMENTAL' in run(flags=0)[1]        # a 10-input shape without the flag is told which flag it needs
 
 
 def test_k1_fit_rule_counts_the_ten_input_genome():

@@ -148,7 +148,7 @@ def test_replay_layout_of_symmetric_control(tmp_path):
 
 
 # ---- launch checks (no CUDA call) --------------------------------------------------------------------------------------------
-def test_the_symmetric_flag_is_checked_before_any_cuda_call():
+def test_rollout_run_checks_the_symmetric_flag_before_any_cuda_call():
     from serl_b200 import _native, build
     build.build()
     L = _native.lib()
@@ -174,14 +174,7 @@ def test_the_symmetric_flag_is_checked_before_any_cuda_call():
     for kw in cases:
         rc, msg = run(**kw)
         assert rc == -1 and ('symmetric' in msg.lower() or (kw.get('flags', 0) & _native.ROLLOUT_INCREMENTAL and 'incremental' in msg.lower())), (kw, rc, msg)
-    # the legacy entry points cannot carry the flag: a 2 -> 1 shape is refused there
-    sh = _native.ActorShape(2, 1, 72, 3, 0)
-    fake = [0x10000 + 0x1000 * i for i in range(8)]
-    rc = L.serl_rollout(fake[0], 4, ctypes.byref(sh), fake[1], fake[2], fake[3], 8, 100, None, fake[4], fake[5], None, None, None, None)
-    assert rc == -1 and 'SERL_ROLLOUT_SYMMETRIC' in L.serl_last_error().decode()
-    rc = L.serl_rollout_eval(fake[0], 4, ctypes.byref(sh), fake[1], fake[2], fake[3], 8, 100, None, fake[4], fake[5], None, None, None,
-                             ctypes.c_double(80.0), ctypes.c_double(11.0), None)
-    assert rc == -1 and 'SERL_ROLLOUT_SYMMETRIC' in L.serl_last_error().decode()
+    assert 'SERL_ROLLOUT_SYMMETRIC' in run(flags=0)[1]          # a 2 -> 1 shape without the flag is told which flag it needs
 
 
 def test_symmetric_actors_k1_cannot_hold_are_routed_to_k1_tc():
